@@ -537,7 +537,7 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
         if (idx->cfg.kind == DFX_FLAT) {
             DFX_REQUIRE(nbytes % (d * 4) == 0, "xb: wrong size");
             idx->n_sorted = nbytes / (d * 4);
-            idx->tc_flat_rows = -1;  // imported rows: any bf16 planes are stale
+            idx->tc_flat_rows = -1;  // imported rows: any fp16 planes are stale
             upload(idx->payload, nbytes);
             if (idx->cfg.metric == DFX_METRIC_L2) {
                 idx->xnorm.reserve((size_t)std::max<int64_t>(idx->n_sorted, 1) * 4);

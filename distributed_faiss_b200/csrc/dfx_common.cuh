@@ -148,6 +148,25 @@ __device__ __forceinline__ float dfx_warp_butterfly(float acc) {
     for (int off = 16; off >= 1; off >>= 1) acc = acc + __shfl_xor_sync(0xffffffffu, acc, off);
     return acc;
 }
+// seq-k dot product q . x: acc = fma(q[k], x[k], acc), k ascending (oracle/dfx_oracle.c).
+// d % 4 == 0 and x 16-byte aligned: float4 row loads, unrolled so that 8 are in flight.
+__device__ __forceinline__ float dfx_dot_seqk(const float* q, const float* x, int d) {
+    float acc = 0.f;
+#pragma unroll 8
+    for (int k = 0; k < d; k += 4) {
+        const float4 xv = *reinterpret_cast<const float4*>(x + k);
+        acc = __fmaf_rn(q[k + 0], xv.x, acc);
+        acc = __fmaf_rn(q[k + 1], xv.y, acc);
+        acc = __fmaf_rn(q[k + 2], xv.z, acc);
+        acc = __fmaf_rn(q[k + 3], xv.w, acc);
+    }
+    return acc;
+}
+// ranking value of column col from its inner product with the query: -ip (IP), or |x|^2 - 2 ip
+// (L2, |q|^2 left out); xnorm is only read for L2
+__device__ __forceinline__ float dfx_rank_value(float ip, int metric, const float* xnorm, int64_t col) {
+    return (metric == DFX_METRIC_IP) ? -ip : __fmaf_rn(-2.f, ip, xnorm[col]);
+}
 
 static inline int64_t dfx_ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 static inline int dfx_next_pow2(int x) {

@@ -56,7 +56,6 @@ struct dfx_index {
     // shows that FAST's wider tolerance would not overflow the kept groups (and back if it does).
     int tc_mode = 0;
     bool tc_fast = false;       // the precision the next screening launch uses (AUTO state)
-    int tc_cent_npl = 0;        // planes currently held by tc_cent (0: none)
     int32_t* tc_stat_h = nullptr;      // pinned [2]: {overflow rows, rows that FAST would overflow} of a past launch
     cudaEvent_t tc_stat_ev = nullptr;
     bool tc_stat_pending = false, tc_stat_fast = false;

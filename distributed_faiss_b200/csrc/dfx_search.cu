@@ -18,20 +18,16 @@
 // =====================================================================================
 // K1a: values GEMM (fp32 FFMA).  acc = fmaf(q[k], x[k], acc), k ascending.
 // =====================================================================================
+// The FFMA tile shared by K1a and K7a: the CTA computes rows m0 .. m0 + BM of Q against columns
+// n0 .. n0 + BN of X; thread (tx, ty) leaves acc[i][j] = q(m0 + ty TM + i) . x(n0 + tx TN + j).
 template <int BM, int BN, int BK, int TM, int TN>
-__global__ void __launch_bounds__((BM / TM) * (BN / TN))
-gemm_values_kernel(const float* __restrict__ Q, int64_t nq, const float* __restrict__ X,
-                   const float* __restrict__ xnorm, int64_t ncols, int d, int metric,
-                   float* __restrict__ out, int64_t ld_out) {
+__device__ __forceinline__ void gemm_tile_ffma(const float* __restrict__ Q, int64_t nq, const float* __restrict__ X,
+                                               int64_t ncols, int d, int64_t m0, int64_t n0, int tx, int ty,
+                                               float (&acc)[TM][TN]) {
     constexpr int THREADS = (BM / TM) * (BN / TN);
     __shared__ float sQ[BK][BM + 4];
     __shared__ float sX[BK][BN + 4];
     const int tid = threadIdx.x;
-    const int tx = tid % (BN / TN), ty = tid / (BN / TN);
-    const int64_t m0 = (int64_t)blockIdx.y * BM;
-    const int64_t n0 = (int64_t)blockIdx.x * BN;
-
-    float acc[TM][TN];
 #pragma unroll
     for (int i = 0; i < TM; i++)
 #pragma unroll
@@ -67,6 +63,19 @@ gemm_values_kernel(const float* __restrict__ Q, int64_t nq, const float* __restr
     }
     // NOTE: zero padding of the k tail adds fmaf(0,0,acc) == acc exactly (acc is never -0 here
     // in a way that matters: acc + (+0) keeps acc), so the canonical order is preserved.
+}
+
+template <int BM, int BN, int BK, int TM, int TN>
+__global__ void __launch_bounds__((BM / TM) * (BN / TN))
+gemm_values_kernel(const float* __restrict__ Q, int64_t nq, const float* __restrict__ X,
+                   const float* __restrict__ xnorm, int64_t ncols, int d, int metric,
+                   float* __restrict__ out, int64_t ld_out) {
+    const int tid = threadIdx.x;
+    const int tx = tid % (BN / TN), ty = tid / (BN / TN);
+    const int64_t m0 = (int64_t)blockIdx.y * BM;
+    const int64_t n0 = (int64_t)blockIdx.x * BN;
+    float acc[TM][TN];
+    gemm_tile_ffma<BM, BN, BK, TM, TN>(Q, nq, X, ncols, d, m0, n0, tx, ty, acc);
 #pragma unroll
     for (int i = 0; i < TM; i++) {
         int64_t gm = m0 + ty * TM + i;
@@ -75,9 +84,7 @@ gemm_values_kernel(const float* __restrict__ Q, int64_t nq, const float* __restr
         for (int j = 0; j < TN; j++) {
             int64_t gn = n0 + tx * TN + j;
             if (gn >= ncols) continue;
-            float ip = acc[i][j];
-            float v = (metric == DFX_METRIC_IP) ? -ip : __fmaf_rn(-2.f, ip, xnorm[gn]);
-            out[gm * ld_out + gn] = v;
+            out[gm * ld_out + gn] = dfx_rank_value(acc[i][j], metric, xnorm, gn);
         }
     }
 }
@@ -151,7 +158,6 @@ struct ResultWriter {  // composites -> faiss-style (D, I)
     int64_t* I;
     int k;
     int metric;
-    float qnorm_add;             // unused (0)
     const float* qnorm;          // FLAT L2: add |q|^2 back and clamp at 0
     __device__ __forceinline__ void operator()(int64_t row, int j, uint64_t c) const {
         if (c == DFX_COMP_NONE) {
@@ -607,7 +613,7 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
         const int64_t N = idx->n_sorted;
         const int metric = idx->cfg.metric;
         if (N == 0) {
-            ResultWriter wr{d_D, d_I, k, metric, 0.f, nullptr};
+            ResultWriter wr{d_D, d_I, k, metric, nullptr};
             CompLoader ldr{nullptr, 0};
             dfx_launch_select<128>(ldr, wr, nq, 0, k, st);
             return;
@@ -630,7 +636,7 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
                     dfx_launch_row_norms(d_x, nq, d, qnorm_tc, st);
                 }
                 CompLoader ldr{idx->tc_cand.as<uint64_t>(), ncand};
-                ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, metric, 0.f, qnorm_tc ? qnorm_tc + q0 : nullptr};
+                ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, metric, qnorm_tc ? qnorm_tc + q0 : nullptr};
                 dfx_launch_select<128>(ldr, wr, qc, ncand, k, st);
             }
             if (handled) return;
@@ -660,7 +666,7 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
                                        ntiles * k, st);
             }
             CompLoader ldr{idx->w_part.as<uint64_t>(), ntiles * k};
-            ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, metric, 0.f, qnorm ? qnorm + q0 : nullptr};
+            ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, metric, qnorm ? qnorm + q0 : nullptr};
             dfx_launch_select<128>(ldr, wr, qc, (int)(ntiles * k), k, st);
         }
         return;
@@ -773,7 +779,7 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
         if (pev) DFX_CUDA(cudaEventRecord(pev->second, st));
         if (!final_written) {
             CompLoader ldr{part, (int64_t)ngroups * k};
-            ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, smetric, 0.f, nullptr};
+            ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, smetric, nullptr};
             dfx_launch_select<128>(ldr, wr, qc, ngroups * k, k, st);
         }
     }
@@ -793,46 +799,12 @@ __global__ void __launch_bounds__((BM / TM) * (BN / TN))
 gemm_argmin_kernel(const float* __restrict__ Q, int64_t nq, const float* __restrict__ X,
                    const float* __restrict__ xnorm, int64_t ncols, int d, int metric,
                    unsigned long long* __restrict__ best) {
-    constexpr int THREADS = (BM / TM) * (BN / TN);
-    __shared__ float sQ[BK][BM + 4];
-    __shared__ float sX[BK][BN + 4];
     const int tid = threadIdx.x;
     const int tx = tid % (BN / TN), ty = tid / (BN / TN);
     const int64_t m0 = (int64_t)blockIdx.y * BM;
     const int64_t n0 = (int64_t)blockIdx.x * BN;
     float acc[TM][TN];
-#pragma unroll
-    for (int i = 0; i < TM; i++)
-#pragma unroll
-        for (int j = 0; j < TN; j++) acc[i][j] = 0.f;
-    for (int k0 = 0; k0 < d; k0 += BK) {
-        for (int e = tid; e < BM * BK; e += THREADS) {
-            int m = e / BK, kk = e % BK;
-            int64_t gm = m0 + m;
-            int gk = k0 + kk;
-            sQ[kk][m] = (gm < nq && gk < d) ? Q[gm * d + gk] : 0.f;
-        }
-        for (int e = tid; e < BN * BK; e += THREADS) {
-            int n = e / BK, kk = e % BK;
-            int64_t gn = n0 + n;
-            int gk = k0 + kk;
-            sX[kk][n] = (gn < ncols && gk < d) ? X[gn * d + gk] : 0.f;
-        }
-        __syncthreads();
-#pragma unroll
-        for (int kk = 0; kk < BK; kk++) {
-            float a[TM], b[TN];
-#pragma unroll
-            for (int i = 0; i < TM; i++) a[i] = sQ[kk][ty * TM + i];
-#pragma unroll
-            for (int j = 0; j < TN; j++) b[j] = sX[kk][tx * TN + j];
-#pragma unroll
-            for (int i = 0; i < TM; i++)
-#pragma unroll
-                for (int j = 0; j < TN; j++) acc[i][j] = __fmaf_rn(a[i], b[j], acc[i][j]);
-        }
-        __syncthreads();
-    }
+    gemm_tile_ffma<BM, BN, BK, TM, TN>(Q, nq, X, ncols, d, m0, n0, tx, ty, acc);
     constexpr int TXN = BN / TN;  // threads sharing a row (consecutive lanes)
 #pragma unroll
     for (int i = 0; i < TM; i++) {
@@ -841,9 +813,7 @@ gemm_argmin_kernel(const float* __restrict__ Q, int64_t nq, const float* __restr
         for (int j = 0; j < TN; j++) {
             int64_t gn = n0 + tx * TN + j;
             if (gn < ncols) {
-                float ip = acc[i][j];
-                float v = (metric == DFX_METRIC_IP) ? -ip : __fmaf_rn(-2.f, ip, xnorm[gn]);
-                unsigned long long cc = dfx_comp(v, (uint32_t)gn);
+                unsigned long long cc = dfx_comp(dfx_rank_value(acc[i][j], metric, xnorm, gn), (uint32_t)gn);
                 c = cc < c ? cc : c;
             }
         }

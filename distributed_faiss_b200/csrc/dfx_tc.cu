@@ -6,11 +6,11 @@
 //
 // Scheme ("screen on tensor cores, decide in canonical fp32"):
 //   1. both operands are scaled by a power of two (queries per row, the table as a whole, so that
-//      every row norm lands in [2^13, 2^14)) and rounded to fp16; q.c ~= (qh.ch) / (sq sc) is
-//      accumulated in fp32 registers by ONE wgmma per k-step.  The rounding error is bounded
-//      rigorously: |q.c - screen| <= |q||c| (2^-10 + 2^-13)  (two 2^-11 relative roundings per
-//      product, fp32 accumulation), see screen_tol.  The decide stage makes the result exact for
-//      ANY bounded error, so the cheap one-MMA screening is the default where it rarely overflows.
+//      every row norm lands in [2^13, 2^14)) and rounded to fp16; q.c is accumulated in fp32
+//      registers by wgmma: PRECISE splits each operand into fp16 hi + lo planes (three MMAs per
+//      k-step), FAST uses the hi planes alone (one MMA).  The rounding error is bounded rigorously
+//      for both, see screen_tol_rel.  The decide stage makes the result exact for ANY bounded
+//      error; AUTO (the default) starts PRECISE and moves to FAST where FAST rarely overflows.
 //   2. the epilogue turns each 128x128 accumulator tile into ranking values
 //      (L2: |c|^2 - 2 q.c, IP: -q.c) and keeps only the MINIMUM of every group of 32
 //      consecutive centroids -> gmin[nq][nlist/32]  (32x less traffic than the full matrix).
@@ -35,7 +35,6 @@
 #include "dfx_ptx.cuh"
 #ifndef DFX_EMU
 #include <cuda.h>
-#include <cuda_bf16.h>
 #endif
 
 #ifndef DFX_EMU  // wgmma / TMA / mbarrier PTX: hardware only (the CPU emulator uses emu_tc_screen below)
@@ -485,20 +484,33 @@ __device__ __forceinline__ bool screen_overflow(const int32_t* __restrict__ grou
     const int gl = groups[row * G + G - 1];
     return gl >= 0 && gmin[row * ng + gl] <= thr;
 }
-// ovf = [overflow rows, rows that the FAST tolerance would overflow (counted by PRECISE launches
-// for the AUTO mode), row list ...].  t = the nprobe-th smallest group minimum (inf: no pruning).
+// The decide threshold of a row, t + tol with t = the nprobe-th smallest group minimum (inf when
+// there are fewer groups than probes: nothing is pruned).  A row with more near-ties than
+// selected groups is queued for tc_exact_rows_kernel.  ovf = [overflow rows, rows that the FAST
+// tolerance would overflow (counted by PRECISE launches for the AUTO mode), row list ...].
 struct ScreenTol {
     float rel;       // of this launch's precision
     float rel_fast;  // > 0: also count the rows FAST would overflow
 };
-__device__ __forceinline__ float screen_threshold(const int32_t* __restrict__ groups, int64_t row, int G, int ng,
-                                                  const float* __restrict__ gmin, float t, float qn2, float cmax2,
+__device__ __forceinline__ float screen_threshold(const int32_t* __restrict__ groups, int64_t row, int G, int nprobe,
+                                                  int ng, const float* __restrict__ gmin, float qn2, float cmax2,
                                                   ScreenTol tol, int32_t* __restrict__ ovf) {
+    const int gk = (nprobe <= G) ? groups[row * G + nprobe - 1] : -1;
+    const float t = gk >= 0 ? gmin[row * ng + gk] : __int_as_float(0x7f800000);
     const float thr = t + screen_tol(qn2, cmax2, tol.rel);
     if (screen_overflow(groups, row, G, ng, gmin, thr)) ovf[2 + atomicAdd(&ovf[0], 1)] = (int32_t)row;
     if (tol.rel_fast > 0.f && screen_overflow(groups, row, G, ng, gmin, t + screen_tol(qn2, cmax2, tol.rel_fast)))
         atomicAdd(&ovf[1], 1);
     return thr;
+}
+// Can a selected group (o = row * ng + group) still matter?  Only if its minimum is within the
+// threshold (the return value); then through all 32 columns if its runner-up is within it too
+// (expand, which means nothing for a group that is not live), otherwise through its arg-min
+// column alone.  Neither load waits for the other's compare.
+__device__ __forceinline__ bool group_live(const float* __restrict__ gmin, const float* __restrict__ gmin2,
+                                           int64_t o, float thr, bool& expand) {
+    expand = gmin2[o] <= thr;
+    return gmin[o] <= thr;
 }
 
 // The G (<= 32) smallest group minima of a row, ascending by (value, group): one warp per row.
@@ -513,28 +525,6 @@ __device__ __forceinline__ float screen_threshold(const int32_t* __restrict__ gr
 // on the n / 4 tile minima, then the 4 G groups of the G smallest tiles are sorted and the first
 // G kept.  The G smallest groups always lie in the G smallest tiles: a group g outside them
 // would have G tiles, each holding a group with (minimum, index) below g's, before it.
-template <int CAP>
-__device__ __forceinline__ void warp_sort_buf(uint64_t* buf, int cnt, int lane, int& P) {
-    P = 32;
-    while (P < cnt) P <<= 1;
-    for (int e = cnt + lane; e < P; e += 32) buf[e] = DFX_COMP_NONE;
-    __syncwarp();
-    for (int size = 2; size <= P; size <<= 1) {
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            for (int i = lane; i < (P >> 1); i += 32) {
-                const int pos = 2 * i - (i & (stride - 1));
-                const int partner = pos + stride;
-                const bool up = ((pos & size) == 0);
-                const uint64_t a = buf[pos], bb = buf[partner];
-                if ((a > bb) == up) {
-                    buf[pos] = bb;
-                    buf[partner] = a;
-                }
-            }
-            __syncwarp();
-        }
-    }
-}
 template <int CAP>
 __global__ void __launch_bounds__(256)
 topg_collect_kernel(const float* __restrict__ coarse, int64_t nq, int n, int G, const float* __restrict__ fine,
@@ -575,19 +565,7 @@ topg_collect_kernel(const float* __restrict__ coarse, int64_t nq, int n, int G, 
             lmin = c < lmin ? c : lmin;
         }
     }
-    // bitonic sort of the 32 lane minima across the warp (ascending by lane)
-    uint64_t x = lmin;
-#pragma unroll
-    for (int size = 2; size <= 32; size <<= 1) {
-#pragma unroll
-        for (int stride = size >> 1; stride > 0; stride >>= 1) {
-            const uint64_t y = __shfl_xor_sync(0xffffffffu, x, stride);
-            const bool up = ((lane & size) == 0);
-            const bool lower = ((lane & stride) == 0);
-            const bool take_min = (lower == up);
-            x = take_min ? (x < y ? x : y) : (x < y ? y : x);
-        }
-    }
+    const uint64_t x = dfx_warp_sort32_asc(lmin, lane);  // the 32 lane minima, ascending by lane
     const int gth = min(G, 32) - 1;
     const uint64_t bound = __shfl_sync(0xffffffffu, x, gth);  // G-th smallest lane minimum
     // 2. collect everything <= bound
@@ -614,7 +592,7 @@ topg_collect_kernel(const float* __restrict__ coarse, int64_t nq, int n, int G, 
     }
     int P = 32;
     if (!overflow) {
-        warp_sort_buf<CAP>(buf, cnt, lane, P);  // 3. sort the candidates
+        P = dfx_warp_sort_buf(buf, cnt, lane);  // 3. sort the candidates
     } else {
         // fallback: G rounds of "smallest composite above the previous pick", left in buf[0..G)
         uint64_t prev = 0;
@@ -646,7 +624,7 @@ topg_collect_kernel(const float* __restrict__ coarse, int64_t nq, int n, int G, 
                 (tc_ != DFX_COMP_NONE && gi < n_fine) ? dfx_comp(f[gi], (uint32_t)gi) : DFX_COMP_NONE;
         }
         __syncwarp();
-        warp_sort_buf<CAP>(buf, 32 * FINE_PER, lane, P);
+        P = dfx_warp_sort_buf(buf, 32 * FINE_PER, lane);
         overflow = false;
     }
     for (int r = lane; r < G; r += 32) {
@@ -685,11 +663,7 @@ rerank_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent
         if (threadIdx.x == 0) {
             float qn2 = 0.f;
             for (int i = 0; i < d; i++) qn2 += s_q[i] * s_q[i];
-            // the bound needs nprobe distinct groups: with fewer groups than probes nothing is pruned
-            const int gk = (nprobe <= G) ? groups[row * G + nprobe - 1] : -1;
-            // (more near-ties than selected groups: the row is also queued for tc_exact_rows_kernel)
-            s_thr = screen_threshold(groups, row, G, ng, gmin,
-                                     gk >= 0 ? gmin[row * ng + gk] : __int_as_float(0x7f800000), qn2, cmax2, tol, ovf);
+            s_thr = screen_threshold(groups, row, G, nprobe, ng, gmin, qn2, cmax2, tol, ovf);
         }
         __syncthreads();
         const float thr = s_thr;
@@ -699,23 +673,12 @@ rerank_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent
             unsigned long long comp = DFX_COMP_NONE;
             if (gid >= 0) {
                 const int64_t o = row * ng + gid;
-                const bool expand = gmin2[o] <= thr;
-                const bool live = gmin[o] <= thr && (expand || (c & 31) == (int)gargc[o]);
+                bool expand;
+                const bool live = group_live(gmin, gmin2, o, thr, expand) && (expand || (c & 31) == (int)gargc[o]);
                 const int64_t col = (int64_t)gid * 32 + (c & 31);
-                if (live && col < nlist) {
-                    const float* x = cent + col * d;
-                    float acc = 0.f;
-#pragma unroll 8
-                    for (int k = 0; k < d; k += 4) {  // (unrolled: 8 row loads in flight, same FMA chain)
-                        const float4 xv = *reinterpret_cast<const float4*>(x + k);
-                        acc = __fmaf_rn(s_q[k + 0], xv.x, acc);
-                        acc = __fmaf_rn(s_q[k + 1], xv.y, acc);
-                        acc = __fmaf_rn(s_q[k + 2], xv.z, acc);
-                        acc = __fmaf_rn(s_q[k + 3], xv.w, acc);
-                    }
-                    const float v = (metric == DFX_METRIC_IP) ? -acc : __fmaf_rn(-2.f, acc, cnorm[col]);
-                    comp = dfx_comp(v, (uint32_t)col);
-                }
+                if (live && col < nlist)
+                    comp = dfx_comp(dfx_rank_value(dfx_dot_seqk(s_q, cent + col * d, d), metric, cnorm, col),
+                                    (uint32_t)col);
             }
             if (MODE == 1) best = comp < best ? comp : best;
             else if (MODE == 0) out[row * ncand + c] = comp;
@@ -782,11 +745,8 @@ rerank2_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cen
     }
     const float qn2 = dfx_warp_butterfly(part);
     __syncwarp();
-    const int gk = (nprobe <= G) ? groups[row * G + nprobe - 1] : -1;
     float thr = 0.f;
-    if (lane == 0)
-        thr = screen_threshold(groups, row, G, ng, gmin, gk >= 0 ? gmin[row * ng + gk] : __int_as_float(0x7f800000),
-                               qn2, cmax2, tol, ovf);
+    if (lane == 0) thr = screen_threshold(groups, row, G, nprobe, ng, gmin, qn2, cmax2, tol, ovf);
     thr = __shfl_sync(0xffffffffu, thr, 0);
     // ---- candidate list: one entry for a live group's arg-min column, 32 for an expanded group
     int cnt = 0;
@@ -799,8 +759,8 @@ rerank2_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cen
             gid = groups[row * G + gi];
             if (gid >= 0) {
                 const int64_t o = row * ng + gid;
-                live = gmin[o] <= thr;
-                expand = live && gmin2[o] <= thr;
+                live = group_live(gmin, gmin2, o, thr, expand);
+                expand = live && expand;
                 argc = (int)gargc[o];
             }
         }
@@ -827,18 +787,7 @@ rerank2_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cen
         uint64_t comp = DFX_COMP_NONE;
         if (c0 + lane < cnt) {
             const int64_t col = s_cand[c0 + lane];
-            const float* x = cent + col * d;
-            float acc = 0.f;
-#pragma unroll 8
-            for (int k = 0; k < d; k += 4) {  // (unrolled: 8 row loads in flight, same FMA chain)
-                const float4 xv = *reinterpret_cast<const float4*>(x + k);
-                acc = __fmaf_rn(s_q[k + 0], xv.x, acc);
-                acc = __fmaf_rn(s_q[k + 1], xv.y, acc);
-                acc = __fmaf_rn(s_q[k + 2], xv.z, acc);
-                acc = __fmaf_rn(s_q[k + 3], xv.w, acc);
-            }
-            const float v = (metric == DFX_METRIC_IP) ? -acc : __fmaf_rn(-2.f, acc, cnorm[col]);
-            comp = dfx_comp(v, (uint32_t)col);
+            comp = dfx_comp(dfx_rank_value(dfx_dot_seqk(s_q, cent + col * d, d), metric, cnorm, col), (uint32_t)col);
         }
         kept = dfx_warp_merge_sorted32(kept, dfx_warp_sort32_asc(comp, lane), lane);
     }
@@ -881,18 +830,7 @@ struct ExactLoader {
     const float* xnorm;
     int d, metric;   // d % 4 == 0 (the tensor-core path requires d % 64 == 0)
     __device__ __forceinline__ uint64_t operator()(int64_t /*row*/, int e) const {
-        const float* x = X + (int64_t)e * d;
-        float acc = 0.f;
-#pragma unroll 8
-        for (int k = 0; k < d; k += 4) {  // 8 row loads in flight, the canonical seq-k FMA chain
-            const float4 xv = *reinterpret_cast<const float4*>(x + k);
-            acc = __fmaf_rn(q[k + 0], xv.x, acc);
-            acc = __fmaf_rn(q[k + 1], xv.y, acc);
-            acc = __fmaf_rn(q[k + 2], xv.z, acc);
-            acc = __fmaf_rn(q[k + 3], xv.w, acc);
-        }
-        const float v = (metric == DFX_METRIC_IP) ? -acc : __fmaf_rn(-2.f, acc, xnorm[e]);
-        return dfx_comp(v, (uint32_t)e);
+        return dfx_comp(dfx_rank_value(dfx_dot_seqk(q, X + (int64_t)e * d, d), metric, xnorm, e), (uint32_t)e);
     }
 };
 struct ExactWriter {  // mode 2: keys[row][K]; mode 1: assign[row]; mode 0: out[row][K] composites
@@ -1005,19 +943,22 @@ static float tc_prepare_table(const float* x, int64_t n, int d, float cmax2, int
     return scale;
 }
 
-// (re)build the fp16 copy of the centroids (both planes: either precision can use it); call after
-// training / import
-void dfx_tc_prepare_centroids(dfx_index* idx, cudaStream_t st) {
-    const int d = idx->cfg.d;
-    if (!dfx_tc_supported(d)) return;
-    const int64_t nlist = idx->cfg.nlist;
-    idx->tc_cmax2 = max_norm2(idx, idx->cnorm.as<float>(), nlist, st);
-    idx->tc_cscale = tc_prepare_table(idx->centroids.as<float>(), nlist, d, idx->tc_cmax2, 2, idx->tc_cent, st);
-    idx->tc_cent_npl = 2;
-    idx->tc_ready = true;
-    if (idx->tc_mode == 0) idx->tc_fast = false;  // AUTO: a new table starts PRECISE
+// install the index's screening table (its centroids, or the rows of a FLAT index): the norm
+// bound, the fp16 copy with both planes (either precision can use it) and its scale; AUTO starts
+// PRECISE on a new table
+static void tc_install_table(dfx_index* idx, const float* x, const float* norms, int64_t n, cudaStream_t st) {
+    idx->tc_cmax2 = max_norm2(idx, norms, n, st);
+    idx->tc_cscale = tc_prepare_table(x, n, idx->cfg.d, idx->tc_cmax2, 2, idx->tc_cent, st);
+    if (idx->tc_mode == 0) idx->tc_fast = false;
     idx->tc_stat_pending = false;
     idx->tc_acc_rows = idx->tc_acc_bad = 0;
+}
+
+// (re)build the screening table of the centroids; call after training / import
+void dfx_tc_prepare_centroids(dfx_index* idx, cudaStream_t st) {
+    if (!dfx_tc_supported(idx->cfg.d)) return;
+    tc_install_table(idx, idx->centroids.as<float>(), idx->cnorm.as<float>(), idx->cfg.nlist, st);
+    idx->tc_ready = true;
 }
 
 // ---- AUTO precision: statistics of a past launch come back through pinned memory, no sync
@@ -1034,23 +975,29 @@ static bool tc_stream_capturing(cudaStream_t st) {
 // overflows practically never happen: PRECISE -> FAST after at least 16 384 observed rows none of
 // which would have overflowed under FAST's tolerance; FAST -> PRECISE as soon as more than one row
 // in 16 384 did overflow.  Counts accumulate across launches (a batch of one query says nothing
-// on its own).  Either way the results are exact; only the cost moves.  A switch bumps
-// `generation` (captured graphs are stale).
+// on its own).  Either way the results are exact; only the cost moves.
+// Folds the counts of one launch of precision `fast` into (acc_rows, acc_bad) and returns the
+// precision of the next launch; a decision starts a new window.
+static bool tc_auto_step(bool fast, int64_t rows, int64_t overflowed, int64_t fast_would, int64_t window,
+                         int64_t& acc_rows, int64_t& acc_bad) {
+    acc_rows += rows;
+    acc_bad += fast ? overflowed : fast_would;
+    if (!fast && acc_rows >= window) {
+        fast = acc_bad == 0;
+        acc_rows = acc_bad = 0;
+    } else if (fast && acc_bad > 0 && acc_bad * window > acc_rows) {
+        fast = false;
+        acc_rows = acc_bad = 0;
+    }
+    return fast;
+}
+// The search-path AUTO state of an index.  A switch bumps `generation` (captured graphs are stale).
 static void tc_auto_update(dfx_index* idx, bool was_fast, int64_t rows, int64_t overflowed, int64_t fast_would) {
     if (idx->tc_mode != 0 || rows <= 0 || was_fast != idx->tc_fast) return;
-    idx->tc_acc_rows += rows;
-    idx->tc_acc_bad += was_fast ? overflowed : fast_would;
-    bool fast = idx->tc_fast;
-    const int64_t window = idx->tc_auto_window;  // 16 384 rows unless dfx_set_param("tc_auto_window") says otherwise
-    if (!fast && idx->tc_acc_rows >= window) {
-        fast = idx->tc_acc_bad == 0;
-        idx->tc_acc_rows = idx->tc_acc_bad = 0;
-    } else if (fast && idx->tc_acc_bad > 0 && idx->tc_acc_bad * window > idx->tc_acc_rows) {
-        fast = false;
-        idx->tc_acc_rows = idx->tc_acc_bad = 0;
-    } else if (fast && idx->tc_acc_rows >= (1 << 20)) {
-        idx->tc_acc_rows = idx->tc_acc_bad = 0;  // a fresh window
-    }
+    // window: 16 384 rows unless dfx_set_param("tc_auto_window") says otherwise
+    const bool fast = tc_auto_step(was_fast, rows, overflowed, fast_would, idx->tc_auto_window, idx->tc_acc_rows,
+                                   idx->tc_acc_bad);
+    if (fast && idx->tc_acc_rows >= (1 << 20)) idx->tc_acc_rows = idx->tc_acc_bad = 0;  // a fresh window
     if (fast != idx->tc_fast) {
         idx->tc_fast = fast;
         idx->generation++;
@@ -1093,7 +1040,7 @@ static ScreenTol tc_tol(const dfx_index* idx, int d, bool fast) {
 }
 
 // screening pass: gmin[nq][ng] for a batch of rows against a table prepared by tc_prepare_table
-// (npl planes used; the table must hold at least npl); also leaves |q|^2 in idx->tc_qn
+// (npl planes used; the table must hold at least npl)
 static void tc_screen(dfx_index* idx, int d, const float* d_x, int64_t nq, const void* table_h, float table_scale,
                       int npl, const float* cnorm, int64_t nlist, int metric, float* gmin, float* gmin2,
                       uint8_t* gargc, float* tmin, cudaStream_t st) {
@@ -1186,11 +1133,34 @@ static void tc_select_groups(const float* gmin, const float* tmin, int64_t nrows
     }
 }
 
-// the overflow record of a decide launch: [overflow rows, FAST-would-overflow rows, row list ...]
-static int32_t* tc_ovf_reset(dfx_index* idx, int64_t nrows, cudaStream_t st) {
-    idx->tc_ovf.reserve((size_t)(nrows + 2) * 4);
+// what the decide stage reads: the screening summary [rows][ng], the G selected groups per row,
+// and the overflow record [overflow rows, FAST-would-overflow rows, row list ...], zeroed
+struct Screened {
+    const float* gmin;
+    const float* gmin2;
+    const uint8_t* gargc;
+    const int32_t* groups;
+    int32_t* ovf;
+};
+// screen a chunk of `rows` rows against a table (as tc_screen) and select their G groups; the
+// workspace is sized for chunks of up to rmax rows
+static Screened tc_screen_chunk(dfx_index* idx, int d, const float* d_x, int64_t rows, int64_t rmax, int ng, int G,
+                                const void* table_h, float table_scale, int npl, const float* cnorm, int64_t nlist,
+                                int metric, cudaStream_t st) {
+    idx->tc_gmin.reserve((size_t)rmax * ng * 4);
+    idx->tc_gmin2.reserve((size_t)rmax * ng * 4);
+    idx->tc_gargc.reserve((size_t)rmax * ng);
+    idx->tc_groups.reserve((size_t)rmax * G * 4);
+    idx->tc_tmin.reserve((size_t)rmax * (ng / 4 + 1) * 4);
+    float* gmin = idx->tc_gmin.as<float>();
+    float* tmin = idx->tc_tmin.as<float>();
+    tc_screen(idx, d, d_x, rows, table_h, table_scale, npl, cnorm, nlist, metric, gmin, idx->tc_gmin2.as<float>(),
+              idx->tc_gargc.as<uint8_t>(), tmin, st);
+    tc_select_groups(gmin, tmin, rows, ng, G, idx->tc_groups.as<int32_t>(), st);
+    idx->tc_ovf.reserve((size_t)(rows + 2) * 4);
     DFX_CUDA(cudaMemsetAsync(idx->tc_ovf.p, 0, 8, st));
-    return idx->tc_ovf.as<int32_t>();
+    return {gmin, idx->tc_gmin2.as<float>(), idx->tc_gargc.as<uint8_t>(), idx->tc_groups.as<int32_t>(),
+            idx->tc_ovf.as<int32_t>()};
 }
 
 // top-nprobe lists per query -> keys int32 [nq, nprobe] (exactly the oracle's coarse result)
@@ -1206,18 +1176,8 @@ void dfx_tc_coarse_search(dfx_index* idx, const float* d_x, int64_t nq, int npro
     if (G > ng || ng <= 64) G = ng;
     const int64_t QC = std::max<int64_t>(tc::TILE, ((64ll << 20) / ((int64_t)ng * 4)) / tc::TILE * tc::TILE);
     const int64_t qmax = std::min<int64_t>(nq, QC);
-    idx->tc_gmin.reserve((size_t)qmax * ng * 4);
-    idx->tc_gmin2.reserve((size_t)qmax * ng * 4);
-    idx->tc_gargc.reserve((size_t)qmax * ng);
-    idx->tc_groups.reserve((size_t)qmax * G * 4);
-    idx->tc_tmin.reserve((size_t)qmax * (ng / 4 + 1) * 4);
-    float* tmin = idx->tc_tmin.as<float>();
     const float* cent = idx->centroids.as<float>();
     const float* cnorm = idx->cnorm.as<float>();
-    float* gmin = idx->tc_gmin.as<float>();
-    float* gmin2 = idx->tc_gmin2.as<float>();
-    uint8_t* gargc = idx->tc_gargc.as<uint8_t>();
-    int32_t* groups = idx->tc_groups.as<int32_t>();
     tc_stats_poll(idx, st);
     const bool fast = idx->tc_fast;
     const ScreenTol tol = tc_tol(idx, d, fast);
@@ -1225,34 +1185,34 @@ void dfx_tc_coarse_search(dfx_index* idx, const float* d_x, int64_t nq, int npro
         const int64_t qc = std::min(QC, nq - q0);
         const float* xq = d_x + q0 * d;
         int32_t* kq = keys + q0 * nprobe;
-        tc_screen(idx, d, xq, qc, idx->tc_cent.p, idx->tc_cscale, fast ? 1 : 2, cnorm, nlist, metric, gmin, gmin2,
-                  gargc, tmin, st);
-        tc_select_groups(gmin, tmin, qc, ng, G, groups, st);
-        int32_t* ovf = tc_ovf_reset(idx, qc, st);
+        const Screened s = tc_screen_chunk(idx, d, xq, qc, qmax, ng, G, idx->tc_cent.p, idx->tc_cscale, fast ? 1 : 2,
+                                           cnorm, nlist, metric, st);
         const int P_cand = dfx_next_pow2(G * 32 < 32 ? 32 : G * 32);
         if (nprobe <= 32 && G <= 64 && d % 4 == 0) {  // warp per query
             const size_t smem = (size_t)RR2_WARPS * ((d + 3) / 4 * 4) * 4 + (size_t)RR2_WARPS * G * 32 * 4;
             if (smem > 48 * 1024)
                 DFX_CUDA(cudaFuncSetAttribute(rerank2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             DFX_LAUNCH(rerank2_kernel, (unsigned)dfx_ceil_div(qc, RR2_WARPS), RR2_WARPS * 32, smem, st, xq, d, cent,
-                       cnorm, nlist, metric, groups, G, nprobe, gmin, gmin2, gargc, ng, idx->tc_cmax2, tol, qc, kq, ovf);
+                       cnorm, nlist, metric, s.groups, G, nprobe, s.gmin, s.gmin2, s.gargc, ng, idx->tc_cmax2, tol, qc,
+                       kq, s.ovf);
         } else if (P_cand <= 4096) {  // fused: candidates never leave the SM
             auto kern = rerank_kernel<2>;
             const size_t smem = ((size_t)d * 4 + 15) / 16 * 16 + (size_t)P_cand * 8;
-            DFX_LAUNCH(kern, (unsigned)qc, 128, smem, st, xq, d, cent, cnorm, nlist, metric, groups, G, nprobe, gmin,
-                       gmin2, gargc, ng, idx->tc_cmax2, tol, (uint64_t*)nullptr, (int32_t*)nullptr,
-                       (const int32_t*)nullptr, (const int32_t*)nullptr, qc, kq, ovf);
+            DFX_LAUNCH(kern, (unsigned)qc, 128, smem, st, xq, d, cent, cnorm, nlist, metric, s.groups, G, nprobe,
+                       s.gmin, s.gmin2, s.gargc, ng, idx->tc_cmax2, tol, (uint64_t*)nullptr, (int32_t*)nullptr,
+                       (const int32_t*)nullptr, (const int32_t*)nullptr, qc, kq, s.ovf);
         } else {
             idx->tc_cand.reserve((size_t)qmax * G * 32 * 8);
             auto kern = rerank_kernel<0>;
-            DFX_LAUNCH(kern, (unsigned)qc, 128, (size_t)d * 4, st, xq, d, cent, cnorm, nlist, metric, groups, G,
-                       nprobe, gmin, gmin2, gargc, ng, idx->tc_cmax2, tol, idx->tc_cand.as<uint64_t>(),
-                       (int32_t*)nullptr, (const int32_t*)nullptr, (const int32_t*)nullptr, qc, (int32_t*)nullptr, ovf);
+            DFX_LAUNCH(kern, (unsigned)qc, 128, (size_t)d * 4, st, xq, d, cent, cnorm, nlist, metric, s.groups, G,
+                       nprobe, s.gmin, s.gmin2, s.gargc, ng, idx->tc_cmax2, tol, idx->tc_cand.as<uint64_t>(),
+                       (int32_t*)nullptr, (const int32_t*)nullptr, (const int32_t*)nullptr, qc, (int32_t*)nullptr,
+                       s.ovf);
             dfx_launch_select_comp(idx->tc_cand.as<uint64_t>(), qc, G * 32, (int64_t)G * 32, nprobe, kq, st);
         }
         // rows with more near-ties than selected groups (screen_overflow): exact, over all lists
-        launch_exact_rows(xq, cent, cnorm, nlist, d, metric, ovf, qc, 2, nprobe, kq, nullptr, nullptr, st);
-        if (q0 + QC >= nq) tc_stats_post(idx, ovf, qc, fast, st);
+        launch_exact_rows(xq, cent, cnorm, nlist, d, metric, s.ovf, qc, 2, nprobe, kq, nullptr, nullptr, st);
+        if (q0 + QC >= nq) tc_stats_post(idx, s.ovf, qc, fast, st);
     }
 }
 
@@ -1260,7 +1220,7 @@ void dfx_tc_coarse_search(dfx_index* idx, const float* d_x, int64_t nq, int npro
 // "flat_tensor_cores" = 0 selects the FFMA GEMM; the results are bit-identical): flat search (reference
 // index.py:94 IndexFlatIP, and IndexFlatL2 of the C-ABI) through the same machinery, with the
 // database rows in place of the centroids and k in place of nprobe.  Screening on tensor cores
-// over bf16 planes of the rows (built lazily, rebuilt after an add), the k + 8 groups with the
+// over fp16 planes of the rows (built lazily, rebuilt after an add), the k + 8 groups with the
 // smallest minima, exact canonical values of the columns the screening cannot rule out
 // (rerank_kernel<0>) -- the values gemm_values_kernel would have produced for them, bit for bit.
 // Leaves nq x ncand composites in idx->tc_cand; the caller selects and writes (D, I).
@@ -1272,20 +1232,15 @@ int dfx_tc_flat_candidates(dfx_index* idx, const float* d_x, int64_t nq, int k, 
     const int metric = idx->cfg.metric;
     const int64_t nl_pad = dfx_ceil_div(N, tc::TILE) * tc::TILE;
     const int ng = (int)(nl_pad / 32);
-    if (idx->tc_flat_rows != N) {  // (re)build the fp16 copy of the rows and the norm bound
+    if (idx->tc_flat_rows != N) {  // (re)build the screening table of the rows
         const float* norms = idx->xnorm.as<float>();
         if (metric != DFX_METRIC_L2) {  // inner product keeps no row norms: the tolerance needs their maximum
             idx->cnorm.reserve((size_t)N * 4);
             dfx_launch_row_norms(idx->payload.as<float>(), N, d, idx->cnorm.as<float>(), st);
             norms = idx->cnorm.as<float>();
         }
-        idx->tc_cmax2 = max_norm2(idx, norms, N, st);
-        idx->tc_cscale = tc_prepare_table(idx->payload.as<float>(), N, d, idx->tc_cmax2, 2, idx->tc_cent, st);
-        idx->tc_cent_npl = 2;
+        tc_install_table(idx, idx->payload.as<float>(), norms, N, st);
         idx->tc_flat_rows = N;
-        if (idx->tc_mode == 0) idx->tc_fast = false;  // AUTO: new rows start PRECISE
-        idx->tc_stat_pending = false;
-        idx->tc_acc_rows = idx->tc_acc_bad = 0;
     }
     tc_stats_poll(idx, st);
     const bool fast = idx->tc_fast;
@@ -1293,26 +1248,17 @@ int dfx_tc_flat_candidates(dfx_index* idx, const float* d_x, int64_t nq, int k, 
     int G = k + 8;
     if (G > ng) G = ng;
     const int ncand = G * 32;
-    idx->tc_gmin.reserve((size_t)nq * ng * 4);
-    idx->tc_gmin2.reserve((size_t)nq * ng * 4);
-    idx->tc_gargc.reserve((size_t)nq * ng);
-    idx->tc_groups.reserve((size_t)nq * G * 4);
     idx->tc_cand.reserve((size_t)nq * ncand * 8);
-    idx->tc_tmin.reserve((size_t)nq * (ng / 4 + 1) * 4);
-    tc_screen(idx, d, d_x, nq, idx->tc_cent.p, idx->tc_cscale, fast ? 1 : 2, idx->xnorm.as<float>(), N, metric,
-              idx->tc_gmin.as<float>(), idx->tc_gmin2.as<float>(), idx->tc_gargc.as<uint8_t>(),
-              idx->tc_tmin.as<float>(), st);
-    tc_select_groups(idx->tc_gmin.as<float>(), idx->tc_tmin.as<float>(), nq, ng, G, idx->tc_groups.as<int32_t>(), st);
-    int32_t* ovf = tc_ovf_reset(idx, nq, st);
+    const Screened s = tc_screen_chunk(idx, d, d_x, nq, nq, ng, G, idx->tc_cent.p, idx->tc_cscale, fast ? 1 : 2,
+                                       idx->xnorm.as<float>(), N, metric, st);
     auto kern = rerank_kernel<0>;
     DFX_LAUNCH(kern, (unsigned)nq, 128, (size_t)d * 4, st, d_x, d, idx->payload.as<float>(), idx->xnorm.as<float>(), N,
-               metric, idx->tc_groups.as<int32_t>(), G, k, idx->tc_gmin.as<float>(), idx->tc_gmin2.as<float>(),
-               idx->tc_gargc.as<uint8_t>(), ng, idx->tc_cmax2, tol, idx->tc_cand.as<uint64_t>(), (int32_t*)nullptr,
-               (const int32_t*)nullptr, (const int32_t*)nullptr, nq, (int32_t*)nullptr, ovf);
+               metric, s.groups, G, k, s.gmin, s.gmin2, s.gargc, ng, idx->tc_cmax2, tol, idx->tc_cand.as<uint64_t>(),
+               (int32_t*)nullptr, (const int32_t*)nullptr, (const int32_t*)nullptr, nq, (int32_t*)nullptr, s.ovf);
     // rows with more near-ties than selected groups: their ncand slots become the exact top-ncand
-    launch_exact_rows(d_x, idx->payload.as<float>(), idx->xnorm.as<float>(), N, d, metric, ovf, nq, 0, ncand, nullptr,
-                      nullptr, idx->tc_cand.as<uint64_t>(), st);
-    tc_stats_post(idx, ovf, nq, fast, st);
+    launch_exact_rows(d_x, idx->payload.as<float>(), idx->xnorm.as<float>(), N, d, metric, s.ovf, nq, 0, ncand,
+                      nullptr, nullptr, idx->tc_cand.as<uint64_t>(), st);
+    tc_stats_post(idx, s.ovf, nq, fast, st);
     return ncand;
 }
 
@@ -1327,11 +1273,6 @@ void dfx_tc_assign(dfx_index* idx, int d, const float* d_cent, const float* d_cn
     const int G = ng < 6 ? ng : 6;
     const int64_t RC = std::max<int64_t>(tc::TILE, ((256ll << 20) / ((int64_t)ng * 4)) / tc::TILE * tc::TILE);
     const int64_t rmax = std::min<int64_t>(n, RC);
-    idx->tc_gmin.reserve((size_t)rmax * ng * 4);
-    idx->tc_gmin2.reserve((size_t)rmax * ng * 4);
-    idx->tc_gargc.reserve((size_t)rmax * ng);
-    idx->tc_groups.reserve((size_t)rmax * G * 4);
-    idx->tc_tmin.reserve((size_t)rmax * (ng / 4 + 1) * 4);
     idx->tc_qn.reserve((size_t)rmax * 4);
     idx->tc_amb.reserve((size_t)(rmax + 1) * 4);
     // fp16 copy of this centroid table (k-means changes it every iteration; converting is cheap).
@@ -1351,40 +1292,26 @@ void dfx_tc_assign(dfx_index* idx, int d, const float* d_cent, const float* d_cn
         tol.rel = screen_tol_rel(d, fast);
         tol.rel_fast = 0.f;  // counted once per row by assign_resolve_kernel
         const float rel_fast = (!fast && idx->tc_mode == 0) ? screen_tol_rel(d, true) : 0.f;
-        tc_screen(idx, d, xr, rc, idx->tc_cent_tmp.p, cscale, fast ? 1 : 2, d_cnorm, nlist, metric,
-                  idx->tc_gmin.as<float>(), idx->tc_gmin2.as<float>(), idx->tc_gargc.as<uint8_t>(),
-                  idx->tc_tmin.as<float>(), st);
-        tc_select_groups(idx->tc_gmin.as<float>(), idx->tc_tmin.as<float>(), rc, ng, G, idx->tc_groups.as<int32_t>(),
-                         st);
+        const Screened s = tc_screen_chunk(idx, d, xr, rc, rmax, ng, G, idx->tc_cent_tmp.p, cscale, fast ? 1 : 2,
+                                           d_cnorm, nlist, metric, st);
         dfx_launch_row_norms(xr, rc, d, idx->tc_qn.as<float>(), st);
         int32_t* amb_count = idx->tc_amb.as<int32_t>();
         int32_t* amb_rows = amb_count + 1;
         DFX_CUDA(cudaMemsetAsync(amb_count, 0, 4, st));
-        int32_t* ovf = tc_ovf_reset(idx, rc, st);
         DFX_LAUNCH(assign_resolve_kernel, (unsigned)dfx_ceil_div(rc, 256), 256, 0, st, idx->tc_qn.as<float>(),
-                   idx->tc_groups.as<int32_t>(), idx->tc_gmin.as<float>(), idx->tc_gmin2.as<float>(),
-                   idx->tc_gargc.as<uint8_t>(), ng, G, cmax2, tol.rel, rel_fast, rc, d_assign + r0, amb_rows,
-                   amb_count, ovf);
+                   s.groups, s.gmin, s.gmin2, s.gargc, ng, G, cmax2, tol.rel, rel_fast, rc, d_assign + r0, amb_rows,
+                   amb_count, s.ovf);
         auto kern = rerank_kernel<1>;
         const unsigned grid = (unsigned)std::min<int64_t>(rc, dfx_num_sms() * 16);
-        DFX_LAUNCH(kern, grid, 128, (size_t)d * 4, st, xr, d, d_cent, d_cnorm, nlist, metric,
-                   idx->tc_groups.as<int32_t>(), G, 1, idx->tc_gmin.as<float>(), idx->tc_gmin2.as<float>(),
-                   idx->tc_gargc.as<uint8_t>(), ng, cmax2, tol, (uint64_t*)nullptr, d_assign + r0,
-                   (const int32_t*)amb_rows, (const int32_t*)amb_count, rc, (int32_t*)nullptr, ovf);
-        launch_exact_rows(xr, d_cent, d_cnorm, nlist, d, metric, ovf, rc, 1, 1, nullptr, d_assign + r0, nullptr, st);
-        if (idx->tc_mode == 0 && r0 + rc < n) {  // AUTO: the next chunk's precision (rule of tc_auto_update)
+        DFX_LAUNCH(kern, grid, 128, (size_t)d * 4, st, xr, d, d_cent, d_cnorm, nlist, metric, s.groups, G, 1, s.gmin,
+                   s.gmin2, s.gargc, ng, cmax2, tol, (uint64_t*)nullptr, d_assign + r0, (const int32_t*)amb_rows,
+                   (const int32_t*)amb_count, rc, (int32_t*)nullptr, s.ovf);
+        launch_exact_rows(xr, d_cent, d_cnorm, nlist, d, metric, s.ovf, rc, 1, 1, nullptr, d_assign + r0, nullptr, st);
+        if (idx->tc_mode == 0 && r0 + rc < n) {  // AUTO: the next chunk's precision
             int32_t h[2] = {0, 0};
-            DFX_CUDA(cudaMemcpyAsync(h, ovf, 8, cudaMemcpyDeviceToHost, st));
+            DFX_CUDA(cudaMemcpyAsync(h, s.ovf, 8, cudaMemcpyDeviceToHost, st));
             DFX_CUDA(cudaStreamSynchronize(st));
-            acc_rows += rc;
-            acc_bad += fast ? h[0] : h[1];
-            if (!fast && acc_rows >= idx->tc_auto_window) {
-                fast = acc_bad == 0;
-                acc_rows = acc_bad = 0;
-            } else if (fast && acc_bad > 0 && acc_bad * idx->tc_auto_window > acc_rows) {
-                fast = false;
-                acc_rows = acc_bad = 0;
-            }
+            fast = tc_auto_step(fast, rc, h[0], h[1], idx->tc_auto_window, acc_rows, acc_bad);
         }
     }
 }

@@ -3,6 +3,31 @@
 #include "dfx_common.cuh"
 #include "dfx_select.cuh"
 
+// ascending bitonic sort of buf[0, cnt) by one warp: the slots up to P = the next power of two
+// >= max(cnt, 32) are padded with NONE and sorted with them; returns P
+__device__ __forceinline__ int dfx_warp_sort_buf(uint64_t* buf, int cnt, int lane) {
+    int P = 32;
+    while (P < cnt) P <<= 1;
+    for (int e = cnt + lane; e < P; e += 32) buf[e] = DFX_COMP_NONE;
+    __syncwarp();
+    for (int size = 2; size <= P; size <<= 1) {
+        for (int stride = size >> 1; stride > 0; stride >>= 1) {
+            for (int i = lane; i < (P >> 1); i += 32) {
+                const int pos = 2 * i - (i & (stride - 1));
+                const int partner = pos + stride;
+                const bool up = ((pos & size) == 0);
+                const uint64_t a = buf[pos], b = buf[partner];
+                if ((a > b) == up) {
+                    buf[pos] = b;
+                    buf[partner] = a;
+                }
+            }
+            __syncwarp();
+        }
+    }
+    return P;
+}
+
 // =====================================================================================
 // per-warp candidate set: keeps the k best composites seen so far in shared memory.
 // buf has CAP = 2*KP slots (KP = pow2 >= max(k,32)); when it cannot take another 32
@@ -47,27 +72,9 @@ struct WarpTopK {
     }
     __device__ __forceinline__ void sort_and_cut() {
         const int lane = threadIdx.x & 31;
-        // sort only as many slots as are live (rounded up to a power of two, >= 32); slots
-        // beyond P are never read before they are overwritten by later pushes
-        int P = 32;
-        while (P < cnt) P <<= 1;
-        for (int e = cnt + lane; e < P; e += 32) buf[e] = DFX_COMP_NONE;
-        __syncwarp();
-        for (int size = 2; size <= P; size <<= 1) {
-            for (int stride = size >> 1; stride > 0; stride >>= 1) {
-                for (int i = lane; i < (P >> 1); i += 32) {
-                    int pos = 2 * i - (i & (stride - 1));
-                    int partner = pos + stride;
-                    bool up = ((pos & size) == 0);
-                    uint64_t a = buf[pos], b = buf[partner];
-                    if ((a > b) == up) {
-                        buf[pos] = b;
-                        buf[partner] = a;
-                    }
-                }
-                __syncwarp();
-            }
-        }
+        // sort only as many slots as are live; slots beyond P are never read before they are
+        // overwritten by later pushes
+        dfx_warp_sort_buf(buf, cnt, lane);
         if (cnt > k) cnt = k;
         if (cnt == k) {
             const uint64_t kth = buf[k - 1];

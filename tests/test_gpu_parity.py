@@ -413,6 +413,43 @@ def test_tensor_core_near_tie_overflow_is_redone_exactly():
             _assert_same(*gf.search(qf, 10), Do, Io, f"duplicate rows flat metric={metric} mode={mode}")
 
 
+def test_tensor_core_many_groups_select_from_all_candidates():
+    """nlist 8192 = 256 groups of 32 lists: nprobe 128 keeps G = 136 groups, more candidate slots
+    (G x 32 > 4096) than the fused decide kernel sorts in shared memory, so every candidate's exact
+    composite is written out (rerank_kernel<0>) and the top-nprobe selected from them; nprobe 1 / 7
+    take the warp-per-query kernel and 40 the fused one.  Centroids come from set_state (no
+    training), rows are assigned by the tensor-core screening (dfx_tc_assign)."""
+    from oracle import oracle as O
+
+    E = _engine()
+    rs = np.random.RandomState(31)
+    d, nlist = 64, 8192
+    cent = rs.randn(nlist, d).astype(np.float32)
+
+    def empty():
+        return {"centroids": cent, "list_off": np.zeros(nlist + 1, np.int64), "ids": np.zeros(0, np.int64),
+                "vecs": np.zeros((0, d), np.float32)}
+
+    o = O.make_index("ivf_flat", d, metric=L2, nlist=nlist)
+    o.set_state(empty())
+    g = E.GpuIndex(E.KIND_IVF_FLAT, d, L2, nlist=nlist)
+    g.set_state(empty())
+    n, nq = _sz(10_000, 2_000), _sz(200, 16)
+    xb = (cent[rs.randint(0, nlist, n)] + 0.3 * rs.randn(n, d)).astype(np.float32)
+    o.add(xb)
+    g.add(xb)
+    st = g.get_state()
+    assert np.array_equal(st["list_off"], o.list_off) and np.array_equal(st["ids"], o.ids)
+    xq = (cent[rs.randint(0, nlist, nq)] + 0.3 * rs.randn(nq, d)).astype(np.float32)
+    for nprobe in (1, 7, 40, 128):
+        g.nprobe = nprobe; o.nprobe = nprobe
+        Do, Io = o.search(xq, 10)
+        for mode in (2, 1, 0):
+            g.set_param("tc_screen_mode", mode)
+            _assert_same(*g.search(xq, 10), Do, Io, f"nlist 8192 nprobe={nprobe} mode={mode}")
+            assert g.last_stats()["ndis"] == o.last_ndis
+
+
 def test_tensor_core_auto_precision_follows_the_data():
     """tc_screen_mode 0 (AUTO): a shard starts with the PRECISE screening (fp16 hi/lo split, three
     MMAs) and moves to FAST (one MMA) only after a window of observed rows none of which would
