@@ -77,7 +77,7 @@ int dfx_debug_il_byte(int layout, int v, int m) { return dfx_il_byte_of(layout, 
 int dfx_create(const dfx_cfg* cfg, dfx_index** out) {
     DFX_API_BEGIN
     DFX_REQUIRE(cfg && out, "null argument");
-    DFX_REQUIRE(cfg->kind >= DFX_FLAT && cfg->kind <= DFX_IVF_SQ16, "unknown index kind");
+    DFX_REQUIRE(cfg->kind >= DFX_FLAT && cfg->kind <= DFX_IVF_SQ8, "unknown index kind");
     DFX_REQUIRE(cfg->metric == DFX_METRIC_IP || cfg->metric == DFX_METRIC_L2,
                 "Only dot and l2 metrics are supported.");
     DFX_REQUIRE(cfg->d > 0 && cfg->d <= 4096, "dimension must be in [1, 4096]");
@@ -439,6 +439,7 @@ static const char* payload_name(int kind) {
         case DFX_IVF_FLAT: return "vecs";
         case DFX_IVF_PQ: return "codes";
         case DFX_IVF_SQ16: return "codes16";
+        case DFX_IVF_SQ8: return "codes8";
     }
     return "";
 }
@@ -472,6 +473,7 @@ int dfx_get_array(dfx_index* idx, const char* name, void* out, int64_t max_bytes
     bool widen_ids = false;
     if (n == "centroids" && idx->is_ivf() && idx->trained) { src = idx->centroids.p; bytes = nlist * d * 4; }
     else if (n == "codebooks" && idx->cfg.kind == DFX_IVF_PQ && idx->trained) { src = idx->codebooks.p; bytes = (int64_t)idx->M * idx->ksub * idx->dsub * 4; }
+    else if (n == "sq_trained" && idx->cfg.kind == DFX_IVF_SQ8 && idx->trained) { src = idx->sq_trained.p; bytes = 2 * d * 4; }
     else if (n == "list_off" && idx->is_ivf() && idx->trained) { src = idx->list_off.p; bytes = (nlist + 1) * 8; }
     else if (n == "ids" && idx->is_ivf()) { widen_ids = true; bytes = nt * 8; }
     else if (n == "tvals" && idx->cfg.kind == DFX_IVF_PQ) { src = idx->tvals.p; bytes = nt * 4; }
@@ -515,6 +517,9 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
         DFX_REQUIRE(nbytes == (int64_t)idx->M * idx->ksub * idx->dsub * 4, "codebooks: wrong size");
         upload(idx->codebooks, nbytes);
         idx->cbT_valid = false;
+    } else if (n == "sq_trained" && idx->cfg.kind == DFX_IVF_SQ8) {
+        DFX_REQUIRE(nbytes == 2 * d * 4, "sq_trained: wrong size (2 * d floats: vmin, then vdiff)");
+        upload(idx->sq_trained, nbytes);
     } else if (n == "list_off" && idx->is_ivf()) {
         DFX_REQUIRE(nbytes == (nlist + 1) * 8, "list_off: wrong size");
         upload(idx->list_off, nbytes);
@@ -568,6 +573,7 @@ int dfx_import_done(dfx_index* idx) {
             dfx_compute_tvals_sorted(idx, idx->stream);  // K7 recomputes the per-vector term
             dfx_pq_rm_to_il(idx, idx->stream);
         }
+        if (idx->cfg.kind == DFX_IVF_SQ8) DFX_REQUIRE(idx->sq_trained.p, "import: sq_trained is required");
         dfx_tc_prepare_centroids(idx, idx->stream);
         DFX_CUDA(cudaStreamSynchronize(idx->stream));
     }

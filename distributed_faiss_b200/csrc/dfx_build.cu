@@ -6,7 +6,8 @@
 // but required to produce a searchable shard without any CPU fallback.
 // faiss semantics restated: Clustering = Lloyd iterations from a random subset, at most
 // 256 points per centroid, empty clusters re-seeded from a large one; ProductQuantizer
-// trained on residuals of <= 256*ksub training vectors; add = nearest centroid under the
+// trained on residuals of <= 256*ksub training vectors; the 8-bit scalar quantizer on the
+// per-dimension range of residuals of <= 100000 of them; add = nearest centroid under the
 // quantizer's metric, ids sequential, ids ascending inside every list.
 #include "dfx_internal.h"
 #include "dfx_ptx.cuh"
@@ -165,6 +166,67 @@ __global__ void sq_encode_kernel(const float* __restrict__ x, const float* __res
     int64_t i = t / d;
     int c = (int)(t - i * d);
     codes[t] = __float2half_rn(x[t] - cent[(size_t)assign[i] * d + c]);
+}
+
+// IEEE division, round to nearest (spelled out so that no compiler setting can relax it)
+__device__ __forceinline__ float dfx_div_rn(float a, float b) {
+#ifdef DFX_EMU
+    return a / b;
+#else
+    return __fdiv_rn(a, b);
+#endif
+}
+
+// IVF-SQ8 encode (faiss QT_8bit, non-uniform, by_residual; DESIGN.md section 2): per component
+// t = (r - vmin) / vdiff clamped to [0, 1] (0 where vdiff == 0), code = (int)(255 t), truncated
+__global__ void sq8_encode_kernel(const float* __restrict__ x, const float* __restrict__ cent,
+                                  const int32_t* __restrict__ assign, int64_t n, int d,
+                                  const float* __restrict__ trained, uint8_t* __restrict__ codes) {
+    int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n * d) return;
+    int64_t i = t / d;
+    int c = (int)(t - i * d);
+    const float r = x[t] - cent[(size_t)assign[i] * d + c];
+    const float vmin = trained[c], vdiff = trained[d + c];
+    float u = 0.f;
+    if (vdiff != 0.f) {
+        u = dfx_div_rn(r - vmin, vdiff);
+        u = u < 0.f ? 0.f : u;
+        u = u > 1.f ? 1.f : u;
+    }
+    codes[t] = (uint8_t)(int)(255.f * u);
+}
+
+// IVF-SQ8 training: per-dimension min / max of n residual rows.  Pass 1: extrema of chunks of
+// `rows_per` rows (grid.y = chunk); pass 2: over the chunks, trained = [vmin, vmax - vmin].
+// min and max do not depend on the order, so the result is exact.
+__global__ void sq8_minmax_partial_kernel(const float* __restrict__ r, int64_t n, int d, int64_t rows_per,
+                                          float* __restrict__ pmin, float* __restrict__ pmax) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= d) return;
+    const int64_t r0 = (int64_t)blockIdx.y * rows_per;
+    const int64_t r1 = min(n, r0 + rows_per);
+    float lo = FLT_MAX, hi = -FLT_MAX;
+    for (int64_t i = r0; i < r1; i++) {
+        const float v = r[i * d + c];
+        lo = v < lo ? v : lo;
+        hi = v > hi ? v : hi;
+    }
+    pmin[(int64_t)blockIdx.y * d + c] = lo;
+    pmax[(int64_t)blockIdx.y * d + c] = hi;
+}
+__global__ void sq8_minmax_final_kernel(const float* __restrict__ pmin, const float* __restrict__ pmax,
+                                        int64_t nchunks, int d, float* __restrict__ trained) {
+    const int c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= d) return;
+    float lo = FLT_MAX, hi = -FLT_MAX;
+    for (int64_t j = 0; j < nchunks; j++) {
+        const float a = pmin[j * d + c], b = pmax[j * d + c];
+        lo = a < lo ? a : lo;
+        hi = b > hi ? b : hi;
+    }
+    trained[c] = lo;
+    trained[d + c] = hi - lo;
 }
 
 // list id of every row of the list-sorted storage
@@ -356,6 +418,29 @@ void dfx_train_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st
                           idx->codebooks.as<float>() + (size_t)m * ksub * dsub, st);
         }
     }
+    if (kind == DFX_IVF_SQ8) {
+        // faiss ScalarQuantizer (QT_8bit, RS_minmax) on the residuals of the first min(nt, 100000)
+        // rows of the k-means sample, the way the PQ above takes a prefix of it
+        const int64_t ns = std::min<int64_t>(nt, 100000);
+        const int64_t rows_per = 256;
+        const int64_t nch = dfx_ceil_div(ns, rows_per);
+        DevBuf d_assign, d_res, d_part;
+        d_assign.reserve((size_t)ns * 4);
+        d_res.reserve((size_t)ns * d * 4);
+        d_part.reserve((size_t)nch * d * 8);
+        dfx_assign_impl(idx, idx->centroids.as<float>(), idx->cnorm.as<float>(), nlist, idx->cfg.metric,
+                        d, ns, xt, d_assign.as<int32_t>(), st);
+        DFX_LAUNCH(residual_kernel, blocks_for(ns * d, 256), 256, 0, st, xt, idx->centroids.as<float>(),
+                   d_assign.as<int32_t>(), ns, d, d_res.as<float>());
+        float* pmin = d_part.as<float>();
+        float* pmax = pmin + (size_t)nch * d;
+        DFX_LAUNCH(sq8_minmax_partial_kernel, dim3(blocks_for(d, 128), (unsigned)nch), 128, 0, st,
+                   d_res.as<float>(), ns, d, rows_per, pmin, pmax);
+        idx->sq_trained.reserve((size_t)2 * d * 4);
+        DFX_LAUNCH(sq8_minmax_final_kernel, blocks_for(d, 128), 128, 0, st, pmin, pmax, nch, d,
+                   idx->sq_trained.as<float>());
+        DFX_CUDA(cudaStreamSynchronize(st));
+    }
     // an empty, trained index
     idx->h_list_off.assign((size_t)nlist + 1, 0);
     idx->list_off.reserve((size_t)(nlist + 1) * 8);
@@ -427,9 +512,12 @@ void dfx_add_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) 
         DFX_LAUNCH(pq_tvals_kernel, blocks_for(n, 128), 128, 0, st, (const uint8_t*)prow, plist,
                    (const int64_t*)nullptr, nlist, n, d, M, ksub, dsub, idx->codebooks.as<float>(),
                    idx->centroids.as<float>(), idx->p_tvals.as<float>() + idx->n_pending);
-    } else {  // IVF_SQ16
+    } else if (kind == DFX_IVF_SQ16) {
         DFX_LAUNCH(sq_encode_kernel, blocks_for(n * d, 256), 256, 0, st, d_x, idx->centroids.as<float>(),
                    plist, n, d, (__half*)prow);
+    } else {  // IVF_SQ8
+        DFX_LAUNCH(sq8_encode_kernel, blocks_for(n * d, 256), 256, 0, st, d_x, idx->centroids.as<float>(),
+                   plist, n, d, idx->sq_trained.as<float>(), (uint8_t*)prow);
     }
     idx->n_pending += n;
 }
@@ -578,6 +666,34 @@ __global__ void reconstruct_kernel(int kind, int d, int M, int ksub, int dsub, i
     }
 }
 
+// IVF-SQ8: centroid + decoded residual (the decode of the list scan, DESIGN.md section 2).  Ids as
+// reconstruct_kernel: tag < 0 local ids (unknown / -1 -> NaN row), tag >= 0 exchange ids.
+__global__ void sq8_reconstruct_kernel(int d, int64_t ntotal, int64_t nlist, const int64_t* __restrict__ want,
+                                       const int32_t* __restrict__ inv, const uint8_t* __restrict__ codes,
+                                       const int64_t* __restrict__ list_off, const float* __restrict__ cent,
+                                       const float* __restrict__ trained, float* __restrict__ out, int64_t tag) {
+    const int64_t r = blockIdx.x;
+    int64_t id = want[r];
+    if (tag >= 0) {
+        if (id < 0 || ((id >> 40) & 0xfffff) != tag) return;
+        id &= (1ll << 40) - 1;
+    }
+    if (id < 0 || id >= ntotal) {
+        for (int k = threadIdx.x; k < d; k += blockDim.x) out[r * d + k] = __int_as_float(0x7fc00000);
+        return;
+    }
+    const int64_t pos = inv[id];
+    int64_t lo = 0, hi = nlist;
+    while (hi - lo > 1) {
+        int64_t mid = (lo + hi) >> 1;
+        if (list_off[mid] <= pos) lo = mid; else hi = mid;
+    }
+    for (int k = threadIdx.x; k < d; k += blockDim.x) {
+        const float t = __fmaf_rn((float)codes[pos * d + k], DFX_SQ8_SCALE, DFX_SQ8_BIAS);
+        out[r * d + k] = cent[(size_t)lo * d + k] + __fmaf_rn(t, trained[d + k], trained[k]);
+    }
+}
+
 void dfx_reconstruct_impl(dfx_index* idx, int64_t n, const int64_t* d_ids, float* d_out,
                           cudaStream_t st, int64_t tag) {
     if (n <= 0) return;
@@ -591,6 +707,12 @@ void dfx_reconstruct_impl(dfx_index* idx, int64_t n, const int64_t* d_ids, float
             DFX_LAUNCH(invert_ids_kernel, blocks_for(npos, 256), 256, 0, st,
                        il ? idx->il_ids.as<int32_t>() : idx->ids.as<int32_t>(), npos, idx->inv.as<int32_t>());
         idx->inv_valid = true;
+    }
+    if (idx->cfg.kind == DFX_IVF_SQ8) {
+        DFX_LAUNCH(sq8_reconstruct_kernel, (unsigned)n, 128, 0, st, idx->cfg.d, nt, idx->cfg.nlist, d_ids,
+                   idx->inv.as<int32_t>(), idx->payload.as<uint8_t>(), idx->list_off.as<int64_t>(),
+                   idx->centroids.as<float>(), idx->sq_trained.as<float>(), d_out, tag);
+        return;
     }
     DFX_LAUNCH(reconstruct_kernel, (unsigned)n, 128, 0, st, idx->cfg.kind, idx->cfg.d, idx->M, idx->ksub,
                idx->dsub, nt, idx->cfg.nlist, d_ids, idx->inv.as<int32_t>(),

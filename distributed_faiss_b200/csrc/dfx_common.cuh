@@ -9,6 +9,10 @@
 
 #include "../../include/dfx.h"
 
+// IVF-SQ8 decode (faiss QT_8bit, DESIGN.md section 2): t = fmaf(code, SCALE, BIAS)
+constexpr float DFX_SQ8_SCALE = 1.f / 255.f;
+constexpr float DFX_SQ8_BIAS = 0.5f / 255.f;
+
 // ---------------------------------------------------------------- errors
 void dfx_set_error(const std::string& msg);
 extern std::atomic<long long> g_dfx_launches;

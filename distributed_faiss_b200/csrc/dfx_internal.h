@@ -19,6 +19,7 @@ struct dfx_index {
     // list-sorted storage ("sorted") and arrival-order staging ("pending")
     int64_t n_sorted = 0, n_pending = 0;
     DevBuf centroids, cnorm, codebooks;
+    DevBuf sq_trained;                  // IVF_SQ8: f32[2][d] = vmin, vdiff (faiss ScalarQuantizer::trained)
     DevBuf list_off;                    // int64[nlist+1]
     std::vector<int64_t> h_list_off;    // host mirror
     DevBuf ids;                         // int32[n_sorted] shard-local ids, list-sorted
@@ -129,6 +130,7 @@ struct dfx_index {
             case DFX_IVF_FLAT: return (size_t)cfg.d * 4;
             case DFX_IVF_PQ: return (size_t)M;
             case DFX_IVF_SQ16: return (size_t)cfg.d * 2;
+            case DFX_IVF_SQ8: return (size_t)cfg.d;
         }
         return 0;
     }

@@ -1,13 +1,14 @@
 // dfx_search.cu -- the search hot path of one shard on one H100 (sm_90a).
 //
 // Replaces `self.faiss_index.search(query_batch, top_k)` (reference
-// distributed_faiss/index.py:257) for the four builders of index.py:93-100 and
+// distributed_faiss/index.py:257) for the four builders of index.py:93-100, the factory strings
+// of index.py:380-396 and
 // `IndexClient._aggregate_results` (client.py:265-310):
 //   K1a  gemm_values      coarse quantizer / flat contraction, fp32 FFMA, seq-k canonical order
 //   K_sel select_rows     exact k-selection (dfx_select.cuh)
 //   K3   pq_prep          per-query PQ table  -2<q_m,P[m][j]>  + exact ||q-c||^2 of probed lists
 //   K4   scan_pq          inverted-list scan of PQ codes, per-warp k-selection
-//   K2/5 scan_rows        inverted-list scan of fp32 rows / fp16 residual codes
+//   K2/5 scan_rows        inverted-list scan of fp32 rows / fp16 / 8-bit residual codes
 //   K6   merge            cross-shard merge (float_maxheap_array_t semantics)
 // Arithmetic orders are the canonical ones of oracle/dfx_oracle.c (bit-exact parity).
 #include "dfx_internal.h"
@@ -285,20 +286,34 @@ scan_pq_kernel(const float* __restrict__ lut, const float* __restrict__ dis0,
 //   MODE 0: fp32 rows, value = -<q,x>      (IVF-Flat, IP)
 //   MODE 1: fp32 rows, value = ||q-x||^2   (IVF-Flat, L2)
 //   MODE 2: fp16 residual codes, value = ||(q-c) - half2float(code)||^2   (IVF-SQ fp16)
+//   MODE 3: 8-bit residual codes, value = ||(q-c) - dfx_sq8_decode(code)||^2   (IVF-SQ8)
 // =====================================================================================
 // U = vectors in flight per warp: 4 (default), 8 = EXPERIMENTAL (dfx_set_param "rows_inflight"):
-// the kernel is bound by memory-level parallelism, not by instructions -- C2 (512 B per vector)
-// reaches 0.46 of the HBM peak and C4 (1536 B per vector) 0.68 with the same code.
+// the kernel is bound by memory-level parallelism, not by instructions -- on a B200, C2 (512 B per
+// vector) reached 0.46 of the HBM peak and C4 (1536 B per vector) 0.68 with the same code.
+//
+// MODE 3 decodes faiss's QT_8bit component (AVX2 form, DESIGN.md section 2):
+//   t = fmaf(code, 1/255, 0.5/255),  x = fmaf(t, vdiff, vmin).
+// (float)code is built as 0x4B0000cc - 2^23 (one PRMT + one FADD, exact) instead of an I2F, which
+// issues at an eighth of the FFMA rate on sm_90.  `sel` picks code byte j: 0x7540 + j.
+__device__ __forceinline__ float dfx_sq8_component(uint32_t w, uint32_t sel, float vmin, float vdiff) {
+    const float c = __uint_as_float(__byte_perm(w, 0x4B000000u, sel)) - 8388608.f;
+    return __fmaf_rn(__fmaf_rn(c, DFX_SQ8_SCALE, DFX_SQ8_BIAS), vdiff, vmin);
+}
+
 template <int MODE, int U = 4>
 __global__ void __launch_bounds__(128)
 scan_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent,
                  const int32_t* __restrict__ keys, int nprobe, int G, int ngroups,
                  const int64_t* __restrict__ list_off, const void* __restrict__ rows,
-                 const int32_t* __restrict__ ids, int k, int cap, uint64_t* __restrict__ part) {
+                 const int32_t* __restrict__ ids, int k, int cap, uint64_t* __restrict__ part,
+                 const float* __restrict__ sq_trained) {
     DFX_DYN_SMEM(unsigned char, smem_raw, 16);
-    float* s_q = reinterpret_cast<float*>(smem_raw);   // query (MODE 2: residual q - c)
-    float* s_q0 = s_q + d;                              // MODE 2: the raw query
-    const int dpad = (MODE == 2) ? 2 * d : d;
+    float* s_q = reinterpret_cast<float*>(smem_raw);   // query (MODE 2 / 3: residual q - c)
+    float* s_q0 = s_q + d;                              // MODE 2 / 3: the raw query
+    float* s_vmin = s_q + 2 * d;                        // MODE 3: vmin, then vdiff
+    float* s_vdiff = s_q + 3 * d;
+    const int dpad = (MODE == 3) ? 4 * d : (MODE == 2) ? 2 * d : d;
     uint64_t* s_buf = reinterpret_cast<uint64_t*>(smem_raw + (((size_t)dpad * 4 + 15) / 16) * 16);
     const int64_t q = blockIdx.x / ngroups;
     const int g = blockIdx.x % ngroups;
@@ -307,7 +322,11 @@ scan_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ c
     for (int i = tid; i < d; i += 128) {
         float qv = Q[q * d + i];
         s_q[i] = qv;
-        if (MODE == 2) s_q0[i] = qv;
+        if (MODE >= 2) s_q0[i] = qv;
+        if (MODE == 3) {
+            s_vmin[i] = sq_trained[i];
+            s_vdiff[i] = sq_trained[d + i];
+        }
     }
     WarpTopK wt;
     wt.init(s_buf + (size_t)warp * cap, cap, k);
@@ -317,7 +336,7 @@ scan_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ c
     for (int p = g * G; p < p_end; p++) {
         const int l = keys[q * nprobe + p];
         if (l < 0) continue;
-        if (MODE == 2) {
+        if (MODE >= 2) {
             __syncthreads();
             for (int i = tid; i < d; i += 128) s_q[i] = s_q0[i] - cent[(size_t)l * d + i];
             __syncthreads();
@@ -334,6 +353,26 @@ scan_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ c
             for (int kb = 4 * lane; kb < d; kb += 128) {
                 const float4 qv = *reinterpret_cast<const float4*>(s_q + kb);
                 float4 xv[U];
+                if (MODE == 3) {
+                    // 4 code bytes per lane and vector: a warp reads 128 contiguous bytes per vector
+                    uint32_t cw[U];
+#pragma unroll
+                    for (int u = 0; u < U; u++) {
+                        const int64_t i = base + u;
+                        cw[u] = (i < end) ? __ldg(reinterpret_cast<const uint32_t*>(
+                                                reinterpret_cast<const uint8_t*>(rows) + i * (int64_t)d + kb))
+                                          : 0u;
+                    }
+                    const float4 vmn = *reinterpret_cast<const float4*>(s_vmin + kb);
+                    const float4 vdf = *reinterpret_cast<const float4*>(s_vdiff + kb);
+#pragma unroll
+                    for (int u = 0; u < U; u++) {
+                        xv[u] = make_float4(dfx_sq8_component(cw[u], 0x7540u, vmn.x, vdf.x),
+                                            dfx_sq8_component(cw[u], 0x7541u, vmn.y, vdf.y),
+                                            dfx_sq8_component(cw[u], 0x7542u, vmn.z, vdf.z),
+                                            dfx_sq8_component(cw[u], 0x7543u, vmn.w, vdf.w));
+                    }
+                } else {
 #pragma unroll
                 for (int u = 0; u < U; u++) {
                     const int64_t i = base + u;
@@ -352,6 +391,7 @@ scan_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ c
                     } else {
                         xv[u] = make_float4(0.f, 0.f, 0.f, 0.f);
                     }
+                }
                 }
 #pragma unroll
                 for (int u = 0; u < U; u++) {
@@ -757,7 +797,8 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
 #undef DFX_SCAN_PQ
             }
         } else {
-            const int dq = (kind == DFX_IVF_SQ16) ? 2 * d : d;
+            // shared memory: the query; + the raw query (SQ16); + vmin and vdiff (SQ8)
+            const int dq = (kind == DFX_IVF_SQ8) ? 4 * d : (kind == DFX_IVF_SQ16) ? 2 * d : d;
             const size_t smem = (((size_t)dq * 4 + 15) / 16) * 16 + (size_t)4 * cap * 8;
             // vectors in flight per warp: rows of up to 1 KB need 8 to cover the DRAM latency,
             // longer rows keep 4 (rows_inflight overrides)
@@ -769,9 +810,10 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
                                       (int)smem));                                               \
         DFX_LAUNCH(kern, (unsigned)(qc * ngroups), 128, smem, st, xq, d, idx->centroids.as<float>(), \
                    keys, nprobe, G, ngroups, idx->list_off.as<int64_t>(), idx->payload.p,        \
-                   idx->ids.as<int32_t>(), k, cap, part);                                        \
+                   idx->ids.as<int32_t>(), k, cap, part, idx->sq_trained.as<float>());           \
     } while (0)
-            if (kind == DFX_IVF_SQ16) DFX_SCAN_ROWS(2);
+            if (kind == DFX_IVF_SQ8) DFX_SCAN_ROWS(3);
+            else if (kind == DFX_IVF_SQ16) DFX_SCAN_ROWS(2);
             else if (smetric == DFX_METRIC_IP) DFX_SCAN_ROWS(0);
             else DFX_SCAN_ROWS(1);
 #undef DFX_SCAN_ROWS

@@ -23,9 +23,10 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdfx.so")
 
-KIND_FLAT, KIND_IVF_FLAT, KIND_IVF_PQ, KIND_IVF_SQ16 = 0, 1, 2, 3
+KIND_FLAT, KIND_IVF_FLAT, KIND_IVF_PQ, KIND_IVF_SQ16, KIND_IVF_SQ8 = 0, 1, 2, 3, 4
 METRIC_INNER_PRODUCT, METRIC_L2 = 0, 1  # faiss enum values (reference index_cfg.py:44-52)
-KIND_NAMES = {KIND_FLAT: "flat", KIND_IVF_FLAT: "ivf_flat", KIND_IVF_PQ: "ivf_pq", KIND_IVF_SQ16: "ivf_sq"}
+KIND_NAMES = {KIND_FLAT: "flat", KIND_IVF_FLAT: "ivf_flat", KIND_IVF_PQ: "ivf_pq", KIND_IVF_SQ16: "ivf_sq",
+              KIND_IVF_SQ8: "ivf_sq8"}
 
 # every symbol include/dfx.h declares (tests check that the library exports each one)
 EXPORTED_SYMBOLS = [
@@ -268,7 +269,7 @@ class GpuIndex:
     # ---- state exchange (tests / persistence)
     _DTYPES = {"centroids": np.float32, "codebooks": np.float32, "list_off": np.int64, "ids": np.int64,
                "codes": np.uint8, "tvals": np.float32, "vecs": np.float32, "codes16": np.uint16,
-               "xb": np.float32}
+               "xb": np.float32, "sq_trained": np.float32, "codes8": np.uint8}
 
     def get_array(self, name):
         nb = C.c_int64(0)
@@ -283,7 +284,8 @@ class GpuIndex:
         _check(lib().dfx_set_array(self._h, name.encode(), _np_ptr(arr), C.c_int64(arr.nbytes)))
 
     def payload_name(self):
-        return {KIND_FLAT: "xb", KIND_IVF_FLAT: "vecs", KIND_IVF_PQ: "codes", KIND_IVF_SQ16: "codes16"}[self.kind]
+        return {KIND_FLAT: "xb", KIND_IVF_FLAT: "vecs", KIND_IVF_PQ: "codes", KIND_IVF_SQ16: "codes16",
+                KIND_IVF_SQ8: "codes8"}[self.kind]
 
     def get_state(self):
         """Same dict layout as oracle.get_state() (list-sorted storage order)."""
@@ -305,6 +307,9 @@ class GpuIndex:
             st["tvals"] = self.get_array("tvals")
         if self.kind == KIND_IVF_SQ16:
             st["codes16"] = self.get_array("codes16").reshape(-1, d)
+        if self.kind == KIND_IVF_SQ8:
+            st["sq_trained"] = self.get_array("sq_trained").reshape(2, d)
+            st["codes8"] = self.get_array("codes8").reshape(-1, d)
         return st
 
     def set_state(self, st):
@@ -314,6 +319,8 @@ class GpuIndex:
             self.set_array("centroids", st["centroids"])
             if self.kind == KIND_IVF_PQ:
                 self.set_array("codebooks", st["codebooks"])
+            if self.kind == KIND_IVF_SQ8:
+                self.set_array("sq_trained", st["sq_trained"])
             self.set_array("list_off", st["list_off"])
             self.set_array("ids", st["ids"])
             self.set_array(self.payload_name(), st[self.payload_name()])

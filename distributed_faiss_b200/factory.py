@@ -1,0 +1,74 @@
+"""faiss `index_factory` strings -> the engine kind that serves them.
+
+The reference lets a deployment describe a shard by a factory string instead of a builder name
+("Alternatively, if `index_builder_type` is not specified, one can set `faiss_factory` just like in
+FAISS API factory call `faiss.index_factory(...)`", reference README; index.py:385-396), and its
+`ivf_gpu` builder takes one too (index.py:71-86).  This module maps the strings that have a kernel
+here onto an engine kind.  It is pure: no engine, no torch, so tests use the same parser to build
+an oracle-backed engine.
+
+Tokens are case-sensitive, as in faiss:
+  "Flat"                          -> flat      (IndexFlat, the given metric)
+  "IVF{n},Flat"                   -> ivf_flat  (IndexIVFFlat, the given metric)
+  "IVF{n},PQ{M}" / "IVF{n},PQ{M}x8" -> ivf_pq  (IndexIVFPQ, 8-bit codes, L2 only)
+  "IVF{n},SQfp16"                 -> ivf_sq    (IndexIVFScalarQuantizer QT_fp16, L2 only)
+  "IVF{n},SQ8"                    -> ivf_sq8   (IndexIVFScalarQuantizer QT_8bit, L2 only)
+Everything else (OPQ / PCA prefixes, HNSW, IVF{n}_HNSW quantizers, RFlat / Refine, IDMap, PQ{M}x4,
+SQ4 / SQ6, malformed n or M) raises RuntimeError.
+"""
+import re
+from typing import NamedTuple
+
+METRIC_INNER_PRODUCT, METRIC_L2 = 0, 1  # faiss enum values
+
+ACCEPTED_FORMS = ("Flat", "IVF{n},Flat", "IVF{n},PQ{M}", "IVF{n},PQ{M}x8", "IVF{n},SQfp16", "IVF{n},SQ8")
+
+_IVF = re.compile(r"IVF([1-9][0-9]*),(Flat|PQ([1-9][0-9]*)(x8)?|SQfp16|SQ8)")
+_PQ_M_MAX = 64  # the IVF-PQ scan keeps at most 64 table values per vector
+
+
+class FactorySpec(NamedTuple):
+    """kind: a name of engine.KIND_NAMES ("flat", "ivf_flat", "ivf_pq", "ivf_sq", "ivf_sq8").
+    metric: flat / ivf_flat: the search metric; the codecs: the coarse quantizer's metric (their
+    search is L2)."""
+    kind: str
+    metric: int
+    nlist: int = 0
+    pq_m: int = 0
+
+
+def substitute_centroids(factory_string: str, centroids: int) -> str:
+    """`{centroids}` -> cfg.centroids, as the reference's factory path does (index.py:391-394);
+    a string without the placeholder is used as it is."""
+    if "{centroids}" in factory_string:
+        return factory_string.format(centroids=int(centroids))
+    return factory_string
+
+
+def parse_factory(dim: int, factory_string: str, metric: int) -> FactorySpec:
+    """(dim, factory string, faiss metric) -> FactorySpec, or RuntimeError for a string no kernel
+    here serves."""
+    s = factory_string if isinstance(factory_string, str) else ""
+    if s == "Flat":
+        return FactorySpec("flat", int(metric))
+    m = _IVF.fullmatch(s)
+    if m is None:
+        raise RuntimeError(
+            f"faiss_factory {factory_string!r} is not supported by the GPU search path; accepted forms: "
+            + ", ".join(ACCEPTED_FORMS) + " (n: number of lists, M: PQ sub-quantizers; case-sensitive)")
+    nlist, codec = int(m.group(1)), m.group(2)
+    if codec == "Flat":
+        return FactorySpec("ivf_flat", int(metric), nlist)
+    if int(metric) != METRIC_L2:
+        raise RuntimeError(
+            f"faiss_factory {factory_string!r} with the inner-product metric is not supported: a PQ or SQ "
+            "codec searched by inner product needs inner-product distance tables, which no list scan here "
+            "has (use metric='l2', or IVF{n},Flat for inner product)")
+    if codec.startswith("PQ"):
+        M = int(m.group(3))
+        if M % 4 != 0 or M > _PQ_M_MAX or dim % M != 0:
+            raise RuntimeError(
+                f"faiss_factory {factory_string!r}: the number of PQ sub-quantizers must be a multiple of 4, "
+                f"at most {_PQ_M_MAX}, that divides d={dim}")
+        return FactorySpec("ivf_pq", int(metric), nlist, M)
+    return FactorySpec("ivf_sq" if codec == "SQfp16" else "ivf_sq8", int(metric), nlist)

@@ -1,6 +1,7 @@
 """Reader / writer for the faiss on-disk index format, for the four index types the reference's
 builders create (reference index.py:94 IndexFlatIP, :36-40 IndexIVFFlat, :43-48 IndexIVFPQ,
-:63-68 IndexIVFScalarQuantizer(QT_fp16)); the reference saves shards with
+:63-68 IndexIVFScalarQuantizer(QT_fp16)) and the 8-bit scalar quantizer of the factory string
+"IVF{n},SQ8" (IndexIVFScalarQuantizer(QT_8bit)); the reference saves shards with
 `faiss.write_index(self.faiss_index, index_file)` (index.py:459) and loads them with
 `faiss.read_index` (index.py:303).  SURVEY.md section 8(f) next-3.
 
@@ -24,9 +25,11 @@ Layout (little endian, no padding; `vec<T>` = u64 count + raw elements):
   IVFFlat  : "IwFl", ivf hdr, invlists (code = raw f32 vector)
   IVFPQ    : "IwPQ", ivf hdr, u8 by_residual, u64 code_size, PQ (u64 d, u64 M, u64 nbits,
              vec<f32> centroids [M][ksub][dsub]), invlists (code = M bytes)
-  IVFSQ    : "IwSq", ivf hdr, SQ (i32 qtype = 4 (fp16), i32 rangestat, f32 rangestat_arg, u64 d,
-             u64 code_size, vec<f32> trained (empty)), u64 code_size, u8 by_residual, invlists
-             (code = d little-endian fp16 of the residual)
+  IVFSQ    : "IwSq", ivf hdr, SQ (i32 qtype, i32 rangestat, f32 rangestat_arg, u64 d,
+             u64 code_size, vec<f32> trained), u64 code_size, u8 by_residual, invlists
+             qtype 4 (fp16): trained empty, code = d little-endian fp16 of the residual
+             qtype 0 (8bit): rangestat 0 (min-max), trained = [vmin (d), vdiff (d)],
+                             code = d bytes of the residual
 """
 import struct
 from typing import BinaryIO, Dict, Tuple
@@ -34,7 +37,7 @@ from typing import BinaryIO, Dict, Tuple
 import numpy as np
 
 METRIC_IP, METRIC_L2 = 0, 1
-QT_FP16 = 4
+QT_8BIT, QT_FP16 = 0, 4
 
 
 class FaissFormatError(RuntimeError):
@@ -223,6 +226,16 @@ def write_index(state: Dict, path: str, nprobe: int = 1) -> None:
             _w(f, "B", 1)  # by_residual
             c16 = np.ascontiguousarray(state["codes16"], dtype="<u2")
             _write_invlists(f, state["list_off"], state["ids"], c16, 2 * d)
+        elif kind == "ivf_sq8":
+            d = int(state["d"])
+            f.write(b"IwSq")
+            _write_ivf_header(f, state, METRIC_L2, int(state["coarse_metric"]), nprobe)
+            _w(f, "iif", QT_8BIT, 0, 0.0)  # rangestat 0 = RS_minmax, rangestat_arg 0
+            _w(f, "QQ", d, d)
+            _wvec(f, np.asarray(state["sq_trained"], dtype=np.float32).reshape(2 * d), np.float32)
+            _w(f, "Q", d)
+            _w(f, "B", 1)  # by_residual
+            _write_invlists(f, state["list_off"], state["ids"], np.ascontiguousarray(state["codes8"], np.uint8), d)
         else:
             raise FaissFormatError(f"unknown index kind {kind!r}")
 
@@ -237,7 +250,7 @@ def read_index(path: str) -> Tuple[Dict, int]:
         if cc not in ("IwFl", "IwPQ", "IwSq"):
             raise FaissFormatError(
                 f"faiss index type {cc!r} is not one of the types the GPU search path serves "
-                "(IndexFlat, IndexIVFFlat, IndexIVFPQ, IndexIVFScalarQuantizer fp16)")
+                "(IndexFlat, IndexIVFFlat, IndexIVFPQ, IndexIVFScalarQuantizer fp16 / 8bit)")
         d, ntotal, metric, nlist, nprobe, cent, cmetric = _read_ivf_header(f)
         st = {"d": d, "nlist": nlist, "centroids": cent}
         if cc == "IwFl":
@@ -258,15 +271,24 @@ def read_index(path: str) -> Tuple[Dict, int]:
             st.update(kind="ivf_pq", coarse_metric=cmetric, M=M, ksub=256,
                       codebooks=cb.reshape(M, 256, d // M), codes=rows.reshape(-1, M))
         else:
-            qtype, _, _ = _r(f, "iif")
+            qtype, rangestat, _ = _r(f, "iif")
             sd, scs = _r(f, "QQ")
-            _rvec(f, np.float32)
+            trained = _rvec(f, np.float32)
             (code_size,) = _r(f, "Q")
             (by_res,) = _r(f, "B")
-            if qtype != QT_FP16 or not by_res or code_size != 2 * d:
-                raise FaissFormatError("IndexIVFScalarQuantizer: only QT_fp16, by_residual is supported")
-            list_off, ids, rows, cs = _read_invlists(f, nlist)
-            st.update(kind="ivf_sq", coarse_metric=cmetric, codes16=rows.view("<u2").reshape(-1, d))
+            if qtype == QT_8BIT:
+                if not by_res or code_size != d or trained.size != 2 * d:
+                    raise FaissFormatError("IndexIVFScalarQuantizer QT_8bit: only by_residual with d codes "
+                                           "and a [vmin, vdiff] trained vector is supported")
+                list_off, ids, rows, cs = _read_invlists(f, nlist)
+                st.update(kind="ivf_sq8", coarse_metric=cmetric, sq_trained=trained.reshape(2, d),
+                          codes8=rows.reshape(-1, d))
+            else:
+                if qtype != QT_FP16 or not by_res or code_size != 2 * d:
+                    raise FaissFormatError("IndexIVFScalarQuantizer: only QT_fp16 and QT_8bit, by_residual, "
+                                           "are supported")
+                list_off, ids, rows, cs = _read_invlists(f, nlist)
+                st.update(kind="ivf_sq", coarse_metric=cmetric, codes16=rows.view("<u2").reshape(-1, d))
         if len(ids) != ntotal:
             raise FaissFormatError("inverted lists do not hold ntotal vectors")
         st.update(list_off=list_off, ids=ids)

@@ -15,8 +15,13 @@ Builders (reference index.py:93-100):
                                           nbits = extra["bits_per_vector"] (8); cfg.nprobe is
                                           overwritten by the index default 1 (quirk B3)
   "ivfsq"      -> IndexIVFScalarQuantizer(QT_fp16), always L2, nprobe = cfg.nprobe
-"hnswsq", "ivf_gpu" and free-form `faiss_factory` strings are outside the hot path this
-package rebuilds (SURVEY.md section 8) and raise.
+  "ivf_gpu"    -> faiss.index_factory(dim, faiss_factory): the raw string, L2 whatever cfg.metric
+                  says, nprobe = cfg.nprobe (index.py:71-86)
+  no builder, `faiss_factory` set -> the factory string with {centroids} substituted, the cfg metric
+                  for the index and its quantizer, nprobe = the faiss default 1 (index.py:385-396)
+Factory strings are parsed by factory.parse_factory ("Flat", "IVF{n},Flat", "IVF{n},PQ{M}[x8]",
+"IVF{n},SQfp16", "IVF{n},SQ8"); any other string raises, and so does "hnswsq" (a graph index,
+outside the hot path this package rebuilds, SURVEY.md section 8).
 """
 import _thread
 import logging
@@ -29,6 +34,7 @@ from typing import Callable, List, Optional, Tuple, Union
 
 import numpy as np
 
+from .factory import METRIC_L2, parse_factory, substitute_centroids
 from .index_cfg import IndexCfg, METRIC_INNER_PRODUCT
 from .index_state import IndexState
 
@@ -40,11 +46,41 @@ INDEX_FILE = "index.dfx.npz"
 FAISS_INDEX_FILE = "index.faiss"
 
 
+def factory_spec(cfg: IndexCfg):
+    """The FactorySpec of a cfg that describes its shard by a factory string (builder "ivf_gpu", or
+    no builder and `faiss_factory` set), else None.  Pure: tests build oracle engines from it."""
+    btype = cfg.index_builder_type
+    if btype == "ivf_gpu":
+        # reference index.py:71-86: faiss.index_factory(cfg.dim, cfg.faiss_factory) -- the raw string
+        # and faiss's default metric, L2, for the index and its quantizer (cfg.metric only picks the
+        # k-means clustering index)
+        spec = parse_factory(cfg.dim, cfg.faiss_factory, METRIC_L2)
+        if spec.kind == "flat":
+            raise RuntimeError(f"ivf_gpu needs an IVF factory string, got {cfg.faiss_factory!r} "
+                               "(faiss.extract_index_ivf fails on it in the reference)")
+        return spec
+    if not btype and cfg.faiss_factory:
+        # reference index.py:385-396: {centroids} substituted, the cfg metric for the index and its
+        # quantizer; nlist is the string's
+        return parse_factory(cfg.dim, substitute_centroids(cfg.faiss_factory, cfg.centroids), cfg.get_metric())
+    return None
+
+
 def default_engine_factory(cfg: IndexCfg, device: Optional[int] = None):
     """cfg -> GPU engine object (the CUDA library is loaded here; fails loudly without it).
     `device`: the GPU ordinal of the owning IndexServer rank; None = the calling thread's current
     device (only safe on the thread that was pinned, see Index._bind_device)."""
     from . import engine
+
+    spec = factory_spec(cfg)
+    if spec is not None:
+        kind = {name: k for k, name in engine.KIND_NAMES.items()}[spec.kind]
+        idx = engine.GpuIndex(kind, cfg.dim, spec.metric, nlist=spec.nlist, pq_m=spec.pq_m, device=device)
+        if cfg.index_builder_type == "ivf_gpu":
+            idx.nprobe = cfg.nprobe  # index.py:84
+        # the factory path keeps faiss's default nprobe (1) and leaves cfg.nprobe alone, unlike
+        # knnlm (quirk B3); set_nprobe or a load_index with a cfg changes it
+        return idx
 
     btype = cfg.index_builder_type
     if btype == "flat":
@@ -65,11 +101,22 @@ def default_engine_factory(cfg: IndexCfg, device: Optional[int] = None):
                               device=device)
         idx.nprobe = cfg.nprobe
         return idx
-    if btype in ("hnswsq", "ivf_gpu") or cfg.faiss_factory:
+    if btype == "hnswsq" or cfg.faiss_factory:
         raise RuntimeError(
             f"index_builder_type={btype!r} / faiss_factory={cfg.faiss_factory!r} is not part of the "
-            "GPU search path (supported builders: flat, ivf_simple, knnlm, ivfsq)")
+            "GPU search path (supported builders: flat, ivf_simple, knnlm, ivfsq, ivf_gpu, or no builder "
+            "and a faiss_factory string)")
     raise RuntimeError("Either faiss_factory or valid index_builder_type should be specified to initialize index")
+
+
+def _kind_name(engine_obj) -> str:
+    """state-dict kind name ("flat", "ivf_sq8", ...) of an engine object (GPU or oracle)"""
+    kind = getattr(engine_obj, "kind", None)
+    if isinstance(kind, str):
+        return kind
+    from . import engine
+
+    return engine.KIND_NAMES.get(kind, str(kind))
 
 
 class IntMetadata:
@@ -508,6 +555,11 @@ class Index:
         saved_nprobe = cfg.nprobe
         engine = result._engine_factory(build_cfg)
         cfg.nprobe = saved_nprobe
+        want = _kind_name(engine)
+        if state.get("kind") != want:
+            # e.g. an SQfp16 file under a cfg that builds IVF-SQ8: never reinterpret the codes
+            raise RuntimeError(f"the stored index is of kind {state.get('kind')!r} but the cfg builds "
+                               f"{want!r}; refusing to load it")
         engine.set_state(state)
         assert len(meta) >= engine.ntotal, "Deserialized meta list should be at least of index size"
         result.faiss_index = engine

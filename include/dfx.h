@@ -40,7 +40,9 @@ enum {
     DFX_FLAT = 0,     /* faiss.IndexFlatIP / IndexFlatL2         index.py:94, 25-33 */
     DFX_IVF_FLAT = 1, /* faiss.IndexIVFFlat                       index.py:36-40     */
     DFX_IVF_PQ = 2,   /* faiss.IndexIVFPQ (L2, by_residual)       index.py:43-48     */
-    DFX_IVF_SQ16 = 3  /* faiss.IndexIVFScalarQuantizer(QT_fp16)   index.py:63-68     */
+    DFX_IVF_SQ16 = 3, /* faiss.IndexIVFScalarQuantizer(QT_fp16)   index.py:63-68     */
+    DFX_IVF_SQ8 = 4   /* faiss.IndexIVFScalarQuantizer(QT_8bit), by_residual: the factory string
+                         "IVF{n},SQ8" (index.py:380-396) -- one byte per dimension */
 };
 
 /* faiss.METRIC_INNER_PRODUCT / faiss.METRIC_L2 (index_cfg.py:44-52) */
@@ -48,14 +50,14 @@ enum { DFX_METRIC_IP = 0, DFX_METRIC_L2 = 1 };
 
 typedef struct dfx_cfg {
     int32_t kind;     /* DFX_FLAT ... */
-    int32_t metric;   /* FLAT / IVF_FLAT: search metric.  IVF_PQ / IVF_SQ16: metric of the
-                         coarse quantizer only -- the reference never forwards it to the
+    int32_t metric;   /* FLAT / IVF_FLAT: search metric.  IVF_PQ / IVF_SQ16 / IVF_SQ8: metric of
+                         the coarse quantizer only -- the reference never forwards it to the
                          index, which is therefore always L2 (index.py:44-46, 64-66). */
     int32_t d;        /* vector dimension (cfg.dim) */
     int32_t pq_m;     /* IVF_PQ: sub-quantizers  (cfg.extra["code_size"], index.py:44) */
     int32_t pq_nbits; /* IVF_PQ: bits per code   (cfg.extra["bits_per_vector"], index.py:45) */
     int32_t device;   /* CUDA device ordinal this shard lives on */
-    int64_t nlist;    /* IVF_*: number of inverted lists (cfg.centroids) */
+    int64_t nlist;    /* IVF_*: number of inverted lists (cfg.centroids); IVF kinds need d % 4 == 0 */
 } dfx_cfg;
 
 /* ---- lifetime: replaces the faiss constructors at index.py:25-48,63-68,94 ---- */
@@ -169,8 +171,11 @@ int dfx_map_ids_dev(int64_t n, const int64_t *d_ids, const int64_t *d_table, int
  *   "centroids" f32[nlist,d]   "codebooks" f32[M,ksub,dsub]   "list_off" i64[nlist+1]
  *   "ids" i64[ntotal]   "codes" u8[ntotal,M]   "tvals" f32[ntotal]
  *   "vecs" f32[ntotal,d] (IVF_FLAT)   "codes16" u16[ntotal,d]   "xb" f32[ntotal,d] (FLAT)
+ *   "sq_trained" f32[2,d] (IVF_SQ8: vmin, then vdiff -- faiss's ScalarQuantizer::trained)
+ *   "codes8" u8[ntotal,d] (IVF_SQ8)
  * dfx_get_array with out == NULL only reports the size.  Import order: centroids,
- * codebooks, then list_off, ids and the payload, then dfx_import_done(). */
+ * codebooks (IVF_PQ) or sq_trained (IVF_SQ8), then list_off, ids and the payload, then
+ * dfx_import_done(). */
 int dfx_get_array(dfx_index *idx, const char *name, void *out, int64_t max_bytes,
                   int64_t *nbytes);
 int dfx_set_array(dfx_index *idx, const char *name, const void *in, int64_t nbytes);
