@@ -36,8 +36,9 @@ static void require_device(int device) {
                                    std::to_string(p.major) + std::to_string(p.minor));
 }
 
-int dfx_num_sms() {
-    static std::atomic<int> cache[64];  // per device ordinal; 0 = not queried yet
+// one property of the current device, read once per device ordinal (cache entry 0 = not queried yet)
+template <class Get>
+static int cached_device_prop(std::atomic<int> (&cache)[64], Get get) {
     int dev = 0;
     DFX_CUDA(cudaGetDevice(&dev));
     DFX_REQUIRE(dev >= 0 && dev < 64, "device ordinal out of range");
@@ -45,10 +46,20 @@ int dfx_num_sms() {
     if (n == 0) {
         cudaDeviceProp p;
         DFX_CUDA(cudaGetDeviceProperties(&p, dev));
-        n = p.multiProcessorCount;
+        n = get(p);
         cache[dev].store(n, std::memory_order_relaxed);
     }
     return n;
+}
+
+int dfx_num_sms() {
+    static std::atomic<int> cache[64];
+    return cached_device_prop(cache, [](const cudaDeviceProp& p) { return p.multiProcessorCount; });
+}
+
+int dfx_smem_optin() {
+    static std::atomic<int> cache[64];
+    return cached_device_prop(cache, [](const cudaDeviceProp& p) { return (int)p.sharedMemPerBlockOptin; });
 }
 
 struct DeviceGuard {
@@ -92,7 +103,10 @@ int dfx_create(const dfx_cfg* cfg, dfx_index** out) {
         DFX_REQUIRE(cfg->pq_nbits == 8, "IVF-PQ: only 8 bits per sub-quantizer are supported");
         DFX_REQUIRE(cfg->pq_m >= 4 && cfg->pq_m % 4 == 0 && cfg->d % cfg->pq_m == 0,
                     "IVF-PQ: the number of sub-quantizers must be a multiple of 4 that divides d");
-        DFX_REQUIRE(cfg->pq_m <= 64, "IVF-PQ: at most 64 sub-quantizers are supported");
+        DFX_REQUIRE(cfg->pq_m <= 128,
+                    "IVF-PQ: at most 128 sub-quantizers are supported (one query's fp32 distance table, "
+                    "M x 256 x 4 bytes, must fit in one thread block's shared memory; more would need split "
+                    "or fp16 tables, which are not bit-exact)");
         idx->M = cfg->pq_m;
         idx->ksub = 256;
         idx->dsub = cfg->d / cfg->pq_m;

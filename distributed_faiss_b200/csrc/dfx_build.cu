@@ -505,6 +505,7 @@ void dfx_add_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) 
     } while (0)
         if (dsub == 2) DFX_PQ_ENCODE(2);
         else if (dsub == 4) DFX_PQ_ENCODE(4);
+        else if (dsub == 6) DFX_PQ_ENCODE(6);  // d = 768 with M = 128
         else if (dsub == 8) DFX_PQ_ENCODE(8);
         else if (dsub == 16) DFX_PQ_ENCODE(16);
         else DFX_PQ_ENCODE(0);

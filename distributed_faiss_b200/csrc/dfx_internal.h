@@ -9,6 +9,8 @@
 
 // streaming multiprocessors of the current device (launch shapes are sized in waves over them)
 int dfx_num_sms();
+// dynamic shared memory one CTA of the current device may opt in to (bytes)
+int dfx_smem_optin();
 
 struct dfx_index {
     dfx_cfg cfg{};

@@ -8,6 +8,7 @@
 //   K_sel select_rows     exact k-selection (dfx_select.cuh)
 //   K3   pq_prep          per-query PQ table  -2<q_m,P[m][j]>  + exact ||q-c||^2 of probed lists
 //   K4   scan_pq          inverted-list scan of PQ codes, per-warp k-selection
+//   K4w  scan_pq_wide     64 < M <= 128: table built in shared memory + scan (dfx_scan_pq_wide_dev.cuh)
 //   K2/5 scan_rows        inverted-list scan of fp32 rows / fp16 / 8-bit residual codes
 //   K6   merge            cross-shard merge (float_maxheap_array_t semantics)
 // Arithmetic orders are the canonical ones of oracle/dfx_oracle.c (bit-exact parity).
@@ -194,6 +195,7 @@ void dfx_launch_select_comp(const uint64_t* comp, int64_t nrows, int n, int64_t 
 }
 
 #include "dfx_pq_prep_dev.cuh"
+#include "dfx_scan_pq_wide_dev.cuh"
 
 // =====================================================================================
 // K4: scan_pq.  one CTA = (query, group of G consecutive probes).  lane-per-vector:
@@ -730,6 +732,24 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
     const int KP = dfx_next_pow2(k < 32 ? 32 : k);
     const int cap = 2 * KP;
 
+    // IVF-PQ with 64 < M <= 128 (scan_pq_wide_kernel): the widest CTA whose table and per-warp
+    // queues fit in the device's shared memory, decided before anything is launched
+    int wide_threads = 0;
+    if (kind == DFX_IVF_PQ && idx->M > 64) {
+        const size_t optin = (size_t)dfx_smem_optin();
+        for (int t : {512, 256, 128}) {
+            if (dfx_pq_wide_smem(idx->M, t, cap) <= optin) {
+                wide_threads = t;
+                break;
+            }
+        }
+        DFX_REQUIRE(wide_threads > 0,
+                    "IVF-PQ with " + std::to_string(idx->M) + " sub-quantizers at k=" + std::to_string(k) +
+                        ": the distance table and the candidate queues need " +
+                        std::to_string(dfx_pq_wide_smem(idx->M, 128, cap)) +
+                        " bytes of shared memory per thread block, the device allows " + std::to_string(optin));
+    }
+
     idx->w_keys.reserve((size_t)nq * nprobe * 4);
     int32_t* keys_all = idx->w_keys.as<int32_t>();
 
@@ -769,6 +789,32 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
             // group per query it also writes the final rows (dfx_scan_il2.cu)
             final_written = dfx_launch_scan_pq_il2(idx, xq, qc, keys, nprobe, G, ngroups, k, cap, part, d_D + q0 * k,
                                                    d_I + q0 * k, st);
+        } else if (kind == DFX_IVF_PQ && idx->M > 64) {
+            // 64 < M <= 128: the scan kernel builds the query's table in its own shared memory, so
+            // only |q - c|^2 of the probed lists is prepared here (no w_lut)
+            const int M = idx->M;
+            idx->w_dis0.reserve((size_t)qc * nprobe * 4);
+            const size_t prep_smem = (size_t)((d + 3) / 4) * 16;
+            DFX_LAUNCH(pq_prep_kernel, (unsigned)qc, 256, prep_smem, st, xq, d, M, idx->ksub, idx->dsub,
+                       idx->codebooks.as<float>(), idx->centroids.as<float>(), keys, nprobe, (float*)nullptr,
+                       idx->w_dis0.as<float>());
+            const size_t smem = dfx_pq_wide_smem(M, wide_threads, cap);
+#define DFX_SCAN_PQ_WIDE(MT)                                                                     \
+    do {                                                                                         \
+        auto kern = (wide_threads == 512)   ? scan_pq_wide_kernel<MT, 512>                       \
+                    : (wide_threads == 256) ? scan_pq_wide_kernel<MT, 256>                       \
+                                            : scan_pq_wide_kernel<MT, 128>;                      \
+        DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,         \
+                                      (int)smem));                                               \
+        DFX_LAUNCH(kern, (unsigned)(qc * ngroups), wide_threads, smem, st, xq, d, M, idx->dsub,  \
+                   idx->codebooks.as<float>(), idx->w_dis0.as<float>(), keys, nprobe, G, ngroups, \
+                   idx->list_off.as<int64_t>(), idx->payload.as<uint8_t>(), idx->tvals.as<float>(), \
+                   idx->ids.as<int32_t>(), k, cap, part);                                        \
+    } while (0)
+            if (M == 128) DFX_SCAN_PQ_WIDE(128);
+            else if (M == 96) DFX_SCAN_PQ_WIDE(96);
+            else DFX_SCAN_PQ_WIDE(0);  // any other M % 4 == 0: 32-bit code loads
+#undef DFX_SCAN_PQ_WIDE
         } else if (kind == DFX_IVF_PQ) {
             const int M = idx->M, ksub = idx->ksub;
             idx->w_lut.reserve((size_t)qc * M * ksub * 4);

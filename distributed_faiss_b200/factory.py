@@ -10,7 +10,8 @@ an oracle-backed engine.
 Tokens are case-sensitive, as in faiss:
   "Flat"                          -> flat      (IndexFlat, the given metric)
   "IVF{n},Flat"                   -> ivf_flat  (IndexIVFFlat, the given metric)
-  "IVF{n},PQ{M}" / "IVF{n},PQ{M}x8" -> ivf_pq  (IndexIVFPQ, 8-bit codes, L2 only)
+  "IVF{n},PQ{M}" / "IVF{n},PQ{M}x8" -> ivf_pq  (IndexIVFPQ, 8-bit codes, L2 only; M a multiple of 4,
+                                              at most 128, that divides d)
   "IVF{n},SQfp16"                 -> ivf_sq    (IndexIVFScalarQuantizer QT_fp16, L2 only)
   "IVF{n},SQ8"                    -> ivf_sq8   (IndexIVFScalarQuantizer QT_8bit, L2 only)
 Everything else (OPQ / PCA prefixes, HNSW, IVF{n}_HNSW quantizers, RFlat / Refine, IDMap, PQ{M}x4,
@@ -24,7 +25,9 @@ METRIC_INNER_PRODUCT, METRIC_L2 = 0, 1  # faiss enum values
 ACCEPTED_FORMS = ("Flat", "IVF{n},Flat", "IVF{n},PQ{M}", "IVF{n},PQ{M}x8", "IVF{n},SQfp16", "IVF{n},SQ8")
 
 _IVF = re.compile(r"IVF([1-9][0-9]*),(Flat|PQ([1-9][0-9]*)(x8)?|SQfp16|SQ8)")
-_PQ_M_MAX = 64  # the IVF-PQ scan keeps at most 64 table values per vector
+# one query's fp32 PQ distance table (M x 256 x 4 bytes) must fit in one thread block's shared memory
+# (128 KB at M = 128); more would need split or fp16 tables, which are not bit-exact
+_PQ_M_MAX = 128
 
 
 class FactorySpec(NamedTuple):
@@ -67,8 +70,10 @@ def parse_factory(dim: int, factory_string: str, metric: int) -> FactorySpec:
     if codec.startswith("PQ"):
         M = int(m.group(3))
         if M % 4 != 0 or M > _PQ_M_MAX or dim % M != 0:
+            why = (" (one query's fp32 distance table, M x 256 x 4 bytes, must fit in one thread block's shared "
+                   "memory)") if M > _PQ_M_MAX else ""
             raise RuntimeError(
                 f"faiss_factory {factory_string!r}: the number of PQ sub-quantizers must be a multiple of 4, "
-                f"at most {_PQ_M_MAX}, that divides d={dim}")
+                f"at most {_PQ_M_MAX}, that divides d={dim}{why}")
         return FactorySpec("ivf_pq", int(metric), nlist, M)
     return FactorySpec("ivf_sq" if codec == "SQfp16" else "ivf_sq8", int(metric), nlist)

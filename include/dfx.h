@@ -54,7 +54,9 @@ typedef struct dfx_cfg {
                          the coarse quantizer only -- the reference never forwards it to the
                          index, which is therefore always L2 (index.py:44-46, 64-66). */
     int32_t d;        /* vector dimension (cfg.dim) */
-    int32_t pq_m;     /* IVF_PQ: sub-quantizers  (cfg.extra["code_size"], index.py:44) */
+    int32_t pq_m;     /* IVF_PQ: sub-quantizers  (cfg.extra["code_size"], index.py:44); 4 <= M <= 128,
+                         M % 4 == 0, d % M == 0.  128: one query's fp32 table (M x 256 x 4 B) must
+                         fit in one thread block's shared memory */
     int32_t pq_nbits; /* IVF_PQ: bits per code   (cfg.extra["bits_per_vector"], index.py:45) */
     int32_t device;   /* CUDA device ordinal this shard lives on */
     int64_t nlist;    /* IVF_*: number of inverted lists (cfg.centroids); IVF kinds need d % 4 == 0 */
