@@ -205,6 +205,7 @@ int dfx_get_param(dfx_index* idx, const char* name, double* value) {
     else if (n == "il2_threads") *value = idx->il2_threads;
     else if (n == "il2_prefetch") *value = idx->il2_prefetch;
     else if (n == "rows_inflight") *value = idx->rows_inflight;
+    else if (n == "workspace_bytes") *value = (double)idx->w_part.cap;  // read-only
     else throw DfxError{"unknown parameter " + n};
     DFX_API_END
 }

@@ -3,11 +3,15 @@
 #include "dfx_scan_il2_dev.cuh"
 #include <cstdlib>
 
+// dynamic shared memory of one CTA: the query's table + one queue (REG) or WarpTopK buffer per warp
+static size_t il2_smem(bool reg, int threads, int cap) {
+    return (size_t)IL2_LUT_BYTES + (size_t)(threads / 32) * (reg ? IL2_QCAP : cap) * 8;
+}
+
 template <bool REG, int THREADS, int MINB>
 static void launch_il2_t(dfx_index* idx, const float* xq, int64_t qc, const int32_t* keys, int nprobe, int G,
                        int ngroups, int k, int cap, uint64_t* part, float* outD, int64_t* outI, cudaStream_t st) {
-    constexpr int NW = THREADS / 32;
-    const size_t smem = (size_t)IL2_LUT_BYTES + (REG ? (size_t)NW * IL2_QCAP * 8 : (size_t)NW * cap * 8);
+    const size_t smem = il2_smem(REG, THREADS, cap);
     auto kern = scan_pq_il2_kernel<REG, THREADS, MINB>;
     DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, 100));
@@ -25,7 +29,9 @@ static void launch_il2_t(dfx_index* idx, const float* xq, int64_t qc, const int3
 }
 
 // CTA shape: 256 threads x 3 CTAs per SM (default) or, DFX_IL2_THREADS=512, 512 threads x 2 CTAs
-// (16 warps share one query's table: 32 instead of 24 warps per SM, half the table builds per SM)
+// (16 warps share one query's table: 32 instead of 24 warps per SM, half the table builds per SM).
+// 512 threads at k > 512 would need 16 buffers of cap = 2048 composites (320 KB): more than one CTA
+// may opt in to, so those searches take the 256-thread shape.
 template <bool REG>
 static void launch_il2(dfx_index* idx, const float* xq, int64_t qc, const int32_t* keys, int nprobe, int G,
                        int ngroups, int k, int cap, uint64_t* part, float* outD, int64_t* outI, cudaStream_t st) {
@@ -34,7 +40,7 @@ static void launch_il2(dfx_index* idx, const float* xq, int64_t qc, const int32_
         return e ? atoi(e) : IL2_THREADS;
     }();
     const int threads = idx->il2_threads ? idx->il2_threads : threads_default;
-    if (threads == 512) launch_il2_t<REG, 512, 2>(idx, xq, qc, keys, nprobe, G, ngroups, k, cap, part, outD, outI, st);
+    if (threads == 512 && il2_smem(REG, 512, cap) <= (size_t)dfx_smem_optin()) launch_il2_t<REG, 512, 2>(idx, xq, qc, keys, nprobe, G, ngroups, k, cap, part, outD, outI, st);
     else launch_il2_t<REG, 256, 3>(idx, xq, qc, keys, nprobe, G, ngroups, k, cap, part, outD, outI, st);
 }
 

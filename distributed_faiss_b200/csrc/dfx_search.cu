@@ -728,6 +728,16 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
     int64_t QC = use_tc ? 8192 : (32ll << 20) / nlist;
     if (QC < 1) QC = 1;
     if (QC > 8192) QC = 8192;
+    // the chunk's partial results (qc x ngroups x k composites) stay within the values matrix's
+    // 128 MiB: cap QC against ngroups <= nprobe, then once more against the ngroups choose_group
+    // gives at that cap (choose_group never gives a larger chunk more groups per query)
+    const int64_t part_max = (int64_t)1 << 24;
+    const int64_t q1 = std::max<int64_t>(1, part_max / ((int64_t)nprobe * k));
+    if (QC > q1) {
+        const int G1 = choose_group(q1, nprobe);
+        const int64_t ng1 = (nprobe + G1 - 1) / G1;
+        QC = std::min(QC, std::max(q1, part_max / (ng1 * k)));
+    }
     if (QC > nq) QC = nq;
     const int KP = dfx_next_pow2(k < 32 ? 32 : k);
     const int cap = 2 * KP;

@@ -86,14 +86,16 @@ int dfx_add_dev(dfx_index *idx, int64_t n, const float *d_x, void *stream);
  * "interleaved" (1): 0 keeps IVF-PQ (M = 32) codes row-major (one vector per lane, table from
  *   pq_prep_kernel) instead of the block-interleaved layout of the fused table-build + scan;
  * "il2_threads" (0 = 256) / "il2_prefetch" (-1 = 4 blocks): CTA shape and L2 prefetch distance of
- *   that scan (tuning);
+ *   that scan (tuning; 512 threads at k > 512 do not fit in shared memory and run with 256);
  * "rows_inflight" (0 = by row size): 4 or 8 vectors per warp in flight in the IVF-Flat / IVF-SQ
  *   list scan */
 int dfx_set_param(dfx_index *idx, const char *name, double value);
 /* read back a knob or a counter: the names of dfx_set_param, plus "tc_fast" (the precision the
  * next screening launch will use: 1 = FAST), "tc_stat_rows" / "tc_stat_overflow" /
  * "tc_stat_fast_would" (rows, rows re-done exactly, and rows FAST would have re-done, of the last
- * launch whose statistics came back; synchronises with that launch) */
+ * launch whose statistics came back; synchronises with that launch), "workspace_bytes" (bytes of
+ * the partial-result workspace, the largest any search so far has needed; IVF searches keep it
+ * within 128 MiB by their query chunk) */
 int dfx_get_param(dfx_index *idx, const char *name, double *value);
 /* pre-size the shard for n_total vectors (optional; avoids regrowth while bulk loading) */
 int dfx_reserve(dfx_index *idx, int64_t n_total);
