@@ -84,6 +84,20 @@ const char* dfx_last_error(void) { return g_last_error.c_str(); }
 const char* dfx_version(void) { return "dfx 0.2 (sm_90a) dfx-src-sha256=" DFX_SRC_HASH; }
 int64_t dfx_launch_count(void) { return (int64_t)g_dfx_launches.load(); }
 int dfx_debug_il_byte(int layout, int v, int m) { return dfx_il_byte_of(layout, v & 31, m & 31); }
+int dfx_debug_tc_screen(dfx_index* idx, int64_t nq, const float* d_x, int npl, float* d_gmin, float* d_gmin2,
+                        uint8_t* d_gargc) {
+    DFX_API_BEGIN
+    DFX_REQUIRE(idx && d_x && d_gmin && d_gmin2 && d_gargc, "null argument");
+    DFX_REQUIRE(nq >= 1, "nq must be >= 1");
+    DFX_REQUIRE(npl == 1 || npl == 2, "npl must be 1 (FAST) or 2 (PRECISE)");
+    DFX_REQUIRE(idx->cfg.kind != DFX_FLAT, "the screening table of an IVF index is its centroids");
+    std::lock_guard<std::mutex> lk(idx->mu);
+    DeviceGuard g(idx->cfg.device);
+    idx->join_dev();
+    dfx_tc_debug_screen(idx, nq, d_x, npl, d_gmin, d_gmin2, d_gargc, idx->stream);
+    DFX_CUDA(cudaStreamSynchronize(idx->stream));
+    DFX_API_END
+}
 
 int dfx_create(const dfx_cfg* cfg, dfx_index** out) {
     DFX_API_BEGIN

@@ -199,6 +199,8 @@ void dfx_tc_prepare_centroids(dfx_index* idx, cudaStream_t st);
 void dfx_tc_coarse_search(dfx_index* idx, const float* d_x, int64_t nq, int nprobe, int32_t* keys,
                           cudaStream_t st);
 int dfx_tc_flat_candidates(dfx_index* idx, const float* d_x, int64_t nq, int k, cudaStream_t st);
+void dfx_tc_debug_screen(dfx_index* idx, int64_t nq, const float* d_x, int npl, float* gmin, float* gmin2,
+                         uint8_t* gargc, cudaStream_t st);
 void dfx_tc_assign(dfx_index* idx, int d, const float* d_cent, const float* d_cnorm, int64_t nlist, int metric,
                    int64_t n, const float* d_x, int32_t* d_assign, cudaStream_t st);
 

@@ -136,16 +136,21 @@ constexpr int MAX_RESIDENT_KATOMS = 4;  // query tile resident in shared memory 
 //   PRECISE NPL 2: hi = fp16(x s), lo = fp16(x s - hi); q.c ~= qh.ch + ql.ch + qh.cl, three MMAs per
 //           k-step; error <= |q||c| 2^-17 (the dropped ql.cl term is 2^-22, hi + lo carries 22 bits)
 // shared-memory plan (offsets inside the 1024-aligned dynamic block)
-//   resident A (NPL x katoms <= 4): A = NPL x katoms x 16 KB, then a ring of 4 B stages of 16 KB
-//                          (FAST d <= 128: 97 KB, two CTAs per SM)
+//   resident A (NPL x katoms <= 4): A = NPL x katoms x 16 KB, then a ring of B stages of 16 KB that
+//                          holds two tiles, at least 4 stages (FAST d <= 128: <= 99 KB, two CTAs per
+//                          SM; PRECISE d = 128 and FAST d = 256: 8 stages, 195 KB); the warpgroups run
+//                          a tile apart, and the one behind still reads the stages of the tile before
 //   streamed A (larger d): a ring of 6 stages of (A atom + B atom) = 32 KB
+//   then 512 B of mbarriers and each warpgroup's copy of the tile's ranking offsets, [2][2][TILE] floats
 struct Smem {
     static constexpr bool resident(int katoms, int npl) { return npl * katoms <= MAX_RESIDENT_KATOMS; }
-    static constexpr int nstage(bool res) { return res ? 4 : 6; }
+    static constexpr int nstage(bool res, int katoms, int npl) {
+        return !res ? 6 : (2 * npl * katoms > 4 ? 2 * npl * katoms : 4);
+    }
     static constexpr int stage_bytes(bool res) { return res ? ATOM_BYTES : 2 * ATOM_BYTES; }
     static constexpr int RING(bool res, int katoms, int npl) { return res ? npl * katoms * ATOM_BYTES : 0; }
-    static constexpr int BARS(bool res, int katoms, int npl) { return RING(res, katoms, npl) + nstage(res) * stage_bytes(res); }
-    static constexpr int total(bool res, int katoms, int npl) { return BARS(res, katoms, npl) + 512 + 2 * TILE * 4; }
+    static constexpr int BARS(bool res, int katoms, int npl) { return RING(res, katoms, npl) + nstage(res, katoms, npl) * stage_bytes(res); }
+    static constexpr int total(bool res, int katoms, int npl) { return BARS(res, katoms, npl) + 512 + 4 * TILE * 4; }
     // CTAs that fit one SM (228 KB of shared memory): two when a CTA's block (+ 1 KB for the
     // alignment) stays within 113 KB, which only FAST shapes reach
     static constexpr int ctas_per_sm(bool res, int katoms, int npl) {
@@ -267,7 +272,7 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     using namespace tc;
     constexpr bool RES = KT != 0;
     const int KATOMS = KT ? KT : katoms_rt;
-    constexpr int NSTAGE = Smem::nstage(RES);
+    constexpr int NSTAGE = Smem::nstage(RES, KT, NPL);
     constexpr int STAGE_BYTES = Smem::stage_bytes(RES);
     constexpr int TN = TILE;  // centroids per tile
     // operand pairs accumulated per k-atom: FAST (qh, ch); PRECISE (qh, ch), (ql, ch), (qh, cl)
@@ -281,7 +286,7 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     uint64_t* full = bars;                 // [NSTAGE]
     uint64_t* empty = bars + NSTAGE;       // [NSTAGE]
     uint64_t* a_full = bars + 2 * NSTAGE;  // [1]
-    float* s_cn = reinterpret_cast<float*>(smem + Smem::BARS(RES, KATOMS, NPL) + 512);  // [2][TN]
+    float* s_cn = reinterpret_cast<float*>(smem + Smem::BARS(RES, KATOMS, NPL) + 512);  // [warpgroup][2][TN]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int qt = blockIdx.y;
@@ -363,15 +368,22 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         __syncwarp();
         if (lane == 0) mbar_arrive(&empty[s]);  // this warp's MMAs have read stage s
     };
+    // Resident shapes: the two warpgroups run out of phase -- while one turns its accumulator into
+    // the summary, the other's MMAs keep the tensor cores busy.  The turn to issue a tile's MMAs
+    // passes back and forth through named barriers 2 (warpgroup 0 waits, from its second tile on)
+    // and 3 (warpgroup 1 waits), so the MMAs of the two never interleave.  The streamed ring holds
+    // less than a tile: there both warpgroups issue together.
     for (int t = 0; t < ntiles; t++) {
         const int buf = t & 1;
         const int col0 = (ct0 + t) * TN;
-        if (threadIdx.x < TN) {
-            const int c = col0 + threadIdx.x;
-            float cn = 0.f;
-            if (METRIC == DFX_METRIC_L2 && c < nlist) cn = cnorm[c];
-            s_cn[buf * TN + threadIdx.x] = (c < nlist) ? cn : big;
+        // the ranking offset of column threadIdx.x % 128 of the tile: |c|^2 (L2) or 0 (IP), `big`
+        // past nlist; loaded now, shared through this warpgroup's copy once the MMAs are issued
+        float cn_own;
+        {
+            const int c = col0 + (threadIdx.x & (TN - 1));
+            cn_own = c < nlist ? (METRIC == DFX_METRIC_L2 ? cnorm[c] : 0.f) : big;
         }
+        if (RES && (wg == 1 || t > 0)) asm volatile("bar.sync %0, %1;" ::"r"(2 + wg), "n"(CONSUMERS) : "memory");
         int prev = -1;  // stage of the group still in flight
         for (int c = 0; c < (RES ? NPL : NCOMBO); c++)
         for (int ka = 0; ka < KATOMS; ka++) {
@@ -398,10 +410,15 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
                 phase ^= 1;
             }
         }
+        if (RES && (wg == 0 || t + 1 < ntiles))
+            asm volatile("bar.arrive %0, %1;" ::"r"(3 - wg), "n"(CONSUMERS) : "memory");
+        float* cn_wg = s_cn + (wg * 2 + buf) * TN;
+        cn_wg[threadIdx.x & (TN - 1)] = cn_own;
         wg_wait<0>();  // the accumulator is complete
         release(prev);
-        asm volatile("bar.sync 1, %0;" ::"n"(CONSUMERS) : "memory");  // s_cn of this tile written
-        const float* cn = s_cn + buf * TN + 2 * quad;
+        // this warpgroup's offsets written (its copy of tile t - 2 was read before tile t - 1's barrier)
+        asm volatile("bar.sync %0, %1;" ::"r"(4 + wg), "n"(CONSUMERS / 2) : "memory");
+        const float* cn = cn_wg + 2 * quad;
         float gm[2][4], gm2[2][4];
         uint32_t ga[2] = {0u, 0u};
 #pragma unroll
@@ -1161,6 +1178,19 @@ static Screened tc_screen_chunk(dfx_index* idx, int d, const float* d_x, int64_t
     DFX_CUDA(cudaMemsetAsync(idx->tc_ovf.p, 0, 8, st));
     return {gmin, idx->tc_gmin2.as<float>(), idx->tc_gargc.as<uint8_t>(), idx->tc_groups.as<int32_t>(),
             idx->tc_ovf.as<int32_t>()};
+}
+
+// the screening summary alone (dfx_debug_tc_screen): gmin / gmin2 float [nq][ng] and gargc u8
+// [nq][ng], ng = ceil(nlist / 128) * 4, of nq device queries against the index's centroid table,
+// at npl planes (1 FAST, 2 PRECISE)
+void dfx_tc_debug_screen(dfx_index* idx, int64_t nq, const float* d_x, int npl, float* gmin, float* gmin2,
+                         uint8_t* gargc, cudaStream_t st) {
+    DFX_REQUIRE(idx->tc_ready, "the index has no tensor-core screening table (untrained, or d not a multiple of 64)");
+    const int64_t nlist = idx->cfg.nlist;
+    const int ng = (int)(dfx_ceil_div(nlist, tc::TILE) * tc::TILE / 32);
+    idx->tc_tmin.reserve((size_t)nq * (ng / 4) * 4);
+    tc_screen(idx, idx->cfg.d, d_x, nq, idx->tc_cent.p, idx->tc_cscale, npl, idx->cnorm.as<float>(), nlist,
+              idx->cfg.metric, gmin, gmin2, gargc, idx->tc_tmin.as<float>(), st);
 }
 
 // top-nprobe lists per query -> keys int32 [nq, nprobe] (exactly the oracle's coarse result)

@@ -36,7 +36,7 @@ EXPORTED_SYMBOLS = [
     "dfx_merge_dev", "dfx_merge_packed_dev", "dfx_encode_ids_dev", "dfx_filter_compact_dev",
     "dfx_reconstruct_dev", "dfx_map_ids_dev", "dfx_get_array", "dfx_set_array", "dfx_import_done",
     "dfx_last_stats", "dfx_profile_enable", "dfx_profile_read", "dfx_launch_count", "dfx_synth_init", "dfx_synth_rows_dev", "dfx_free",
-    "dfx_last_error", "dfx_version", "dfx_debug_il_byte",
+    "dfx_last_error", "dfx_version", "dfx_debug_il_byte", "dfx_debug_tc_screen",
 ]
 
 

@@ -226,6 +226,13 @@ const char *dfx_version(void);
 /* byte offset, inside a 1 KB block of 32 IVF-PQ vectors, of subquantizer m of vector v for block
  * layout 1 or 2 (host function; lets the layout be checked without a GPU) */
 int dfx_debug_il_byte(int layout, int v, int m);
+/* the coarse quantizer's tensor-core screening summary of nq device queries d_x [nq, d] against
+ * the centroids of a trained IVF index (d a multiple of 64), at npl = 1 (FAST) or 2 (PRECISE)
+ * fp16 planes: per query and group of 32 centroids, the smallest ranking value with the winning
+ * column (0..31) in its 5 low bits (d_gmin), the runner-up (d_gmin2) and that column (d_gargc);
+ * device arrays of [nq][ceil(nlist / 128) * 4].  Synchronises. */
+int dfx_debug_tc_screen(dfx_index *idx, int64_t nq, const float *d_x, int npl, float *d_gmin, float *d_gmin2,
+                        uint8_t *d_gargc);
 
 #ifdef __cplusplus
 }

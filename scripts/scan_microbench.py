@@ -1,10 +1,12 @@
 #!/usr/bin/env python
-"""One shard of the bench workload (125 M vectors of the 1 B, nlist 65 536), batch 4096, nprobe 8:
+"""One shard of the bench workload (62.5 M vectors of the 500 M, nlist 65 536), batch 4096, nprobe 8:
 per-launch time of the fused table-build + scan kernel and of the whole shard search, for the
-kernel knobs currently in the environment (DFX_IL2_PREFETCH ...).  ~40 s per run.
+kernel knobs currently in the environment (DFX_IL2_PREFETCH ...), then a per-kernel breakdown of
+one shard search from torch.profiler (MB_PROFILE=0 skips it).  ~60 s per run.
     python scripts/scan_microbench.py [label]"""
 import json
 import os
+import subprocess
 import sys
 import time
 
@@ -23,9 +25,78 @@ class A:
     train_pts = 64
 
 
+# the kernels of one IVF-PQ shard search, in launch order
+BREAKDOWN_KERNELS = ("f16_rows_kernel", "tc_coarse_kernel", "topg_collect_kernel", "rerank2_kernel",
+                     "tc_exact_rows_kernel", "scan_pq_il2_kernel")
+TC_PEAK_TFLOPS = 989.0  # H100 SXM data sheet, dense fp16 with fp32 accumulation
+
+
+def card_info():
+    """name, power limit and maximum SM clock of the card (a read-only query)."""
+    try:
+        r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader",
+                            "-i", str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30)
+        return r.stdout.strip()
+    except (OSError, subprocess.SubprocessError) as e:
+        return f"nvidia-smi failed: {e}"
+
+
+def kernel_breakdown(idx, batch, k, iters=20):
+    """Per-kernel device time of `iters` shard searches of `batch` (torch.profiler, CUDA activities),
+    against the search's own time measured with the profiler off, and the SM clock sampled while
+    the searches ran.  K1 (tc_coarse_kernel) also gets its algorithmic rate 2 nq_pad nl_pad d and
+    its MMA rate (x3 for PRECISE: three products per k-step)."""
+    from torch.profiler import ProfilerActivity, profile
+
+    for _ in range(3):
+        idx.search_dev(batch, k)
+    torch.cuda.synchronize()
+    clocks = bench.ClockSampler(torch.cuda.current_device())
+    clocks.start()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(iters):
+        idx.search_dev(batch, k)
+    e1.record()
+    torch.cuda.synchronize()
+    search_us = e0.elapsed_time(e1) * 1e3 / iters
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(iters):
+            idx.search_dev(batch, k)
+        torch.cuda.synchronize()
+    clk = clocks.stop()
+    per = {}
+    for ev in prof.key_averages():
+        name = next((kn for kn in BREAKDOWN_KERNELS if kn in ev.key), None)
+        if name is None or ev.device_time_total <= 0:
+            continue
+        p = per.setdefault(name, {"launches": 0, "total_us": 0.0})
+        p["launches"] += ev.count
+        p["total_us"] += ev.device_time_total
+    out = {"search_us": search_us, "sm_clock": clk, "kernels": {}}
+    for name in BREAKDOWN_KERNELS:
+        p = per.get(name, {"launches": 0, "total_us": 0.0})
+        launches_per_search = p["launches"] / iters
+        us_search = p["total_us"] / iters
+        out["kernels"][name] = {"us_per_launch": p["total_us"] / p["launches"] if p["launches"] else 0.0,
+                                "launches_per_search": launches_per_search, "us_per_search": us_search,
+                                "share_of_search": us_search / search_us}
+    k1 = out["kernels"]["tc_coarse_kernel"]
+    if k1["launches_per_search"]:
+        nq_pad = -(-batch.shape[0] // 128) * 128
+        nl_pad = -(-idx.nlist // 128) * 128
+        flop = 2.0 * nq_pad * nl_pad * batch.shape[1] * k1["launches_per_search"]
+        products = 1 if idx.get_param("tc_fast") else 3
+        t = k1["us_per_search"] * 1e-6
+        k1["algorithmic_tflops"] = flop / t / 1e12
+        k1["mma_tflops"] = products * flop / t / 1e12
+        k1["mma_frac_of_989"] = k1["mma_tflops"] / TC_PEAK_TFLOPS
+    return out
+
+
 def main():
     label = sys.argv[1] if len(sys.argv) > 1 else "default"
-    nvec = int(os.environ.get("MB_NVEC", 1_000_000_000))
+    nvec = int(os.environ.get("MB_NVEC", 500_000_000))
     G = nvec // 10
     synth = engine.Synth(1234, bench.D, 16, 1, 1.0, 0.02, ngroups=G, eps=0.01, delta=0.1)
     idx, tab, info = bench.build_shard(engine, synth, nvec, 0, A, torch, None)
@@ -117,6 +188,10 @@ def main():
                                  "coarse_ms": e0.elapsed_time(e1) / 12 - ms / nl,
                                  "same": bool(torch.equal(Dm, ref[0]) and torch.equal(Im, ref[1])),
                                  **{k: idx.get_param(k) for k in stat_names}}
+    if os.environ.get("MB_PROFILE", "1") != "0":  # AUTO, as left by the loop above
+        out["card"] = card_info()
+        out["breakdown"] = kernel_breakdown(idx, batches[0], 10)
+        out["breakdown"]["auto_state"] = {k: idx.get_param(k) for k in stat_names}
     print(json.dumps(out))
 
 
