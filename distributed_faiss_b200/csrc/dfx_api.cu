@@ -114,15 +114,25 @@ int dfx_create(const dfx_cfg* cfg, dfx_index** out) {
         DFX_REQUIRE(cfg->d % 4 == 0, "IVF indexes need a dimension that is a multiple of 4");
     }
     if (cfg->kind == DFX_IVF_PQ) {
-        DFX_REQUIRE(cfg->pq_nbits == 8, "IVF-PQ: only 8 bits per sub-quantizer are supported");
-        DFX_REQUIRE(cfg->pq_m >= 4 && cfg->pq_m % 4 == 0 && cfg->d % cfg->pq_m == 0,
-                    "IVF-PQ: the number of sub-quantizers must be a multiple of 4 that divides d");
-        DFX_REQUIRE(cfg->pq_m <= 128,
-                    "IVF-PQ: at most 128 sub-quantizers are supported (one query's fp32 distance table, "
-                    "M x 256 x 4 bytes, must fit in one thread block's shared memory; more would need split "
-                    "or fp16 tables, which are not bit-exact)");
+        DFX_REQUIRE(cfg->pq_nbits == 8 || cfg->pq_nbits == 4,
+                    "IVF-PQ: 8 or 4 bits per sub-quantizer are supported, got " + std::to_string(cfg->pq_nbits));
+        if (cfg->pq_nbits == 8) {
+            DFX_REQUIRE(cfg->pq_m >= 4 && cfg->pq_m % 4 == 0 && cfg->d % cfg->pq_m == 0,
+                        "IVF-PQ: the number of sub-quantizers must be a multiple of 4 that divides d");
+            DFX_REQUIRE(cfg->pq_m <= 128,
+                        "IVF-PQ: at most 128 sub-quantizers are supported (one query's fp32 distance table, "
+                        "M x 256 x 4 bytes, must fit in one thread block's shared memory; more would need split "
+                        "or fp16 tables, which are not bit-exact)");
+        } else {
+            // a packed row (M / 2 bytes) is whole 32-bit words, and the scan's register table
+            // (M / 2 floats per lane) stays within 64 registers
+            DFX_REQUIRE(cfg->pq_m >= 8 && cfg->pq_m <= 128 && cfg->pq_m % 8 == 0 && cfg->d % cfg->pq_m == 0,
+                        "IVF-PQ with 4-bit codes: the number of sub-quantizers must be a multiple of 8 in "
+                        "[8, 128] that divides d, got M=" + std::to_string(cfg->pq_m) + ", d=" +
+                            std::to_string(cfg->d));
+        }
         idx->M = cfg->pq_m;
-        idx->ksub = 256;
+        idx->ksub = 1 << cfg->pq_nbits;
         idx->dsub = cfg->d / cfg->pq_m;
     }
     DeviceGuard g(cfg->device);
@@ -500,19 +510,30 @@ int dfx_get_array(dfx_index* idx, const char* name, void* out, int64_t max_bytes
     const void* src = nullptr;
     int64_t bytes = 0;
     bool widen_ids = false;
+    // 4-bit IVF-PQ codes are stored packed (two per byte) and exchanged one code per byte
+    const bool unpack4 = n == "codes" && idx->cfg.kind == DFX_IVF_PQ && idx->ksub == 16;
     if (n == "centroids" && idx->is_ivf() && idx->trained) { src = idx->centroids.p; bytes = nlist * d * 4; }
     else if (n == "codebooks" && idx->cfg.kind == DFX_IVF_PQ && idx->trained) { src = idx->codebooks.p; bytes = (int64_t)idx->M * idx->ksub * idx->dsub * 4; }
     else if (n == "sq_trained" && idx->cfg.kind == DFX_IVF_SQ8 && idx->trained) { src = idx->sq_trained.p; bytes = 2 * d * 4; }
     else if (n == "list_off" && idx->is_ivf() && idx->trained) { src = idx->list_off.p; bytes = (nlist + 1) * 8; }
     else if (n == "ids" && idx->is_ivf()) { widen_ids = true; bytes = nt * 8; }
     else if (n == "tvals" && idx->cfg.kind == DFX_IVF_PQ) { src = idx->tvals.p; bytes = nt * 4; }
+    else if (unpack4) { bytes = nt * idx->M; }
     else if (n == payload_name(idx->cfg.kind)) { src = idx->payload.p; bytes = nt * (int64_t)idx->row_bytes(); }
     else throw DfxError{"no array named '" + n + "' in this index"};
     if (nbytes) *nbytes = bytes;
     if (!out) return 0;
     DFX_REQUIRE(max_bytes >= bytes, "output buffer too small for '" + n + "'");
     if (bytes == 0) return 0;
-    if (widen_ids) {
+    if (unpack4) {
+        std::vector<uint8_t> packed((size_t)bytes / 2);
+        DFX_CUDA(cudaMemcpy(packed.data(), idx->payload.p, packed.size(), cudaMemcpyDeviceToHost));
+        uint8_t* o = (uint8_t*)out;
+        for (size_t b = 0; b < packed.size(); b++) {  // M is even: byte b holds codes 2b and 2b + 1
+            o[2 * b] = packed[b] & 15;
+            o[2 * b + 1] = packed[b] >> 4;
+        }
+    } else if (widen_ids) {
         std::vector<int32_t> tmp((size_t)nt);
         DFX_CUDA(cudaMemcpy(tmp.data(), idx->ids.p, (size_t)nt * 4, cudaMemcpyDeviceToHost));
         int64_t* o = (int64_t*)out;
@@ -578,6 +599,18 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
                 dfx_launch_row_norms(idx->payload.as<float>(), idx->n_sorted, (int)d, idx->xnorm.as<float>(), idx->stream);
                 DFX_CUDA(cudaStreamSynchronize(idx->stream));
             }
+        } else if (idx->cfg.kind == DFX_IVF_PQ && idx->ksub == 16) {
+            DFX_REQUIRE(nbytes == idx->n_sorted * (int64_t)idx->M,
+                        "codes: wrong size (one byte per code, u8[ntotal, M]; set list_off first)");
+            const uint8_t* s = (const uint8_t*)in;
+            std::vector<uint8_t> packed((size_t)nbytes / 2);
+            for (size_t b = 0; b < packed.size(); b++) {
+                DFX_REQUIRE(s[2 * b] < 16 && s[2 * b + 1] < 16, "codes: a 4-bit code must be in [0, 16)");
+                packed[b] = (uint8_t)(s[2 * b] | (s[2 * b + 1] << 4));
+            }
+            idx->payload.reserve(std::max<size_t>(packed.size(), 4));
+            if (!packed.empty())
+                DFX_CUDA(cudaMemcpy(idx->payload.p, packed.data(), packed.size(), cudaMemcpyHostToDevice));
         } else {
             DFX_REQUIRE(nbytes == idx->n_sorted * (int64_t)idx->row_bytes(), "payload: wrong size (set list_off first)");
             upload(idx->payload, nbytes);

@@ -127,7 +127,16 @@ pq_encode_kernel(const float* __restrict__ x, const float* __restrict__ cent,
     codes[i * M + m] = (uint8_t)bj;
 }
 
-// tvals[i] = sum_m ( |p_m|^2 + 2 <c_m, p_m> ), sequential in m (oracle orc_pq_tvals)
+// 4-bit codes: u8[n][M] (one code per byte, from pq_encode_kernel) -> the packed rows u8[n][M / 2].
+// One thread per output byte, so no two threads write the same byte.
+__global__ void pq_pack4_kernel(const uint8_t* __restrict__ in, int64_t nbytes, uint8_t* __restrict__ out) {
+    int64_t b = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (b < nbytes) out[b] = (uint8_t)(in[2 * b] | (in[2 * b + 1] << 4));
+}
+
+// tvals[i] = sum_m ( |p_m|^2 + 2 <c_m, p_m> ), sequential in m (oracle orc_pq_tvals); NB = bits per
+// stored code (dfx_pq_code)
+template <int NB>
 __global__ void pq_tvals_kernel(const uint8_t* __restrict__ codes, const int32_t* __restrict__ list_of,
                                 const int64_t* __restrict__ list_off, int64_t nlist, int64_t n, int d,
                                 int M, int ksub, int dsub, const float* __restrict__ codebooks,
@@ -148,7 +157,7 @@ __global__ void pq_tvals_kernel(const uint8_t* __restrict__ codes, const int32_t
     const float* c = cent + (size_t)l * d;
     float t = 0.f;
     for (int m = 0; m < M; m++) {
-        const float* p = codebooks + ((size_t)m * ksub + codes[i * M + m]) * dsub;
+        const float* p = codebooks + ((size_t)m * ksub + dfx_pq_code<NB>(codes, i, M, m)) * dsub;
         float ipcp = 0.f, ippp = 0.f;
         for (int tt = 0; tt < dsub; tt++) ipcp = __fmaf_rn(c[m * dsub + tt], p[tt], ipcp);
         for (int tt = 0; tt < dsub; tt++) ippp = __fmaf_rn(p[tt], p[tt], ippp);
@@ -496,12 +505,20 @@ void dfx_add_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) 
         DFX_CUDA(cudaMemcpyAsync(prow, d_x, (size_t)n * rb, cudaMemcpyDeviceToDevice, st));
     } else if (kind == DFX_IVF_PQ) {
         const int M = idx->M, ksub = idx->ksub, dsub = idx->dsub;
+        // one code per byte first; 4-bit codes are packed afterwards (two sub-quantizers share a
+        // byte, so the per-sub-quantizer encode launch cannot write nibbles in place)
+        DevBuf unpacked;
+        uint8_t* enc = (uint8_t*)prow;
+        if (ksub == 16) {
+            unpacked.reserve((size_t)n * M);
+            enc = unpacked.as<uint8_t>();
+        }
         dim3 grid(blocks_for(n, 256), (unsigned)M);
 #define DFX_PQ_ENCODE(DS)                                                                       \
     do {                                                                                        \
         auto kern = pq_encode_kernel<DS>;                                                       \
         DFX_LAUNCH(kern, grid, 256, (size_t)ksub * dsub * 4, st, d_x, idx->centroids.as<float>(), \
-                   plist, n, d, M, ksub, dsub, idx->codebooks.as<float>(), (uint8_t*)prow);     \
+                   plist, n, d, M, ksub, dsub, idx->codebooks.as<float>(), enc);                \
     } while (0)
         if (dsub == 2) DFX_PQ_ENCODE(2);
         else if (dsub == 4) DFX_PQ_ENCODE(4);
@@ -510,9 +527,13 @@ void dfx_add_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) 
         else if (dsub == 16) DFX_PQ_ENCODE(16);
         else DFX_PQ_ENCODE(0);
 #undef DFX_PQ_ENCODE
-        DFX_LAUNCH(pq_tvals_kernel, blocks_for(n, 128), 128, 0, st, (const uint8_t*)prow, plist,
+        DFX_LAUNCH(pq_tvals_kernel<8>, blocks_for(n, 128), 128, 0, st, (const uint8_t*)enc, plist,
                    (const int64_t*)nullptr, nlist, n, d, M, ksub, dsub, idx->codebooks.as<float>(),
                    idx->centroids.as<float>(), idx->p_tvals.as<float>() + idx->n_pending);
+        if (ksub == 16)
+            DFX_LAUNCH(pq_pack4_kernel, blocks_for(n * M / 2, 256), 256, 0, st, (const uint8_t*)enc,
+                       n * M / 2, (uint8_t*)prow);
+        // (`unpacked` is freed on return: cudaFree waits for the kernels above)
     } else if (kind == DFX_IVF_SQ16) {
         DFX_LAUNCH(sq_encode_kernel, blocks_for(n * d, 256), 256, 0, st, d_x, idx->centroids.as<float>(),
                    plist, n, d, (__half*)prow);
@@ -527,7 +548,8 @@ void dfx_compute_tvals_sorted(dfx_index* idx, cudaStream_t st) {
     const int64_t n = idx->n_sorted;
     idx->tvals.reserve((size_t)std::max<int64_t>(n, 1) * 4);
     if (n == 0) return;
-    DFX_LAUNCH(pq_tvals_kernel, blocks_for(n, 128), 128, 0, st, idx->payload.as<uint8_t>(),
+    auto kern = (idx->ksub == 16) ? pq_tvals_kernel<4> : pq_tvals_kernel<8>;
+    DFX_LAUNCH(kern, blocks_for(n, 128), 128, 0, st, idx->payload.as<uint8_t>(),
                (const int32_t*)nullptr, idx->list_off.as<int64_t>(), idx->cfg.nlist, n, idx->cfg.d,
                idx->M, idx->ksub, idx->dsub, idx->codebooks.as<float>(), idx->centroids.as<float>(),
                idx->tvals.as<float>());
@@ -618,7 +640,9 @@ __global__ void invert_ids_kernel(const int32_t* __restrict__ ids, int64_t n, in
 }
 
 // il != 0 (IVF-PQ interleaved, il = block layout 1 or 2): `inv` holds padded block positions and
-// codes are read from the interleaved blocks (dfx_il_byte_of(il, pos%32, m) of block pos/32)
+// codes are read from the interleaved blocks (dfx_il_byte_of(il, pos%32, m) of block pos/32).
+// NB = bits per stored IVF-PQ code of the row-major form (dfx_pq_code).
+template <int NB>
 __global__ void reconstruct_kernel(int kind, int d, int M, int ksub, int dsub, int64_t ntotal,
                                    int64_t nlist, const int64_t* __restrict__ want,
                                    const int32_t* __restrict__ inv, const void* __restrict__ rows,
@@ -660,7 +684,7 @@ __global__ void reconstruct_kernel(int kind, int d, int M, int ksub, int dsub, i
             int m = k / dsub;
             int code;
             if (il) code = reinterpret_cast<const uint8_t*>(rows)[(pos >> 5) * 1024 + dfx_il_byte_of(il, (int)(pos & 31), m)];
-            else code = reinterpret_cast<const uint8_t*>(rows)[pos * M + m];
+            else code = dfx_pq_code<NB>(reinterpret_cast<const uint8_t*>(rows), pos, M, m);
             v = cent[(size_t)l * d + k] + codebooks[((size_t)m * ksub + code) * dsub + (k - m * dsub)];
         }
         out[r * d + k] = v;
@@ -715,7 +739,8 @@ void dfx_reconstruct_impl(dfx_index* idx, int64_t n, const int64_t* d_ids, float
                    idx->centroids.as<float>(), idx->sq_trained.as<float>(), d_out, tag);
         return;
     }
-    DFX_LAUNCH(reconstruct_kernel, (unsigned)n, 128, 0, st, idx->cfg.kind, idx->cfg.d, idx->M, idx->ksub,
+    auto kern = (idx->cfg.kind == DFX_IVF_PQ && idx->ksub == 16) ? reconstruct_kernel<4> : reconstruct_kernel<8>;
+    DFX_LAUNCH(kern, (unsigned)n, 128, 0, st, idx->cfg.kind, idx->cfg.d, idx->M, idx->ksub,
                idx->dsub, nt, idx->cfg.nlist, d_ids, idx->inv.as<int32_t>(),
                il ? (const void*)idx->il_codes.p : (const void*)idx->payload.p, idx->list_off.as<int64_t>(),
                idx->centroids.as<float>(), idx->codebooks.as<float>(), il, idx->blk_off.as<int64_t>(), d_out, tag);

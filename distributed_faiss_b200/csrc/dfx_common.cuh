@@ -172,6 +172,16 @@ __device__ __forceinline__ float dfx_rank_value(float ip, int metric, const floa
     return (metric == DFX_METRIC_IP) ? -ip : __fmaf_rn(-2.f, ip, xnorm[col]);
 }
 
+// code of sub-quantizer m of row i of IVF-PQ codes stored with NB bits per code: NB = 8, one byte
+// per code (u8[n][M]); NB = 4, packed as faiss does (u8[n][M / 2], code m in nibble m & 1 of byte
+// m >> 1, low nibble first)
+template <int NB>
+__device__ __forceinline__ int dfx_pq_code(const uint8_t* codes, int64_t i, int M, int m) {
+    static_assert(NB == 8 || NB == 4, "4 or 8 bits per code");
+    if constexpr (NB == 4) return (codes[i * (M / 2) + (m >> 1)] >> ((m & 1) * 4)) & 15;
+    else return codes[i * M + m];
+}
+
 static inline int64_t dfx_ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 static inline int dfx_next_pow2(int x) {
     int p = 1;

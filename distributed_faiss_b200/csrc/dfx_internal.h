@@ -130,7 +130,7 @@ struct dfx_index {
         switch (cfg.kind) {
             case DFX_FLAT:
             case DFX_IVF_FLAT: return (size_t)cfg.d * 4;
-            case DFX_IVF_PQ: return (size_t)M;
+            case DFX_IVF_PQ: return ksub == 16 ? (size_t)M / 2 : (size_t)M;  // 4-bit codes: two per byte
             case DFX_IVF_SQ16: return (size_t)cfg.d * 2;
             case DFX_IVF_SQ8: return (size_t)cfg.d;
         }

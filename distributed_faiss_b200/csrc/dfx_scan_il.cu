@@ -3,7 +3,8 @@
 #include "dfx_scan_il_dev.cuh"
 
 bool dfx_il_wanted(const dfx_index* idx) {
-    return idx->cfg.kind == DFX_IVF_PQ && idx->M == 32 && idx->il_enabled;
+    // the interleaved blocks hold one byte per code: 4-bit codes always stay row-major
+    return idx->cfg.kind == DFX_IVF_PQ && idx->M == 32 && idx->ksub == 256 && idx->il_enabled;
 }
 
 // payload/tvals/ids (row-major, list-sorted) -> il_* ; frees the row-major arrays

@@ -9,6 +9,7 @@
 //   K3   pq_prep          per-query PQ table  -2<q_m,P[m][j]>  + exact ||q-c||^2 of probed lists
 //   K4   scan_pq          inverted-list scan of PQ codes, per-warp k-selection
 //   K4w  scan_pq_wide     64 < M <= 128: table built in shared memory + scan (dfx_scan_pq_wide_dev.cuh)
+//   K4n  scan_pq4         4-bit codes: table in registers, lookups by warp shuffle (dfx_scan_pq4_dev.cuh)
 //   K2/5 scan_rows        inverted-list scan of fp32 rows / fp16 / 8-bit residual codes
 //   K6   merge            cross-shard merge (float_maxheap_array_t semantics)
 // Arithmetic orders are the canonical ones of oracle/dfx_oracle.c (bit-exact parity).
@@ -196,6 +197,28 @@ void dfx_launch_select_comp(const uint64_t* comp, int64_t nrows, int n, int64_t 
 
 #include "dfx_pq_prep_dev.cuh"
 #include "dfx_scan_pq_wide_dev.cuh"
+#include "dfx_scan_pq4_dev.cuh"
+
+// scan_pq4_kernel<M> for the runtime M (a multiple of 8 in [8, 128], checked by dfx_create)
+template <int MT = 8>
+static void dfx_launch_scan_pq4(int M, unsigned grid, size_t smem, cudaStream_t st, const float* lut,
+                                const float* dis0, const int32_t* keys, int nprobe, int G, int ngroups,
+                                const int64_t* list_off, const uint8_t* codes, const float* tvals,
+                                const int32_t* ids, int k, int cap, uint64_t* part) {
+    if constexpr (MT <= 128) {
+        if (M != MT) {
+            dfx_launch_scan_pq4<MT + 8>(M, grid, smem, st, lut, dis0, keys, nprobe, G, ngroups, list_off, codes,
+                                        tvals, ids, k, cap, part);
+            return;
+        }
+        auto kern = scan_pq4_kernel<MT>;
+        DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        DFX_LAUNCH(kern, grid, 128, smem, st, lut, dis0, keys, nprobe, G, ngroups, list_off, codes, tvals, ids, k,
+                   cap, part);
+    } else {
+        throw DfxError{"IVF-PQ with 4-bit codes: no list scan for M=" + std::to_string(M)};
+    }
+}
 
 // =====================================================================================
 // K4: scan_pq.  one CTA = (query, group of G consecutive probes).  lane-per-vector:
@@ -794,7 +817,20 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
         }
 
         bool final_written = false;
-        if (kind == DFX_IVF_PQ && idx->il) {
+        if (kind == DFX_IVF_PQ && idx->ksub == 16) {
+            // 4-bit codes: the [M][16] table of each query goes to registers (dfx_scan_pq4_dev.cuh)
+            const int M = idx->M;
+            idx->w_lut.reserve((size_t)qc * M * PQ4_KSUB * 4);
+            idx->w_dis0.reserve((size_t)qc * nprobe * 4);
+            const size_t prep_smem = (size_t)((d + 3) / 4) * 16;
+            DFX_LAUNCH(pq_prep_kernel, (unsigned)qc, 256, prep_smem, st, xq, d, M, PQ4_KSUB, idx->dsub,
+                       idx->codebooks.as<float>(), idx->centroids.as<float>(), keys, nprobe,
+                       idx->w_lut.as<float>(), idx->w_dis0.as<float>());
+            dfx_launch_scan_pq4(M, (unsigned)(qc * ngroups), dfx_pq4_smem(cap), st, idx->w_lut.as<float>(),
+                                idx->w_dis0.as<float>(), keys, nprobe, G, ngroups, idx->list_off.as<int64_t>(),
+                                idx->payload.as<uint8_t>(), idx->tvals.as<float>(), idx->ids.as<int32_t>(), k, cap,
+                                part);
+        } else if (kind == DFX_IVF_PQ && idx->il) {
             // M == 32: table build + exact |q-c|^2 + block scan in ONE kernel; with a single probe
             // group per query it also writes the final rows (dfx_scan_il2.cu)
             final_written = dfx_launch_scan_pq_il2(idx, xq, qc, keys, nprobe, G, ngroups, k, cap, part, d_D + q0 * k,

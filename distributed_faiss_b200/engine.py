@@ -125,6 +125,8 @@ class GpuIndex:
         if self.kind != KIND_FLAT:
             self.quantizer = _Quantizer(self)
         self.pq_m = int(pq_m)
+        self.pq_nbits = int(pq_nbits)
+        self.ksub = 1 << self.pq_nbits if self.kind == KIND_IVF_PQ else 0
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -301,8 +303,8 @@ class GpuIndex:
         else:
             st["coarse_metric"] = self.metric
         if self.kind == KIND_IVF_PQ:
-            st["M"], st["ksub"] = self.pq_m, 256
-            st["codebooks"] = self.get_array("codebooks").reshape(self.pq_m, 256, d // self.pq_m)
+            st["M"], st["ksub"] = self.pq_m, self.ksub
+            st["codebooks"] = self.get_array("codebooks").reshape(self.pq_m, self.ksub, d // self.pq_m)
             st["codes"] = self.get_array("codes").reshape(-1, self.pq_m)
             st["tvals"] = self.get_array("tvals")
         if self.kind == KIND_IVF_SQ16:

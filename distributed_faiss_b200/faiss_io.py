@@ -12,7 +12,8 @@ term `tvals` is not part of the faiss format; the engine recomputes it on import
 
 STATUS: written from the layout of faiss 1.7.x `impl/index_write.cpp` / `index_read.cpp`; faiss
 itself is not available in this environment (SURVEY.md section 8c), so the format is checked for
-self-consistency only (tests/test_faiss_io.py), never against a file written by faiss.
+self-consistency only (tests/test_faiss_io.py), never against a file written by faiss.  The same
+holds for the 4-bit IndexIVFPQ codes [faiss-upstream], restated from faiss's PQEncoderGeneric.
 
 Layout (little endian, no padding; `vec<T>` = u64 count + raw elements):
   header   : i32 d, i64 ntotal, i64 1<<20, i64 1<<20, u8 is_trained, i32 metric (0 IP, 1 L2)
@@ -24,7 +25,8 @@ Layout (little endian, no padding; `vec<T>` = u64 count + raw elements):
              every non-empty list: codes (size * code_size bytes), ids (size * i64)
   IVFFlat  : "IwFl", ivf hdr, invlists (code = raw f32 vector)
   IVFPQ    : "IwPQ", ivf hdr, u8 by_residual, u64 code_size, PQ (u64 d, u64 M, u64 nbits,
-             vec<f32> centroids [M][ksub][dsub]), invlists (code = M bytes)
+             vec<f32> centroids [M][ksub][dsub]), invlists (code = M bytes; nbits 4: ceil(M / 2)
+             bytes, two codes per byte, low nibble first [faiss-upstream: PQEncoderGeneric])
   IVFSQ    : "IwSq", ivf hdr, SQ (i32 qtype, i32 rangestat, f32 rangestat_arg, u64 d,
              u64 code_size, vec<f32> trained), u64 code_size, u8 by_residual, invlists
              qtype 4 (fp16): trained empty, code = d little-endian fp16 of the residual
@@ -191,6 +193,31 @@ def _read_invlists(f, nlist_expected):
     return list_off, ids, rows, code_size
 
 
+def _pack_pq_codes(codes: np.ndarray, nbits: int) -> np.ndarray:
+    """[n, M] codes, one per byte -> faiss's stored rows.  8 bits: unchanged.  4 bits
+    [faiss-upstream: PQEncoderGeneric writes each code's bits least significant first]: code m in the
+    low nibble of byte m // 2 when m is even, in the high nibble when odd; an odd M leaves the last
+    high nibble 0.  code_size = ceil(M / 2)."""
+    if nbits == 8:
+        return np.ascontiguousarray(codes, dtype=np.uint8)
+    if codes.size and int(codes.max()) >= 16:
+        raise FaissFormatError("IndexIVFPQ with 4 bits per sub-quantizer: a code is >= 16")
+    n, M = codes.shape
+    c = np.zeros((n, M + (M & 1)), dtype=np.uint8)
+    c[:, :M] = codes
+    return np.ascontiguousarray(c[:, 0::2] | (c[:, 1::2] << 4))
+
+
+def _unpack_pq_codes(rows: np.ndarray, M: int, nbits: int) -> np.ndarray:
+    """faiss's stored rows -> [n, M] codes, one per byte (the inverse of _pack_pq_codes)"""
+    if nbits == 8:
+        return rows.reshape(-1, M)
+    out = np.empty((rows.shape[0], 2 * rows.shape[1]), dtype=np.uint8)
+    out[:, 0::2] = rows & 15
+    out[:, 1::2] = rows >> 4
+    return np.ascontiguousarray(out[:, :M])
+
+
 # ------------------------------------------------------------------ public
 def write_index(state: Dict, path: str, nprobe: int = 1) -> None:
     """state: engine / oracle `get_state()` dict.  Writes a faiss index file."""
@@ -205,16 +232,17 @@ def write_index(state: Dict, path: str, nprobe: int = 1) -> None:
             _write_invlists(f, state["list_off"], state["ids"], vecs, 4 * int(state["d"]))
         elif kind == "ivf_pq":
             M, ksub = int(state["M"]), int(state["ksub"])
-            if ksub != 256:
-                raise FaissFormatError("only 8-bit product quantizers are supported")
+            nbits = {256: 8, 16: 4}.get(ksub)
+            if nbits is None:
+                raise FaissFormatError(f"only 8-bit and 4-bit product quantizers are supported, got ksub={ksub}")
+            codes = _pack_pq_codes(np.asarray(state["codes"], dtype=np.uint8).reshape(-1, M), nbits)
             f.write(b"IwPQ")
             _write_ivf_header(f, state, METRIC_L2, int(state["coarse_metric"]), nprobe)
             _w(f, "B", 1)  # by_residual
-            _w(f, "Q", M)  # code_size
-            _w(f, "QQQ", int(state["d"]), M, 8)
+            _w(f, "Q", codes.shape[1])  # code_size
+            _w(f, "QQQ", int(state["d"]), M, nbits)
             _wvec(f, state["codebooks"], np.float32)
-            codes = np.ascontiguousarray(state["codes"], dtype=np.uint8)
-            _write_invlists(f, state["list_off"], state["ids"], codes, M)
+            _write_invlists(f, state["list_off"], state["ids"], codes, codes.shape[1])
         elif kind == "ivf_sq":
             d = int(state["d"])
             f.write(b"IwSq")
@@ -263,13 +291,17 @@ def read_index(path: str) -> Tuple[Dict, int]:
             (code_size,) = _r(f, "Q")
             pd, M, nbits = _r(f, "QQQ")
             cb = _rvec(f, np.float32)
-            if not by_res or nbits != 8 or pd != d or code_size != M:
-                raise FaissFormatError("IndexIVFPQ: only by_residual, 8 bits per sub-quantizer is supported")
+            if not by_res or nbits not in (8, 4) or pd != d or code_size != (M * nbits + 7) // 8:
+                raise FaissFormatError("IndexIVFPQ: only by_residual with 8 or 4 bits per sub-quantizer is "
+                                       f"supported (nbits={nbits}, M={M}, code_size={code_size})")
             if metric != METRIC_L2:
                 raise FaissFormatError("IndexIVFPQ: only METRIC_L2 is supported")
             list_off, ids, rows, cs = _read_invlists(f, nlist)
-            st.update(kind="ivf_pq", coarse_metric=cmetric, M=M, ksub=256,
-                      codebooks=cb.reshape(M, 256, d // M), codes=rows.reshape(-1, M))
+            if cs != code_size:
+                raise FaissFormatError("IndexIVFPQ: inverted lists / header code_size mismatch")
+            ksub = 1 << nbits
+            st.update(kind="ivf_pq", coarse_metric=cmetric, M=M, ksub=ksub,
+                      codebooks=cb.reshape(M, ksub, d // M), codes=_unpack_pq_codes(rows, M, nbits))
         else:
             qtype, rangestat, _ = _r(f, "iif")
             sd, scs = _r(f, "QQ")

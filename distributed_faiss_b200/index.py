@@ -12,7 +12,8 @@ Builders (reference index.py:93-100):
   "flat"       -> IndexFlatIP            (always inner product, quirk B1 of SURVEY.md)
   "ivf_simple" -> IndexIVFFlat(metric)   nprobe = cfg.nprobe
   "knnlm"      -> IndexIVFPQ             always L2 / by_residual; M = extra["code_size"] (64),
-                                          nbits = extra["bits_per_vector"] (8); cfg.nprobe is
+                                          nbits = extra["bits_per_vector"] (8, or 4: codes packed
+                                          two per byte, M % 8 == 0, 8 <= M <= 128); cfg.nprobe is
                                           overwritten by the index default 1 (quirk B3)
   "ivfsq"      -> IndexIVFScalarQuantizer(QT_fp16), always L2, nprobe = cfg.nprobe
   "ivf_gpu"    -> faiss.index_factory(dim, faiss_factory): the raw string, L2 whatever cfg.metric
@@ -560,6 +561,13 @@ class Index:
             # e.g. an SQfp16 file under a cfg that builds IVF-SQ8: never reinterpret the codes
             raise RuntimeError(f"the stored index is of kind {state.get('kind')!r} but the cfg builds "
                                f"{want!r}; refusing to load it")
+        if want == "ivf_pq":
+            # e.g. 4-bit codes under a cfg that builds 8-bit ones: the codebooks would not fit either
+            stored = (int(state["M"]), int(state["ksub"]))
+            built = (int(getattr(engine, "pq_m", getattr(engine, "M", 0))), int(engine.ksub))
+            if stored != built:
+                raise RuntimeError(f"the stored IVF-PQ index has (M, ksub) = {stored} but the cfg builds {built}; "
+                                   "refusing to load it")
         engine.set_state(state)
         assert len(meta) >= engine.ntotal, "Deserialized meta list should be at least of index size"
         result.faiss_index = engine

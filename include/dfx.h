@@ -54,10 +54,13 @@ typedef struct dfx_cfg {
                          the coarse quantizer only -- the reference never forwards it to the
                          index, which is therefore always L2 (index.py:44-46, 64-66). */
     int32_t d;        /* vector dimension (cfg.dim) */
-    int32_t pq_m;     /* IVF_PQ: sub-quantizers  (cfg.extra["code_size"], index.py:44); 4 <= M <= 128,
-                         M % 4 == 0, d % M == 0.  128: one query's fp32 table (M x 256 x 4 B) must
-                         fit in one thread block's shared memory */
-    int32_t pq_nbits; /* IVF_PQ: bits per code   (cfg.extra["bits_per_vector"], index.py:45) */
+    int32_t pq_m;     /* IVF_PQ: sub-quantizers  (cfg.extra["code_size"], index.py:44).  8-bit codes:
+                         4 <= M <= 128, M % 4 == 0, d % M == 0 (128: one query's fp32 table,
+                         M x 256 x 4 B, must fit in one thread block's shared memory).  4-bit codes:
+                         8 <= M <= 128, M % 8 == 0, d % M == 0 */
+    int32_t pq_nbits; /* IVF_PQ: bits per code   (cfg.extra["bits_per_vector"], index.py:45): 8, or 4
+                         (ksub = 16; codes stored two per byte, low nibble first, as faiss packs
+                         them) */
     int32_t device;   /* CUDA device ordinal this shard lives on */
     int64_t nlist;    /* IVF_*: number of inverted lists (cfg.centroids); IVF kinds need d % 4 == 0 */
 } dfx_cfg;
@@ -174,6 +177,9 @@ int dfx_map_ids_dev(int64_t n, const int64_t *d_ids, const int64_t *d_table, int
  * named arrays, host memory, list-sorted storage order:
  *   "centroids" f32[nlist,d]   "codebooks" f32[M,ksub,dsub]   "list_off" i64[nlist+1]
  *   "ids" i64[ntotal]   "codes" u8[ntotal,M]   "tvals" f32[ntotal]
+ *   (IVF_PQ: "codes" holds one code per byte whatever pq_nbits is, and "codebooks" has ksub =
+ *   1 << pq_nbits; 4-bit codes are packed and unpacked on the way, and an imported code >= 16 is
+ *   refused)
  *   "vecs" f32[ntotal,d] (IVF_FLAT)   "codes16" u16[ntotal,d]   "xb" f32[ntotal,d] (FLAT)
  *   "sq_trained" f32[2,d] (IVF_SQ8: vmin, then vdiff -- faiss's ScalarQuantizer::trained)
  *   "codes8" u8[ntotal,d] (IVF_SQ8)
