@@ -220,7 +220,8 @@ int dfx_get_param(dfx_index* idx, const char* name, double* value) {
     else if (n == "tc_screen_mode") *value = idx->tc_mode;
     else if (n == "tc_fast") *value = idx->tc_fast;
     else if (n == "tc_auto_window") *value = (double)idx->tc_auto_window;
-    else if (n == "tc_cmax2") *value = idx->tc_cmax2;
+    else if (n == "tc_cmax2") *value = idx->tc_tab.cmax2;
+    else if (n == "tc_cmax2c") *value = idx->tc_tab.cmax2c;
     else if (n == "tc_stat_rows") *value = (double)idx->tc_last_rows;
     else if (n == "tc_stat_overflow") *value = (double)idx->tc_last_overflow;
     else if (n == "tc_stat_fast_would") *value = (double)idx->tc_last_fast_would;

@@ -12,6 +12,18 @@ int dfx_num_sms();
 // dynamic shared memory one CTA of the current device may opt in to (bytes)
 int dfx_smem_optin();
 
+// A screening table of the tensor-core coarse quantizer (dfx_tc.cu): an index's centroids, the
+// rows of a FLAT index, or the centroids of one k-means step.  Rows are screened centred on
+// their mean m, which leaves the ranking unchanged and shrinks the screening error.
+struct dfx_tc_table {
+    DevBuf planes;        // fp16 [2][n_pad][d]: hi and lo planes of (c - m) * scale
+    DevBuf cterm;         // f32 [n_pad]: column term, L2 |c - m|^2, IP -m.c; 3e38 for padded rows
+    DevBuf mean;          // f32 [d] m, then f32 [2] and f64 [MEAN_CHUNKS][d] of work space
+    float scale = 1.f;    // power of two of the planes
+    float cmax2 = 0.f;    // max |c|^2
+    float cmax2c = 0.f;   // max |c - m|^2
+};
+
 struct dfx_index {
     dfx_cfg cfg{};
     int M = 0, ksub = 0, dsub = 0;
@@ -50,10 +62,10 @@ struct dfx_index {
     DevBuf codebooksT;  // [ksub][M][dsub]: the order the fused table build reads (dfx_scan_il2.cu)
     bool cbT_valid = false;
 
-    // tensor-core coarse quantizer (dfx_tc.cu): fp16 copies (1 or 2 planes) and screening workspace
-    DevBuf tc_cent, tc_cent_tmp, tc_q, tc_qmult, tc_gmin, tc_tmin, tc_gmin2, tc_gargc, tc_groups, tc_cand, tc_qn, tc_amb, tc_ovf;
-    float tc_cmax2 = 0.f;
-    float tc_cscale = 1.f;      // power-of-two scale of the fp16 copy tc_cent
+    // tensor-core coarse quantizer (dfx_tc.cu): the index's screening table, the one of a k-means
+    // step, and screening workspace (tc_qn: f32x2 (|q|^2, |q - m|^2) per query row, tc_qterm its row term)
+    dfx_tc_table tc_tab, tc_tab_tmp;
+    DevBuf tc_q, tc_qmult, tc_qterm, tc_gmin, tc_tmin, tc_gmin2, tc_gargc, tc_groups, tc_cand, tc_qn, tc_amb, tc_ovf;
     // screening precision (dfx_tc.cu): tc_mode 0 = AUTO, 1 = FAST (one fp16 MMA per k-step),
     // 2 = PRECISE (hi/lo split, three MMAs).  AUTO starts PRECISE and moves to FAST once a launch
     // shows that FAST's wider tolerance would not overflow the kept groups (and back if it does).

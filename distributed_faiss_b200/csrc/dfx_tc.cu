@@ -110,6 +110,12 @@ __device__ __forceinline__ float tc_pack_col(float v, uint32_t mask, uint32_t id
     asm("lop3.b32 %0, %1, %2, %3, 0xEA;" : "=r"(r) : "r"(__float_as_uint(v)), "r"(mask), "r"(idx));
     return __uint_as_float(r);
 }
+// (bits(v) & mask) | (bits(old) & ~mask) in one LOP3: v with the column bits of old
+__device__ __forceinline__ float tc_repack(float v, uint32_t mask, float old) {
+    uint32_t r;
+    asm("lop3.b32 %0, %1, %2, %3, 0xE2;" : "=r"(r) : "r"(__float_as_uint(v)), "r"(mask), "r"(__float_as_uint(old)));
+    return __uint_as_float(r);
+}
 
 // K-major, SWIZZLE_128B shared-memory matrix descriptor (rows of 128 B, 8-row atoms of 1024 B)
 __device__ __forceinline__ uint64_t make_kmajor_sw128_desc(uint32_t smem_addr) {
@@ -169,38 +175,116 @@ __host__ __device__ __forceinline__ float dfx_pow2_scale(float nrm) {
     return ldexpf(1.f, 14 - e);
 }
 
-// fp32 rows -> fp16 rows scaled by a power of two, rows >= n zero filled; one warp per row.
-//   row_scaled != 0 (queries): the row is scaled so that its norm lands in [2^13, 2^14) and
-//       mult[row] = factor / (row scale * table_scale) -- what the screening epilogue multiplies
-//       the accumulator with (factor = -2 for L2, -1 for inner product; all powers of two, exact);
-//   row_scaled == 0 (a centroid table / the rows of a FLAT index): every row times table_scale.
-// Elements more than 2^28 below the row norm fall into fp16's subnormal range and lose relative
-// (not absolute) precision: an error of at most 2^-39 of the norm, far inside screen_tol.
-// npl == 2 also writes the residual plane lo = fp16(x s - hi) at out + n_pad * d.
+__device__ __forceinline__ double tc_warp_sum(double v) {
+#pragma unroll
+    for (int off = 16; off >= 1; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+    return v;
+}
+
+// Centring.  |c|^2 - 2 q.c = -2 (q-m).(c-m) + |c-m|^2 + (|m|^2 - 2 q.m) and
+// -q.c = -(q-m).(c-m) - m.c + (|m|^2 - q.m) hold for any m: the tensor cores take the centred
+// operands, the epilogue adds a column term (|c-m|^2 or -m.c) and a row term.  The screening
+// error scales with |q-m| max|c-m| instead of |q| max|c|, far smaller where the rows share a
+// large common mean.  m = the mean of the table's rows, summed in fp64 (deterministically: row
+// slices, then the slices in order).
+constexpr int MEAN_CHUNKS = 128;
 __global__ void __launch_bounds__(256)
-f16_rows_kernel(const float* __restrict__ x, int64_t n, int64_t n_pad, int d, int row_scaled, float table_scale,
-                float factor, int npl, __half* __restrict__ out, float* __restrict__ mult, float* __restrict__ norm2) {
+col_part_kernel(const float* __restrict__ x, int64_t n, int d, double* __restrict__ part) {
+    __shared__ double s[8][32];
+    const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    const int k = blockIdx.x * 32 + lane;  // d % 32 == 0
+    const int64_t per = (n + MEAN_CHUNKS - 1) / MEAN_CHUNKS;
+    const int64_t r0 = (int64_t)blockIdx.y * per, r1 = r0 + per < n ? r0 + per : n;
+    double acc = 0.0;
+    for (int64_t r = r0 + w; r < r1; r += 8) acc += (double)x[r * d + k];
+    s[w][lane] = acc;
+    __syncthreads();
+    if (w == 0) {
+        double t = 0.0;
+        for (int i = 0; i < 8; i++) t += s[i][lane];
+        part[(int64_t)blockIdx.y * d + k] = t;
+    }
+}
+__global__ void col_mean_kernel(const double* __restrict__ part, int d, int64_t n, float* __restrict__ mean) {
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= d) return;
+    double t = 0.0;
+    for (int c = 0; c < MEAN_CHUNKS; c++) t += part[(int64_t)c * d + k];
+    mean[k] = n > 0 ? (float)(t / (double)n) : 0.f;
+}
+// per table row (one warp per row, fp64 sums rounded once): the column term, L2 |x-m|^2 or IP
+// -m.x (3e38 for the padded rows: never selected), and maxima[0..1] = max |x|^2, max |x-m|^2
+// (atomicMax on the bits of non-negative floats)
+__global__ void __launch_bounds__(256)
+table_terms_kernel(const float* __restrict__ x, int64_t n, int64_t n_pad, int d, const float* __restrict__ mean,
+                   int metric, float* __restrict__ cterm, float* __restrict__ maxima) {
+    const int lane = threadIdx.x & 31;
+    const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= n_pad) return;
+    if (row >= n) {
+        if (lane == 0) cterm[row] = 3.0e38f;
+        return;
+    }
+    double n2 = 0.0, n2c = 0.0, xm = 0.0;
+    for (int k = lane; k < d; k += 32) {
+        const double v = x[row * d + k], mk = mean[k];
+        n2 += v * v;
+        n2c += (v - mk) * (v - mk);
+        xm += v * mk;
+    }
+    n2 = tc_warp_sum(n2);
+    n2c = tc_warp_sum(n2c);
+    xm = tc_warp_sum(xm);
+    if (lane == 0) {
+        cterm[row] = metric == DFX_METRIC_L2 ? (float)n2c : (float)(-xm);
+        atomicMax(reinterpret_cast<int*>(maxima), __float_as_int((float)n2));
+        atomicMax(reinterpret_cast<int*>(maxima) + 1, __float_as_int((float)n2c));
+    }
+}
+
+// fp32 rows minus m -> fp16 rows scaled by a power of two, rows >= n zero filled; one warp per row.
+//   row_scaled != 0 (queries): the row is scaled so that its centred norm lands in [2^13, 2^14);
+//       mult[row] = factor / (row scale * table_scale) is what the screening epilogue multiplies
+//       the accumulator with (factor = -2 for L2, -1 for inner product; all powers of two, exact),
+//       qterm[row] = |m|^2 + factor q.m the row term it adds, qn[row] = (|q|^2, |q-m|^2) for the
+//       tolerance (fp64 sums, rounded once; zero for padded rows);
+//   row_scaled == 0 (a screening table): every row times table_scale.
+// x - m is rounded to fp32 before the scaling (a power of two, exact).  Elements more than 2^28
+// below the row norm fall into fp16's subnormal range and lose relative (not absolute)
+// precision: an error of at most 2^-39 of the norm, far inside screen_tol.
+// npl == 2 also writes the residual plane lo = fp16(v - hi) at out + n_pad * d.
+__global__ void __launch_bounds__(256)
+f16_rows_kernel(const float* __restrict__ x, int64_t n, int64_t n_pad, int d, const float* __restrict__ mean,
+                int row_scaled, float table_scale, float factor, int npl, __half* __restrict__ out,
+                float* __restrict__ mult, float2* __restrict__ qn, float* __restrict__ qterm) {
     const int lane = threadIdx.x & 31;
     const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (row >= n_pad) return;
     const bool real = row < n;
     float scale = table_scale;
     if (row_scaled) {
-        float part = 0.f;
+        double n2 = 0.0, n2c = 0.0, qm = 0.0, mm = 0.0;
         if (real)
             for (int k = lane; k < d; k += 32) {
-                const float v = x[row * d + k];
-                part = __fmaf_rn(v, v, part);
+                const double v = x[row * d + k], mk = mean[k];
+                n2 += v * v;
+                n2c += (v - mk) * (v - mk);
+                qm += v * mk;
+                mm += mk * mk;
             }
-        const float n2 = dfx_warp_butterfly(part);
-        scale = dfx_pow2_scale(sqrtf(n2));
+        n2 = tc_warp_sum(n2);
+        n2c = tc_warp_sum(n2c);
+        qm = tc_warp_sum(qm);
+        mm = tc_warp_sum(mm);
+        scale = dfx_pow2_scale(sqrtf((float)n2c));
         if (lane == 0) {
             mult[row] = factor / (scale * table_scale);
-            if (norm2) norm2[row] = n2;
+            qn[row] = make_float2((float)n2, (float)n2c);
+            qterm[row] = (float)(mm + (double)factor * qm);
         }
     }
     for (int k = lane; k < d; k += 32) {
-        const float v = real ? x[row * d + k] * scale : 0.f;
+        const float v = real ? (x[row * d + k] - mean[k]) * scale : 0.f;
         const __half hi = __float2half_rn(v);
         out[row * d + k] = hi;
         if (npl == 2) out[n_pad * d + row * d + k] = __float2half_rn(v - __half2float(hi));
@@ -209,15 +293,24 @@ f16_rows_kernel(const float* __restrict__ x, int64_t n, int64_t n_pad, int d, in
 
 #ifdef DFX_EMU
 // ---- CPU emulator stand-in (tests/emu/): the screening kernel cannot be emulated instruction
-// by instruction, so its RESULT is restated: the fp16 operands the product code prepared
+// by instruction, so its RESULT is restated: the centred fp16 operands the product code prepared
 // (f16_rows_kernel), fp32 accumulation (order not specified by the hardware either), the
-// epilogue's ranking value fma(acc, mult[row], cn) and its packed (min, runner-up, arg-min) per
-// 32 centroids.  Everything downstream (group selection, exact canonical re-evaluation, the
+// epilogue's centred ranking value fma(acc, mult[row], cterm[col]), its packed (min, runner-up,
+// arg-min) per 32 centroids, and the row term added to the minimum and runner-up with their
+// column bits kept.  Everything downstream (group selection, exact canonical re-evaluation, the
 // overflow fallback, the drivers) is the product code.
-static void emu_tc_screen(const __half* qh, const float* qmult, int64_t nq, int64_t nq_pad, const __half* ch,
-                          int64_t nlist, int64_t nl_pad, int d, int npl, const float* cnorm, int metric, float* gmin,
+static void emu_tc_screen(const __half* qh, const float* qmult, const float* qterm, int64_t nq, int64_t nq_pad,
+                          const __half* ch, int64_t nl_pad, int d, int npl, const float* cterm, float* gmin,
                           float* gmin2, uint8_t* gargc, float* tmin, int ng) {
     const float big = 3.0e38f;
+    auto repack = [](float v, float col_of) {  // v with the 5 low bits of col_of
+        uint32_t u, c;
+        memcpy(&u, &v, 4);
+        memcpy(&c, &col_of, 4);
+        u = (u & ~31u) | (c & 31u);
+        memcpy(&v, &u, 4);
+        return v;
+    };
     std::vector<float> cf((size_t)npl * nl_pad * d), qf((size_t)npl * d);
     for (size_t i = 0; i < cf.size(); i++) cf[i] = __half2float(ch[i]);
     for (int64_t row = 0; row < nq; row++) {
@@ -234,9 +327,7 @@ static void emu_tc_screen(const __half* qh, const float* qmult, int64_t nq, int6
                     const float* l = &cf[(size_t)nl_pad * d + (size_t)col * d];
                     for (int k = 0; k < d; k++) acc += qf[d + k] * h[k] + qf[k] * l[k];
                 }
-                float cn = big;
-                if (col < nlist) cn = (metric == DFX_METRIC_L2) ? cnorm[col] : 0.f;
-                const float v = fmaf(acc, qmult[row], cn);
+                const float v = fmaf(acc, qmult[row], cterm[col]);
                 uint32_t u;
                 memcpy(&u, &v, 4);
                 u = (u & ~31u) | (uint32_t)j;
@@ -245,6 +336,8 @@ static void emu_tc_screen(const __half* qh, const float* qmult, int64_t nq, int6
                 m2 = fminf(m2, fmaxf(m1, vj));
                 m1 = fminf(m1, vj);
             }
+            m1 = repack(m1 + qterm[row], m1);
+            m2 = repack(m2 + qterm[row], m2);
             uint32_t u1;
             memcpy(&u1, &m1, 4);
             gmin[row * ng + g] = m1;
@@ -260,15 +353,17 @@ static void emu_tc_screen(const __half* qh, const float* qmult, int64_t nq, int6
 #else
 // tmQ: fp16 [NPL * nq_pad, d] (scaled query rows; NPL == 2: hi plane then lo plane), tmC: fp16
 // [NPL * nl_pad, d] (scaled table rows), d = 64 KATOMS
-// qmult: float [nq_pad], the per-row multiplier of the accumulator (f16_rows_kernel)
+// qmult, qterm: float [nq_pad], the per-row multiplier of the accumulator and the row term
+// (f16_rows_kernel); cterm: float [nl_pad], the column term (padded with 3e38)
 // gmin / gmin2: float [nq][ng], gargc: u8 [nq][ng], ng = nl_pad/32
 // KT: d / 64 at compile time for the resident shapes (1, 2, 4); 0 = streamed, k-atoms at run time
-template <int KT, int METRIC, int NPL>
+template <int KT, int NPL>
 __global__ void __launch_bounds__(tc::THREADS, KT != 0 ? tc::Smem::ctas_per_sm(true, KT, NPL) : 1)
 tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmC, int nq,
-                 int nq_pad, int nlist, int nl_pad, int katoms_rt, const float* __restrict__ cnorm,
-                 const float* __restrict__ qmult, int ctiles_per_cta, float* __restrict__ gmin,
-                 float* __restrict__ gmin2, uint8_t* __restrict__ gargc, float* __restrict__ tmin, int ng) {
+                 int nq_pad, int nl_pad, int katoms_rt, const float* __restrict__ cterm,
+                 const float* __restrict__ qmult, const float* __restrict__ qterm, int ctiles_per_cta,
+                 float* __restrict__ gmin, float* __restrict__ gmin2, uint8_t* __restrict__ gargc,
+                 float* __restrict__ tmin, int ng) {
     using namespace tc;
     constexpr bool RES = KT != 0;
     const int KATOMS = KT ? KT : katoms_rt;
@@ -354,6 +449,7 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     const int64_t grow0 = (int64_t)qt * TILE + row0;
     const float big = 3.0e38f;                 // out-of-range columns: finite, never selected
     const float mult0 = qmult[grow0], mult1 = qmult[grow0 + 8];  // padded rows carry a multiplier too
+    const float rq0 = qterm[grow0], rq1 = qterm[grow0 + 8];
     uint32_t idx_mask;                         // ~31 in a REGISTER: (v & mask) | j is then one LOP3
     asm volatile("mov.u32 %0, 0xffffffe0;" : "=r"(idx_mask));
     const uint32_t a_off = (uint32_t)wg * (TILE / 2) * 128;  // this warpgroup's 64 rows of an A atom
@@ -376,13 +472,9 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     for (int t = 0; t < ntiles; t++) {
         const int buf = t & 1;
         const int col0 = (ct0 + t) * TN;
-        // the ranking offset of column threadIdx.x % 128 of the tile: |c|^2 (L2) or 0 (IP), `big`
-        // past nlist; loaded now, shared through this warpgroup's copy once the MMAs are issued
-        float cn_own;
-        {
-            const int c = col0 + (threadIdx.x & (TN - 1));
-            cn_own = c < nlist ? (METRIC == DFX_METRIC_L2 ? cnorm[c] : 0.f) : big;
-        }
+        // the column term of column threadIdx.x % 128 of the tile (`big` past nlist); loaded now,
+        // shared through this warpgroup's copy once the MMAs are issued
+        const float cn_own = cterm[col0 + (threadIdx.x & (TN - 1))];
         if (RES && (wg == 1 || t > 0)) asm volatile("bar.sync %0, %1;" ::"r"(2 + wg), "n"(CONSUMERS) : "memory");
         int prev = -1;  // stage of the group still in flight
         for (int c = 0; c < (RES ? NPL : NCOMBO); c++)
@@ -443,6 +535,10 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
                     m2 = fminf(fmaxf(m1, o1), fminf(m2, o2));
                     m1 = fminf(m1, o1);
                 }
+                // back to the original ranking frame: + the row term, column bits kept
+                const float rq = h ? rq1 : rq0;
+                m1 = tc_repack(m1 + rq, idx_mask, m1);
+                m2 = tc_repack(m2 + rq, idx_mask, m2);
                 gm[h][g] = m1;
                 gm2[h][g] = m2;
                 ga[h] |= (__float_as_uint(m1) & 31u) << (8 * g);
@@ -475,23 +571,44 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 // approx(c) >= gmin2(group).  So a group is expanded to all 32 columns only if
 // gmin2 <= t + tol, otherwise its arg-min column is the only candidate.
 //
-// Screening error, s = |q| max|c| (Cauchy-Schwarz bounds sum |q_k c_k| by it):
-//   FAST (fp16 operands): every product carries two relative roundings of at most 2^-11
-//     (2^-10 + 2^-22 together), the fp32 accumulation of the d products at most d 2^-24:
-//       |q.c - screen| <= s (2^-10 + 2^-22 + d 2^-24)
-//   PRECISE (hi + lo planes, three partial products): hi + lo represents an operand to 2^-22, the
-//     dropped ql.cl term is 2^-22, 3d products are accumulated:
-//       |q.c - screen| <= s (3 2^-22 + 3 d 2^-24)
-// The L2 ranking value |c|^2 - 2 q.c doubles it and the tolerance must be twice the error of a
-// value (threshold and candidate are both approximations): tol = 4 err (+5 % slack).  The packed
-// column index perturbs a value by 2^-18 |v|, |v| <= max|c|^2 + 2 s: the 1e-5 term.
+// The tolerance must be twice the error e of one value against its canonical value (threshold
+// and candidate are both approximations), up to a constant per row (it moves every value of the
+// row alike).  With sc = |q-m| max|c-m|, Vc = max|c-m|^2 + 2 sc (bounds a centred value),
+// s = |q| max|c| and V = max|c|^2 + 2 s (bounds a value in the original frame):
+//   the centred product (q-m).(c-m) on the tensor cores, Cauchy-Schwarz bounding sum |q_k c_k|:
+//     FAST (fp16 operands): every product carries two relative roundings of at most 2^-11
+//       (2^-10 + 2^-22 together), the fp32 accumulation of the d products at most d 2^-24:
+//         err = 2^-10 + 2^-22 + d 2^-24
+//     PRECISE (hi + lo planes, three partial products): hi + lo represents an operand to 2^-22,
+//       the dropped ql.cl term is 2^-22, 3d products are accumulated:
+//         err = 3 2^-22 + 3 d 2^-24
+//     plus 2^-23 for the fp32 subtractions q - m and c - m (2^-24 per operand); the L2 value
+//     takes the product twice: 2 (err + 2^-23) sc;
+//   in the centred frame, <= (2^-18 + 2^-23) Vc: the epilogue's fma (2^-24), the fp32 column
+//     term (2^-24) and the packed column index (2^-18 of the value);
+//   in the original frame, <= (2^-17 + 2^-22 + d 2^-24) V: the row term's addition (2^-24) and
+//     the re-packed column index (2^-18); the canonical value's own rounding (d 2^-24 for |c|^2
+//     and for q.c, 2^-24 for their difference), no longer shared with the screening value; for
+//     inner product, where a centred value is bounded by V + Vc, the centred-frame terms on V.
+// tol = 2 e, +5 % slack.  The row term itself (fp64, rounded once) is a constant per row.
 static float screen_tol_rel(int d, bool fast) {
     const double err = fast ? (1.0 / 1024 + 1.0 / 4194304 + d / 16777216.0) : (3.0 / 4194304 + 3.0 * d / 16777216.0);
-    return (float)(4.2 * err);
+    return (float)(4.2 * (err + 1.0 / 8388608));
 }
-__device__ __forceinline__ float screen_tol(float qn2, float cmax2, float rel) {
-    const float s = sqrtf(qn2 * cmax2);
-    return rel * s + 1e-5f * (cmax2 + 2.f * s) + 1e-30f;
+static float screen_tol_raw(int d) { return (float)(2.1 * (1.0 / 131072 + 1.0 / 4194304 + d / 16777216.0)); }
+constexpr float SCREEN_TOL_CENTRED = (float)(2.1 * (1.0 / 262144 + 1.0 / 8388608));
+// what the tolerance of a row needs besides its precision: the table's maxima and the rows' norms
+struct ScreenTol {
+    float rel;            // of this launch's precision
+    float rel_fast;       // > 0: also count the rows FAST would overflow
+    float raw;            // screen_tol_raw(d)
+    float cmax2, cmax2c;  // max |c|^2, max |c-m|^2
+    const float2* qn;     // per row: |q|^2, |q-m|^2 (f16_rows_kernel)
+};
+__device__ __forceinline__ float screen_tol(const ScreenTol& t, int64_t row, float rel) {
+    const float2 qn = t.qn[row];
+    const float s = sqrtf(qn.x * t.cmax2), sc = sqrtf(qn.y * t.cmax2c);
+    return rel * sc + SCREEN_TOL_CENTRED * (t.cmax2c + 2.f * sc) + t.raw * (t.cmax2 + 2.f * s) + 1e-30f;
 }
 // "the selected groups may not be all that matter": the G-th (last) selected group is itself
 // within the tolerance, so an unselected group could be too -> the row is re-done exactly
@@ -505,18 +622,14 @@ __device__ __forceinline__ bool screen_overflow(const int32_t* __restrict__ grou
 // there are fewer groups than probes: nothing is pruned).  A row with more near-ties than
 // selected groups is queued for tc_exact_rows_kernel.  ovf = [overflow rows, rows that the FAST
 // tolerance would overflow (counted by PRECISE launches for the AUTO mode), row list ...].
-struct ScreenTol {
-    float rel;       // of this launch's precision
-    float rel_fast;  // > 0: also count the rows FAST would overflow
-};
 __device__ __forceinline__ float screen_threshold(const int32_t* __restrict__ groups, int64_t row, int G, int nprobe,
-                                                  int ng, const float* __restrict__ gmin, float qn2, float cmax2,
-                                                  ScreenTol tol, int32_t* __restrict__ ovf) {
+                                                  int ng, const float* __restrict__ gmin, const ScreenTol& tol,
+                                                  int32_t* __restrict__ ovf) {
     const int gk = (nprobe <= G) ? groups[row * G + nprobe - 1] : -1;
     const float t = gk >= 0 ? gmin[row * ng + gk] : __int_as_float(0x7f800000);
-    const float thr = t + screen_tol(qn2, cmax2, tol.rel);
+    const float thr = t + screen_tol(tol, row, tol.rel);
     if (screen_overflow(groups, row, G, ng, gmin, thr)) ovf[2 + atomicAdd(&ovf[0], 1)] = (int32_t)row;
-    if (tol.rel_fast > 0.f && screen_overflow(groups, row, G, ng, gmin, t + screen_tol(qn2, cmax2, tol.rel_fast)))
+    if (tol.rel_fast > 0.f && screen_overflow(groups, row, G, ng, gmin, t + screen_tol(tol, row, tol.rel_fast)))
         atomicAdd(&ovf[1], 1);
     return thr;
 }
@@ -660,7 +773,7 @@ __global__ void __launch_bounds__(128)
 rerank_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent, const float* __restrict__ cnorm,
               int64_t nlist, int metric, const int32_t* __restrict__ groups, int G, int nprobe,
               const float* __restrict__ gmin, const float* __restrict__ gmin2, const uint8_t* __restrict__ gargc,
-              int ng, float cmax2, ScreenTol tol, uint64_t* __restrict__ out, int32_t* __restrict__ assign,
+              int ng, ScreenTol tol, uint64_t* __restrict__ out, int32_t* __restrict__ assign,
               const int32_t* __restrict__ rows, const int32_t* __restrict__ nrows_dev, int64_t nrows,
               int32_t* __restrict__ keys, int32_t* __restrict__ ovf) {
     DFX_DYN_SMEM(unsigned char, rr_smem, 16);
@@ -677,11 +790,7 @@ rerank_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent
         for (int i = threadIdx.x; i < d; i += 128) s_q[i] = Q[row * d + i];
         if (threadIdx.x == 0) s_cnt = 0;
         __syncthreads();
-        if (threadIdx.x == 0) {
-            float qn2 = 0.f;
-            for (int i = 0; i < d; i++) qn2 += s_q[i] * s_q[i];
-            s_thr = screen_threshold(groups, row, G, nprobe, ng, gmin, qn2, cmax2, tol, ovf);
-        }
+        if (threadIdx.x == 0) s_thr = screen_threshold(groups, row, G, nprobe, ng, gmin, tol, ovf);
         __syncthreads();
         const float thr = s_thr;
         unsigned long long best = DFX_COMP_NONE;
@@ -731,21 +840,19 @@ rerank_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent
 
 // Search path, nprobe <= 32 and G <= 64: the same decision as rerank_kernel<2>, one WARP per
 // query instead of one 128-thread CTA.  rerank_kernel<2> spends a whole CTA on a query although
-// only ~9 candidates per query survive the screening: one thread sums |q|^2 serially, 128 threads walk 512 candidate slots of
+// only ~9 candidates per query survive the screening: 128 threads walk 512 candidate slots of
 // which a handful are live, then a block-wide sort.  Here: lanes own the selected groups, live
 // candidates are compacted into a per-warp list (arg-min column, or all 32 columns of a group
 // whose runner-up is within the tolerance), each lane evaluates one candidate in the canonical
 // seq-k order, and the nprobe smallest come out of a register bitonic network.  The candidate set
 // is a superset of the true top-nprobe for any tolerance >= the screening error, so the keys are
-// identical to rerank_kernel<2>'s (|q|^2 is summed in a different order: only the tolerance moves,
-// by one ulp).
+// identical to rerank_kernel<2>'s.
 constexpr int RR2_WARPS = 4;
 __global__ void __launch_bounds__(RR2_WARPS * 32)
 rerank2_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent, const float* __restrict__ cnorm,
                int64_t nlist, int metric, const int32_t* __restrict__ groups, int G, int nprobe,
                const float* __restrict__ gmin, const float* __restrict__ gmin2, const uint8_t* __restrict__ gargc,
-               int ng, float cmax2, ScreenTol tol, int64_t nrows, int32_t* __restrict__ keys,
-               int32_t* __restrict__ ovf) {
+               int ng, ScreenTol tol, int64_t nrows, int32_t* __restrict__ keys, int32_t* __restrict__ ovf) {
     DFX_DYN_SMEM(unsigned char, rr2_smem, 16);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int64_t row = (int64_t)blockIdx.x * RR2_WARPS + warp;
@@ -753,17 +860,11 @@ rerank2_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cen
     const int dq = (d + 3) / 4 * 4;
     float* s_q = reinterpret_cast<float*>(rr2_smem) + (size_t)warp * dq;
     int32_t* s_cand = reinterpret_cast<int32_t*>(rr2_smem + (size_t)RR2_WARPS * dq * 4) + (size_t)warp * G * 32;
-    float part = 0.f;
 #pragma unroll 4
-    for (int i = lane; i < d; i += 32) {
-        const float v = Q[row * d + i];
-        s_q[i] = v;
-        part = __fmaf_rn(v, v, part);
-    }
-    const float qn2 = dfx_warp_butterfly(part);
+    for (int i = lane; i < d; i += 32) s_q[i] = Q[row * d + i];
     __syncwarp();
     float thr = 0.f;
-    if (lane == 0) thr = screen_threshold(groups, row, G, nprobe, ng, gmin, qn2, cmax2, tol, ovf);
+    if (lane == 0) thr = screen_threshold(groups, row, G, nprobe, ng, gmin, tol, ovf);
     thr = __shfl_sync(0xffffffffu, thr, 0);
     // ---- candidate list: one entry for a live group's arg-min column, 32 for an expanded group
     int cnt = 0;
@@ -814,19 +915,18 @@ rerank2_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cen
 // assign fast path: one thread per row decides from the screening summary alone when the best
 // group's arg-min column is unambiguous (no other column within tol); other rows are queued
 // for the exact evaluation above.
-__global__ void assign_resolve_kernel(const float* __restrict__ qnorm2, const int32_t* __restrict__ groups,
-                                      const float* __restrict__ gmin, const float* __restrict__ gmin2,
-                                      const uint8_t* __restrict__ gargc, int ng, int G, float cmax2, float tol_rel,
-                                      float tol_rel_fast, int64_t n, int32_t* __restrict__ assign,
+__global__ void assign_resolve_kernel(const int32_t* __restrict__ groups, const float* __restrict__ gmin,
+                                      const float* __restrict__ gmin2, const uint8_t* __restrict__ gargc, int ng,
+                                      int G, ScreenTol tol, int64_t n, int32_t* __restrict__ assign,
                                       int32_t* __restrict__ amb_rows, int32_t* __restrict__ amb_count,
                                       int32_t* __restrict__ ovf) {
     const int64_t row = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (row >= n) return;
     const int g0 = groups[row * G + 0], g1 = (G > 1) ? groups[row * G + 1] : -1;
     const int64_t o0 = row * ng + g0;
-    const float thr = gmin[o0] + screen_tol(qnorm2[row], cmax2, tol_rel);
-    if (tol_rel_fast > 0.f &&
-        screen_overflow(groups, row, G, ng, gmin, gmin[o0] + screen_tol(qnorm2[row], cmax2, tol_rel_fast)))
+    const float thr = gmin[o0] + screen_tol(tol, row, tol.rel);
+    if (tol.rel_fast > 0.f &&
+        screen_overflow(groups, row, G, ng, gmin, gmin[o0] + screen_tol(tol, row, tol.rel_fast)))
         atomicAdd(&ovf[1], 1);  // AUTO mode statistic: FAST would send this row to the exact fallback
     const bool clear = gmin2[o0] > thr && (g1 < 0 || gmin[row * ng + g1] > thr);
     if (clear) {
@@ -895,14 +995,6 @@ static void launch_exact_rows(const float* Q, const float* X, const float* xnorm
     DFX_LAUNCH(tc_exact_rows_kernel, grid, 256, smem, st, Q, ld, wr, ovf, n, K, P, sort_cap);
 }
 
-__global__ void max_reduce_kernel(const float* __restrict__ x, int64_t n, float* __restrict__ out) {
-    float m = 0.f;
-    for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x)
-        m = fmaxf(m, x[i]);
-    for (int off = 16; off >= 1; off >>= 1) m = fmaxf(m, __shfl_xor_sync(0xffffffffu, m, off));
-    if ((threadIdx.x & 31) == 0) atomicMax(reinterpret_cast<int*>(out), __float_as_int(m));  // m >= 0
-}
-
 // ------------------------------------------------------------------ host side
 #ifndef DFX_EMU
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -938,34 +1030,36 @@ static void make_tmap(CUtensorMap* tm, const void* base, int64_t rows, int d, in
 // d = a whole number of 64-element k-atoms (d <= 256: query tile resident; above: streamed)
 bool dfx_tc_supported(int d) { return d >= 64 && d % 64 == 0 && d <= 2048; }
 
-// max |c|^2 of a centroid table (for the screening tolerance), synchronises
-static float max_norm2(dfx_index* idx, const float* cnorm, int64_t nlist, cudaStream_t st) {
-    idx->w_misc.reserve(8);
-    DFX_CUDA(cudaMemsetAsync(idx->w_misc.p, 0, 4, st));
-    DFX_LAUNCH(max_reduce_kernel, 64, 256, 0, st, cnorm, nlist, idx->w_misc.as<float>());
-    float h = 0.f;
-    DFX_CUDA(cudaMemcpyAsync(&h, idx->w_misc.p, 4, cudaMemcpyDeviceToHost, st));
-    DFX_CUDA(cudaStreamSynchronize(st));
-    return h;
-}
-
-// fp16 copy of a table (centroids / FLAT rows), npl planes, scaled so that the largest row norm
-// lands in [2^13, 2^14); returns the scale
-static float tc_prepare_table(const float* x, int64_t n, int d, float cmax2, int npl, DevBuf& out, cudaStream_t st) {
+// the screening table of rows x [n][d] (centroids / FLAT rows), synchronises: their mean m, the
+// column terms, the norm maxima, and the fp16 hi and lo planes of x - m (either precision can use
+// them), scaled so that the largest centred row norm lands in [2^13, 2^14)
+static void tc_prepare_table(const float* x, int64_t n, int d, int metric, dfx_tc_table& tab, cudaStream_t st) {
     const int64_t n_pad = dfx_ceil_div(n, tc::TILE) * tc::TILE;
-    out.reserve((size_t)npl * n_pad * d * 2);
-    const float scale = dfx_pow2_scale(sqrtf(cmax2));
-    DFX_LAUNCH(f16_rows_kernel, (unsigned)dfx_ceil_div(n_pad, 8), 256, 0, st, x, n, n_pad, d, 0, scale, 0.f, npl,
-               out.as<__half>(), (float*)nullptr, (float*)nullptr);
-    return scale;
+    tab.mean.reserve((size_t)d * 4 + 8 + (size_t)MEAN_CHUNKS * d * 8);
+    float* mean = tab.mean.as<float>();
+    float* maxima = mean + d;                                  // [2]
+    double* part = reinterpret_cast<double*>(maxima + 2);      // d % 64 == 0: 8-byte aligned
+    DFX_LAUNCH(col_part_kernel, dim3((unsigned)(d / 32), MEAN_CHUNKS), 256, 0, st, x, n, d, part);
+    DFX_LAUNCH(col_mean_kernel, (unsigned)dfx_ceil_div(d, 128), 128, 0, st, part, d, n, mean);
+    tab.cterm.reserve((size_t)n_pad * 4);
+    DFX_CUDA(cudaMemsetAsync(maxima, 0, 8, st));
+    DFX_LAUNCH(table_terms_kernel, (unsigned)dfx_ceil_div(n_pad, 8), 256, 0, st, x, n, n_pad, d, mean, metric,
+               tab.cterm.as<float>(), maxima);
+    float h[2] = {0.f, 0.f};
+    DFX_CUDA(cudaMemcpyAsync(h, maxima, 8, cudaMemcpyDeviceToHost, st));
+    DFX_CUDA(cudaStreamSynchronize(st));
+    tab.cmax2 = h[0];
+    tab.cmax2c = h[1];
+    tab.scale = dfx_pow2_scale(sqrtf(tab.cmax2c));
+    tab.planes.reserve((size_t)2 * n_pad * d * 2);
+    DFX_LAUNCH(f16_rows_kernel, (unsigned)dfx_ceil_div(n_pad, 8), 256, 0, st, x, n, n_pad, d, (const float*)mean, 0,
+               tab.scale, 0.f, 2, tab.planes.as<__half>(), (float*)nullptr, (float2*)nullptr, (float*)nullptr);
 }
 
-// install the index's screening table (its centroids, or the rows of a FLAT index): the norm
-// bound, the fp16 copy with both planes (either precision can use it) and its scale; AUTO starts
+// install the index's screening table (its centroids, or the rows of a FLAT index); AUTO starts
 // PRECISE on a new table
-static void tc_install_table(dfx_index* idx, const float* x, const float* norms, int64_t n, cudaStream_t st) {
-    idx->tc_cmax2 = max_norm2(idx, norms, n, st);
-    idx->tc_cscale = tc_prepare_table(x, n, idx->cfg.d, idx->tc_cmax2, 2, idx->tc_cent, st);
+static void tc_install_table(dfx_index* idx, const float* x, int64_t n, cudaStream_t st) {
+    tc_prepare_table(x, n, idx->cfg.d, idx->cfg.metric, idx->tc_tab, st);
     if (idx->tc_mode == 0) idx->tc_fast = false;
     idx->tc_stat_pending = false;
     idx->tc_acc_rows = idx->tc_acc_bad = 0;
@@ -974,7 +1068,7 @@ static void tc_install_table(dfx_index* idx, const float* x, const float* norms,
 // (re)build the screening table of the centroids; call after training / import
 void dfx_tc_prepare_centroids(dfx_index* idx, cudaStream_t st) {
     if (!dfx_tc_supported(idx->cfg.d)) return;
-    tc_install_table(idx, idx->centroids.as<float>(), idx->cnorm.as<float>(), idx->cfg.nlist, st);
+    tc_install_table(idx, idx->centroids.as<float>(), idx->cfg.nlist, st);
     idx->tc_ready = true;
 }
 
@@ -1049,30 +1143,39 @@ static void tc_stats_post(dfx_index* idx, const int32_t* ovf, int64_t rows, bool
     idx->tc_stat_fast = fast;
     idx->tc_stat_rows = rows;
 }
-static ScreenTol tc_tol(const dfx_index* idx, int d, bool fast) {
+// the tolerance of a launch against table `tab`, for the rows tc_screen last prepared
+static ScreenTol tc_tol(const dfx_index* idx, const dfx_tc_table& tab, int d, bool fast) {
     ScreenTol t;
     t.rel = screen_tol_rel(d, fast);
     t.rel_fast = (!fast && idx->tc_mode == 0) ? screen_tol_rel(d, true) : 0.f;
+    t.raw = screen_tol_raw(d);
+    t.cmax2 = tab.cmax2;
+    t.cmax2c = tab.cmax2c;
+    t.qn = idx->tc_qn.as<float2>();
     return t;
 }
 
 // screening pass: gmin[nq][ng] for a batch of rows against a table prepared by tc_prepare_table
-// (npl planes used; the table must hold at least npl)
-static void tc_screen(dfx_index* idx, int d, const float* d_x, int64_t nq, const void* table_h, float table_scale,
-                      int npl, const float* cnorm, int64_t nlist, int metric, float* gmin, float* gmin2,
-                      uint8_t* gargc, float* tmin, cudaStream_t st) {
+// (npl planes used); leaves the rows' norms in idx->tc_qn
+static void tc_screen(dfx_index* idx, int d, const float* d_x, int64_t nq, const dfx_tc_table& tab, int npl,
+                      int64_t nlist, int metric, float* gmin, float* gmin2, uint8_t* gargc, float* tmin,
+                      cudaStream_t st) {
     using namespace tc;
     const int64_t nl_pad = dfx_ceil_div(nlist, TILE) * TILE;
     const int64_t nq_pad = dfx_ceil_div(nq, TILE) * TILE;
     const int ng = (int)(nl_pad / 32);
     idx->tc_q.reserve((size_t)npl * nq_pad * d * 2);
     idx->tc_qmult.reserve((size_t)nq_pad * 4);
-    DFX_LAUNCH(f16_rows_kernel, (unsigned)dfx_ceil_div(nq_pad, 8), 256, 0, st, d_x, nq, nq_pad, d, 1, table_scale,
-               metric == DFX_METRIC_IP ? -1.f : -2.f, npl, idx->tc_q.as<__half>(), idx->tc_qmult.as<float>(),
-               (float*)nullptr);
+    idx->tc_qterm.reserve((size_t)nq_pad * 4);
+    idx->tc_qn.reserve((size_t)nq_pad * 8);
+    DFX_LAUNCH(f16_rows_kernel, (unsigned)dfx_ceil_div(nq_pad, 8), 256, 0, st, d_x, nq, nq_pad, d,
+               (const float*)tab.mean.as<float>(), 1, tab.scale, metric == DFX_METRIC_IP ? -1.f : -2.f, npl,
+               idx->tc_q.as<__half>(), idx->tc_qmult.as<float>(), idx->tc_qn.as<float2>(), idx->tc_qterm.as<float>());
+    const void* table_h = tab.planes.p;
+    const float* cterm = tab.cterm.as<float>();
 #ifdef DFX_EMU
-    emu_tc_screen(idx->tc_q.as<__half>(), idx->tc_qmult.as<float>(), nq, nq_pad, static_cast<const __half*>(table_h),
-                  nlist, nl_pad, d, npl, cnorm, metric, gmin, gmin2, gargc, tmin, ng);
+    emu_tc_screen(idx->tc_q.as<__half>(), idx->tc_qmult.as<float>(), idx->tc_qterm.as<float>(), nq, nq_pad,
+                  static_cast<const __half*>(table_h), nl_pad, d, npl, cterm, gmin, gmin2, gargc, tmin, ng);
     return;
 #else
     const int katoms = d / KATOM;
@@ -1106,30 +1209,24 @@ static void tc_screen(dfx_index* idx, int d, const float* d_x, int64_t nq, const
     }
     dim3 grid((unsigned)csplit, (unsigned)qtiles);
     DFX_REQUIRE(qtiles <= 65535, "too many query tiles in one screening launch");
-#define DFX_TC_LAUNCH(KT_, MT, NP)                                                                       \
+#define DFX_TC_LAUNCH(KT_, NP)                                                                           \
     do {                                                                                                 \
-        auto kern = tc_coarse_kernel<KT_, MT, NP>;                                                       \
+        auto kern = tc_coarse_kernel<KT_, NP>;                                                           \
         DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));    \
-        DFX_LAUNCH(kern, grid, THREADS, smem, st, tmQ, tmC, (int)nq, (int)nq_pad, (int)nlist, (int)nl_pad, katoms, \
-                   cnorm, idx->tc_qmult.as<float>(), per, gmin, gmin2, gargc, tmin, ng);                 \
-    } while (0)
-#define DFX_TC_LAUNCH_M(KT_, NP)                                          \
-    do {                                                                  \
-        if (metric == DFX_METRIC_L2) DFX_TC_LAUNCH(KT_, DFX_METRIC_L2, NP); \
-        else DFX_TC_LAUNCH(KT_, DFX_METRIC_IP, NP);                       \
+        DFX_LAUNCH(kern, grid, THREADS, smem, st, tmQ, tmC, (int)nq, (int)nq_pad, (int)nl_pad, katoms, cterm, \
+                   idx->tc_qmult.as<float>(), idx->tc_qterm.as<float>(), per, gmin, gmin2, gargc, tmin, ng); \
     } while (0)
     // resident shapes get their k-atom count at compile time (npl * katoms <= 4)
     if (npl == 1) {
-        if (res && katoms == 1) DFX_TC_LAUNCH_M(1, 1);
-        else if (res && katoms == 2) DFX_TC_LAUNCH_M(2, 1);
-        else if (res && katoms == 4) DFX_TC_LAUNCH_M(4, 1);
-        else DFX_TC_LAUNCH_M(0, 1);
+        if (res && katoms == 1) DFX_TC_LAUNCH(1, 1);
+        else if (res && katoms == 2) DFX_TC_LAUNCH(2, 1);
+        else if (res && katoms == 4) DFX_TC_LAUNCH(4, 1);
+        else DFX_TC_LAUNCH(0, 1);
     } else {
-        if (res && katoms == 1) DFX_TC_LAUNCH_M(1, 2);
-        else if (res && katoms == 2) DFX_TC_LAUNCH_M(2, 2);
-        else DFX_TC_LAUNCH_M(0, 2);
+        if (res && katoms == 1) DFX_TC_LAUNCH(1, 2);
+        else if (res && katoms == 2) DFX_TC_LAUNCH(2, 2);
+        else DFX_TC_LAUNCH(0, 2);
     }
-#undef DFX_TC_LAUNCH_M
 #undef DFX_TC_LAUNCH
 #endif  // DFX_EMU
 }
@@ -1162,8 +1259,7 @@ struct Screened {
 // screen a chunk of `rows` rows against a table (as tc_screen) and select their G groups; the
 // workspace is sized for chunks of up to rmax rows
 static Screened tc_screen_chunk(dfx_index* idx, int d, const float* d_x, int64_t rows, int64_t rmax, int ng, int G,
-                                const void* table_h, float table_scale, int npl, const float* cnorm, int64_t nlist,
-                                int metric, cudaStream_t st) {
+                                const dfx_tc_table& tab, int npl, int64_t nlist, int metric, cudaStream_t st) {
     idx->tc_gmin.reserve((size_t)rmax * ng * 4);
     idx->tc_gmin2.reserve((size_t)rmax * ng * 4);
     idx->tc_gargc.reserve((size_t)rmax * ng);
@@ -1171,8 +1267,8 @@ static Screened tc_screen_chunk(dfx_index* idx, int d, const float* d_x, int64_t
     idx->tc_tmin.reserve((size_t)rmax * (ng / 4 + 1) * 4);
     float* gmin = idx->tc_gmin.as<float>();
     float* tmin = idx->tc_tmin.as<float>();
-    tc_screen(idx, d, d_x, rows, table_h, table_scale, npl, cnorm, nlist, metric, gmin, idx->tc_gmin2.as<float>(),
-              idx->tc_gargc.as<uint8_t>(), tmin, st);
+    tc_screen(idx, d, d_x, rows, tab, npl, nlist, metric, gmin, idx->tc_gmin2.as<float>(), idx->tc_gargc.as<uint8_t>(),
+              tmin, st);
     tc_select_groups(gmin, tmin, rows, ng, G, idx->tc_groups.as<int32_t>(), st);
     idx->tc_ovf.reserve((size_t)(rows + 2) * 4);
     DFX_CUDA(cudaMemsetAsync(idx->tc_ovf.p, 0, 8, st));
@@ -1189,8 +1285,8 @@ void dfx_tc_debug_screen(dfx_index* idx, int64_t nq, const float* d_x, int npl, 
     const int64_t nlist = idx->cfg.nlist;
     const int ng = (int)(dfx_ceil_div(nlist, tc::TILE) * tc::TILE / 32);
     idx->tc_tmin.reserve((size_t)nq * (ng / 4) * 4);
-    tc_screen(idx, idx->cfg.d, d_x, nq, idx->tc_cent.p, idx->tc_cscale, npl, idx->cnorm.as<float>(), nlist,
-              idx->cfg.metric, gmin, gmin2, gargc, idx->tc_tmin.as<float>(), st);
+    tc_screen(idx, idx->cfg.d, d_x, nq, idx->tc_tab, npl, nlist, idx->cfg.metric, gmin, gmin2, gargc,
+              idx->tc_tmin.as<float>(), st);
 }
 
 // top-nprobe lists per query -> keys int32 [nq, nprobe] (exactly the oracle's coarse result)
@@ -1200,42 +1296,45 @@ void dfx_tc_coarse_search(dfx_index* idx, const float* d_x, int64_t nq, int npro
     const int metric = idx->cfg.metric;
     const int64_t nl_pad = dfx_ceil_div(nlist, tc::TILE) * tc::TILE;
     const int ng = (int)(nl_pad / 32);
-    // groups kept per query: nprobe + 8; with few groups in all (nlist <= 2048) every one is kept,
-    // so that no row can overflow (at d = 768, nprobe 32 of 64 groups, most rows did)
+    tc_stats_poll(idx, st);
+    const bool fast = idx->tc_fast;
+    // groups kept per query: nprobe + 8 at PRECISE.  FAST's tolerance is wider: where FAST is used
+    // or may be chosen (AUTO, which counts FAST's overflows on PRECISE launches) up to nprobe + 24,
+    // at most 32 (the two-level group selection); on the bench data nprobe + 8 left 3 rows in
+    // 10 000 with more near-ties than selected groups under FAST, nprobe + 16 none.  With few
+    // groups in all (nlist <= 2048) every one is kept, so that no row can overflow (at d = 768,
+    // nprobe 32 of 64 groups, most rows did)
     int G = nprobe + 8;
+    if (fast || idx->tc_mode == 0) G = std::max(G, std::min(32, nprobe + 24));
     if (G > ng || ng <= 64) G = ng;
     const int64_t QC = std::max<int64_t>(tc::TILE, ((64ll << 20) / ((int64_t)ng * 4)) / tc::TILE * tc::TILE);
     const int64_t qmax = std::min<int64_t>(nq, QC);
     const float* cent = idx->centroids.as<float>();
     const float* cnorm = idx->cnorm.as<float>();
-    tc_stats_poll(idx, st);
-    const bool fast = idx->tc_fast;
-    const ScreenTol tol = tc_tol(idx, d, fast);
     for (int64_t q0 = 0; q0 < nq; q0 += QC) {
         const int64_t qc = std::min(QC, nq - q0);
         const float* xq = d_x + q0 * d;
         int32_t* kq = keys + q0 * nprobe;
-        const Screened s = tc_screen_chunk(idx, d, xq, qc, qmax, ng, G, idx->tc_cent.p, idx->tc_cscale, fast ? 1 : 2,
-                                           cnorm, nlist, metric, st);
+        const Screened s = tc_screen_chunk(idx, d, xq, qc, qmax, ng, G, idx->tc_tab, fast ? 1 : 2, nlist, metric, st);
+        const ScreenTol tol = tc_tol(idx, idx->tc_tab, d, fast);
         const int P_cand = dfx_next_pow2(G * 32 < 32 ? 32 : G * 32);
         if (nprobe <= 32 && G <= 64 && d % 4 == 0) {  // warp per query
             const size_t smem = (size_t)RR2_WARPS * ((d + 3) / 4 * 4) * 4 + (size_t)RR2_WARPS * G * 32 * 4;
             if (smem > 48 * 1024)
                 DFX_CUDA(cudaFuncSetAttribute(rerank2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
             DFX_LAUNCH(rerank2_kernel, (unsigned)dfx_ceil_div(qc, RR2_WARPS), RR2_WARPS * 32, smem, st, xq, d, cent,
-                       cnorm, nlist, metric, s.groups, G, nprobe, s.gmin, s.gmin2, s.gargc, ng, idx->tc_cmax2, tol, qc,
-                       kq, s.ovf);
+                       cnorm, nlist, metric, s.groups, G, nprobe, s.gmin, s.gmin2, s.gargc, ng, tol, qc, kq, s.ovf);
         } else if (P_cand <= 4096) {  // fused: candidates never leave the SM
             auto kern = rerank_kernel<2>;
             const size_t smem = ((size_t)d * 4 + 15) / 16 * 16 + (size_t)P_cand * 8;
             DFX_LAUNCH(kern, (unsigned)qc, 128, smem, st, xq, d, cent, cnorm, nlist, metric, s.groups, G, nprobe,
-                       s.gmin, s.gmin2, s.gargc, ng, idx->tc_cmax2, tol, (uint64_t*)nullptr, (int32_t*)nullptr,
+                       s.gmin, s.gmin2, s.gargc, ng, tol, (uint64_t*)nullptr, (int32_t*)nullptr,
                        (const int32_t*)nullptr, (const int32_t*)nullptr, qc, kq, s.ovf);
         } else {
             idx->tc_cand.reserve((size_t)qmax * G * 32 * 8);
             auto kern = rerank_kernel<0>;
             DFX_LAUNCH(kern, (unsigned)qc, 128, (size_t)d * 4, st, xq, d, cent, cnorm, nlist, metric, s.groups, G,
-                       nprobe, s.gmin, s.gmin2, s.gargc, ng, idx->tc_cmax2, tol, idx->tc_cand.as<uint64_t>(),
+                       nprobe, s.gmin, s.gmin2, s.gargc, ng, tol, idx->tc_cand.as<uint64_t>(),
                        (int32_t*)nullptr, (const int32_t*)nullptr, (const int32_t*)nullptr, qc, (int32_t*)nullptr,
                        s.ovf);
             dfx_launch_select_comp(idx->tc_cand.as<uint64_t>(), qc, G * 32, (int64_t)G * 32, nprobe, kq, st);
@@ -1263,27 +1362,20 @@ int dfx_tc_flat_candidates(dfx_index* idx, const float* d_x, int64_t nq, int k, 
     const int64_t nl_pad = dfx_ceil_div(N, tc::TILE) * tc::TILE;
     const int ng = (int)(nl_pad / 32);
     if (idx->tc_flat_rows != N) {  // (re)build the screening table of the rows
-        const float* norms = idx->xnorm.as<float>();
-        if (metric != DFX_METRIC_L2) {  // inner product keeps no row norms: the tolerance needs their maximum
-            idx->cnorm.reserve((size_t)N * 4);
-            dfx_launch_row_norms(idx->payload.as<float>(), N, d, idx->cnorm.as<float>(), st);
-            norms = idx->cnorm.as<float>();
-        }
-        tc_install_table(idx, idx->payload.as<float>(), norms, N, st);
+        tc_install_table(idx, idx->payload.as<float>(), N, st);
         idx->tc_flat_rows = N;
     }
     tc_stats_poll(idx, st);
     const bool fast = idx->tc_fast;
-    const ScreenTol tol = tc_tol(idx, d, fast);
     int G = k + 8;
     if (G > ng) G = ng;
     const int ncand = G * 32;
     idx->tc_cand.reserve((size_t)nq * ncand * 8);
-    const Screened s = tc_screen_chunk(idx, d, d_x, nq, nq, ng, G, idx->tc_cent.p, idx->tc_cscale, fast ? 1 : 2,
-                                       idx->xnorm.as<float>(), N, metric, st);
+    const Screened s = tc_screen_chunk(idx, d, d_x, nq, nq, ng, G, idx->tc_tab, fast ? 1 : 2, N, metric, st);
+    const ScreenTol tol = tc_tol(idx, idx->tc_tab, d, fast);
     auto kern = rerank_kernel<0>;
     DFX_LAUNCH(kern, (unsigned)nq, 128, (size_t)d * 4, st, d_x, d, idx->payload.as<float>(), idx->xnorm.as<float>(), N,
-               metric, s.groups, G, k, s.gmin, s.gmin2, s.gargc, ng, idx->tc_cmax2, tol, idx->tc_cand.as<uint64_t>(),
+               metric, s.groups, G, k, s.gmin, s.gmin2, s.gargc, ng, tol, idx->tc_cand.as<uint64_t>(),
                (int32_t*)nullptr, (const int32_t*)nullptr, (const int32_t*)nullptr, nq, (int32_t*)nullptr, s.ovf);
     // rows with more near-ties than selected groups: their ncand slots become the exact top-ncand
     launch_exact_rows(d_x, idx->payload.as<float>(), idx->xnorm.as<float>(), N, d, metric, s.ovf, nq, 0, ncand,
@@ -1303,13 +1395,11 @@ void dfx_tc_assign(dfx_index* idx, int d, const float* d_cent, const float* d_cn
     const int G = ng < 6 ? ng : 6;
     const int64_t RC = std::max<int64_t>(tc::TILE, ((256ll << 20) / ((int64_t)ng * 4)) / tc::TILE * tc::TILE);
     const int64_t rmax = std::min<int64_t>(n, RC);
-    idx->tc_qn.reserve((size_t)rmax * 4);
     idx->tc_amb.reserve((size_t)(rmax + 1) * 4);
     // fp16 copy of this centroid table (k-means changes it every iteration; converting is cheap).
     // Precision: tc_mode 1 / 2 as set; AUTO decides per chunk from the counts of the chunk before
     // (read back with a sync -- this is the build path), starting PRECISE on every call.
-    const float cmax2 = max_norm2(idx, d_cnorm, nlist, st);
-    const float cscale = tc_prepare_table(d_cent, nlist, d, cmax2, 2, idx->tc_cent_tmp, st);
+    tc_prepare_table(d_cent, nlist, d, metric, idx->tc_tab_tmp, st);
     bool fast = idx->tc_mode == 1;
     int64_t acc_rows = 0, acc_bad = 0;
     for (int64_t r0 = 0, rc = 0; r0 < n; r0 += rc) {
@@ -1318,23 +1408,19 @@ void dfx_tc_assign(dfx_index* idx, int d, const float* d_cent, const float* d_cn
         rc = (idx->tc_mode == 0 && r0 == 0) ? std::min<int64_t>(n, dfx_ceil_div(idx->tc_auto_window, tc::TILE) * tc::TILE)
                                             : std::min(RC, n - r0);
         const float* xr = d_x + r0 * d;
-        ScreenTol tol;
-        tol.rel = screen_tol_rel(d, fast);
-        tol.rel_fast = 0.f;  // counted once per row by assign_resolve_kernel
-        const float rel_fast = (!fast && idx->tc_mode == 0) ? screen_tol_rel(d, true) : 0.f;
-        const Screened s = tc_screen_chunk(idx, d, xr, rc, rmax, ng, G, idx->tc_cent_tmp.p, cscale, fast ? 1 : 2,
-                                           d_cnorm, nlist, metric, st);
-        dfx_launch_row_norms(xr, rc, d, idx->tc_qn.as<float>(), st);
+        const Screened s = tc_screen_chunk(idx, d, xr, rc, rmax, ng, G, idx->tc_tab_tmp, fast ? 1 : 2, nlist, metric, st);
+        const ScreenTol tol = tc_tol(idx, idx->tc_tab_tmp, d, fast);
+        ScreenTol tol_rr = tol;
+        tol_rr.rel_fast = 0.f;  // counted once per row by assign_resolve_kernel
         int32_t* amb_count = idx->tc_amb.as<int32_t>();
         int32_t* amb_rows = amb_count + 1;
         DFX_CUDA(cudaMemsetAsync(amb_count, 0, 4, st));
-        DFX_LAUNCH(assign_resolve_kernel, (unsigned)dfx_ceil_div(rc, 256), 256, 0, st, idx->tc_qn.as<float>(),
-                   s.groups, s.gmin, s.gmin2, s.gargc, ng, G, cmax2, tol.rel, rel_fast, rc, d_assign + r0, amb_rows,
-                   amb_count, s.ovf);
+        DFX_LAUNCH(assign_resolve_kernel, (unsigned)dfx_ceil_div(rc, 256), 256, 0, st, s.groups, s.gmin, s.gmin2,
+                   s.gargc, ng, G, tol, rc, d_assign + r0, amb_rows, amb_count, s.ovf);
         auto kern = rerank_kernel<1>;
         const unsigned grid = (unsigned)std::min<int64_t>(rc, dfx_num_sms() * 16);
         DFX_LAUNCH(kern, grid, 128, (size_t)d * 4, st, xr, d, d_cent, d_cnorm, nlist, metric, s.groups, G, 1, s.gmin,
-                   s.gmin2, s.gargc, ng, cmax2, tol, (uint64_t*)nullptr, d_assign + r0, (const int32_t*)amb_rows,
+                   s.gmin2, s.gargc, ng, tol_rr, (uint64_t*)nullptr, d_assign + r0, (const int32_t*)amb_rows,
                    (const int32_t*)amb_count, rc, (int32_t*)nullptr, s.ovf);
         launch_exact_rows(xr, d_cent, d_cnorm, nlist, d, metric, s.ovf, rc, 1, 1, nullptr, d_assign + r0, nullptr, st);
         if (idx->tc_mode == 0 && r0 + rc < n) {  // AUTO: the next chunk's precision

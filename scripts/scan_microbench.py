@@ -94,6 +94,55 @@ def kernel_breakdown(idx, batch, k, iters=20):
     return out
 
 
+def screen_tol(d, fast, qn2, cmax2, qn2c=None, cmax2c=None):
+    """dfx_tc.cu's screening tolerance of a row: raw (qn2c None) as before centring, i.e.
+    4.2 err |q| max|c| + 1e-5 (max|c|^2 + 2 |q| max|c|), or centred on the centroid mean m."""
+    err = (2.0 ** -10 + 2.0 ** -22 + d * 2.0 ** -24) if fast else (3 * 2.0 ** -22 + 3 * d * 2.0 ** -24)
+    s = (qn2 * cmax2).sqrt()
+    if qn2c is None:
+        return 4.2 * err * s + 1e-5 * (cmax2 + 2 * s)
+    sc = (qn2c * cmax2c).sqrt()
+    return (4.2 * (err + 2.0 ** -23) * sc + 2.1 * (2.0 ** -18 + 2.0 ** -23) * (cmax2c + 2 * sc)
+            + 2.1 * (2.0 ** -17 + 2.0 ** -22 + d * 2.0 ** -24) * (cmax2 + 2 * s))
+
+
+def fast_overflow_rates(synth, nvec, cent, cn, nprobe, nrows=32768, margins=(8, 16, 24)):
+    """Share of `nrows` bench queries whose decide stage would overflow under FAST's tolerance:
+    the G-th smallest group minimum (exact fp32 ranking values |c|^2 - 2 q.c, groups of 32
+    centroids) within the tolerance of the nprobe-th one, G = nprobe + margin.  Raw tolerance
+    and tolerance centred on the centroid mean."""
+    g = torch.Generator(device="cpu").manual_seed(1237)
+    rows = torch.randint(0, nvec, (nrows,), generator=g, dtype=torch.int64).cuda()
+    xq = synth.rows(0, nrows, rows_t=rows, noise_stream=7)
+    d, nl = cent.shape[1], cent.shape[0]
+    m = cent.double().mean(0).float()
+    cmax2, cmax2c = float(cn.max()), float(((cent - m) ** 2).sum(1).max())
+    Gmax = nprobe + max(margins)
+    cases = {"raw_G+8": [], **{f"centred_G+{mg}": [] for mg in margins}}
+    tol_med = {"raw": [], "centred": []}
+    for r0 in range(0, nrows, 2048):
+        q = xq[r0:r0 + 2048]
+        gm = (cn[None, :] - 2.0 * q @ cent.t())[:, :nl // 32 * 32].view(q.shape[0], -1, 32).amin(2)
+        top = torch.topk(gm, Gmax, dim=1, largest=False, sorted=True).values.double()
+        t = top[:, nprobe - 1]
+        qn2, qn2c = (q.double() ** 2).sum(1), ((q - m).double() ** 2).sum(1)
+        tr = screen_tol(d, True, qn2, cmax2)
+        tc = screen_tol(d, True, qn2, cmax2, qn2c, cmax2c)
+        tol_med["raw"].append(tr)
+        tol_med["centred"].append(tc)
+        cases["raw_G+8"].append(top[:, nprobe + 8 - 1] <= t + tr)
+        for mg in margins:
+            cases[f"centred_G+{mg}"].append(top[:, nprobe + mg - 1] <= t + tc)
+    out = {"rows": nrows, "nprobe": nprobe, "cmax2": cmax2, "cmax2_centred": cmax2c,
+           "qnorm_centred_mean": float(((xq - m) ** 2).sum(1).sqrt().mean())}
+    for k, v in cases.items():
+        v = torch.cat(v)
+        out[k] = {"overflow_rows": int(v.sum()), "share": float(v.double().mean())}
+    for k, v in tol_med.items():
+        out[f"tol_median_{k}"] = float(torch.cat(v).median())
+    return out
+
+
 def main():
     label = sys.argv[1] if len(sys.argv) > 1 else "default"
     nvec = int(os.environ.get("MB_NVEC", 500_000_000))
@@ -165,10 +214,11 @@ def main():
                         "gap_8_to_9": qtl(Vs[:, 8] - Vs[:, 7]), "gap_8_to_16": qtl(Vs[:, 15] - Vs[:, 7]),
                         "gap_8_to_24": qtl(Vs[:, 23] - Vs[:, 7]), "v8": qtl(Vs[:, 7])}
     del V, Vs
-    # coarse-quantizer screening precision: AUTO state after the runs above, then both fixed modes
+    out["fast_overflow"] = fast_overflow_rates(synth, nvec, cent, cn, idx.nprobe)
+    # coarse-quantizer screening precision: AUTO state after the runs above, then the fixed modes
     stat_names = ("tc_fast", "tc_stat_rows", "tc_stat_overflow", "tc_stat_fast_would")
     out["auto_state"] = {k: idx.get_param(k) for k in stat_names}
-    for mode, name in ((2, "precise"), (0, "auto")):
+    for mode, name in ((2, "precise"), (1, "fast"), (0, "auto")):
         idx.set_param("tc_screen_mode", mode)
         for b in batches:
             idx.search_dev(b, 10)
@@ -188,6 +238,8 @@ def main():
                                  "coarse_ms": e0.elapsed_time(e1) / 12 - ms / nl,
                                  "same": bool(torch.equal(Dm, ref[0]) and torch.equal(Im, ref[1])),
                                  **{k: idx.get_param(k) for k in stat_names}}
+        if os.environ.get("MB_PROFILE", "1") != "0" and mode != 0:
+            out["breakdown_" + name] = kernel_breakdown(idx, batches[0], 10)
     if os.environ.get("MB_PROFILE", "1") != "0":  # AUTO, as left by the loop above
         out["card"] = card_info()
         out["breakdown"] = kernel_breakdown(idx, batches[0], 10)
