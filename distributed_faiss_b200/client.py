@@ -251,14 +251,14 @@ class IndexClient:
             conn.close()
 
     # ------------------------------------------------------------ the hot path
-    MAX_TOPK = 1024   # per-query results the engine selects for the IVF kinds (flat: 4096); DESIGN.md §7
+    MAX_TOPK = 4096   # per-query results the engine selects, for every index kind; DESIGN.md §7
 
     def _check_topk(self, topk: int):
         """the reference passes any k to faiss; here the limit is the engine's -- say so on the
         client instead of surfacing it as a ServerException from every shard"""
-        if not 1 <= int(topk) <= 4096:
-            raise ValueError(f"topk={topk}: this engine returns 1..{self.MAX_TOPK} results per query for the IVF "
-                             "builders (4096 for 'flat'); search_with_filter over-fetches 3x")
+        if not 1 <= int(topk) <= self.MAX_TOPK:
+            raise ValueError(f"topk={topk}: this engine returns 1..{self.MAX_TOPK} results per query; "
+                             "search_with_filter over-fetches 3x")
 
     def search(self, query, topk: int, index_id: str, return_embeddings: bool = False) -> Tuple[np.ndarray, List]:
         self._check_topk(topk)

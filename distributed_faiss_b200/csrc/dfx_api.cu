@@ -576,6 +576,7 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
         upload(idx->list_off, nbytes);
         idx->h_list_off.assign((const int64_t*)in, (const int64_t*)in + nlist + 1);
         DFX_REQUIRE(idx->h_list_off[0] == 0, "list_off[0] must be 0");
+        idx->update_list_lengths();
         idx->n_sorted = idx->h_list_off[(size_t)nlist];
         idx->n_pending = 0;
     } else if (n == "ids" && idx->is_ivf()) {

@@ -452,6 +452,7 @@ void dfx_train_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st
     }
     // an empty, trained index
     idx->h_list_off.assign((size_t)nlist + 1, 0);
+    idx->update_list_lengths();
     idx->list_off.reserve((size_t)(nlist + 1) * 8);
     DFX_CUDA(cudaMemsetAsync(idx->list_off.p, 0, (size_t)(nlist + 1) * 8, st));
     DFX_CUDA(cudaStreamSynchronize(st));
@@ -620,6 +621,7 @@ void dfx_finalize_impl(dfx_index* idx, cudaStream_t st) {
     DFX_CUDA(cudaMemcpyAsync(idx->h_list_off.data(), idx->list_off.p, (size_t)(nlist + 1) * 8,
                              cudaMemcpyDeviceToHost, st));
     DFX_CUDA(cudaStreamSynchronize(st));
+    idx->update_list_lengths();
     std::swap(idx->payload, new_payload);
     std::swap(idx->ids, new_ids);
     if (idx->cfg.kind == DFX_IVF_PQ) std::swap(idx->tvals, new_tvals);

@@ -36,6 +36,8 @@ struct dfx_index {
     DevBuf sq_trained;                  // IVF_SQ8: f32[2][d] = vmin, vdiff (faiss ScalarQuantizer::trained)
     DevBuf list_off;                    // int64[nlist+1]
     std::vector<int64_t> h_list_off;    // host mirror
+    // h_len_top[p]: vectors in the p longest lists together (bounds one query's candidates at k > 1024)
+    std::vector<int64_t> h_len_top;
     DevBuf ids;                         // int32[n_sorted] shard-local ids, list-sorted
     DevBuf payload;                     // kind-specific rows, list-sorted (FLAT: arrival order)
     DevBuf tvals;                       // IVF_PQ: f32[n_sorted]
@@ -46,6 +48,7 @@ struct dfx_index {
 
     // search workspace (grow-only)
     DevBuf w_vals, w_keys, w_dis0, w_lut, w_part, w_q, w_D, w_I, w_misc, w_best;
+    DevBuf w_coff;  // k > 1024: int64 [qc][nprobe + 1] slot offsets of the candidate rows (in w_part)
     // reconstruct support: inverse of ids (shard-local id -> storage position)
     DevBuf inv;
     bool inv_valid = false;
@@ -149,6 +152,15 @@ struct dfx_index {
         return 0;
     }
     int64_t ntotal() const { return n_sorted + n_pending; }
+    // after every change of h_list_off
+    void update_list_lengths() {
+        const size_t nl = h_list_off.empty() ? 0 : h_list_off.size() - 1;
+        std::vector<int64_t> len(nl);
+        for (size_t l = 0; l < nl; l++) len[l] = h_list_off[l + 1] - h_list_off[l];
+        std::sort(len.begin(), len.end(), [](int64_t a, int64_t b) { return a > b; });
+        h_len_top.assign(nl + 1, 0);
+        for (size_t l = 0; l < nl; l++) h_len_top[l + 1] = h_len_top[l] + len[l];
+    }
     bool is_ivf() const { return cfg.kind != DFX_FLAT; }
 };
 
@@ -203,6 +215,9 @@ void dfx_pq_il_to_rm(dfx_index* idx, cudaStream_t st);
 bool dfx_launch_scan_pq_il2(dfx_index* idx, const float* xq, int64_t qc, const int32_t* keys, int nprobe, int G,
                             int ngroups, int k, int cap, uint64_t* part, float* outD, int64_t* outI,
                             cudaStream_t st);
+// k > 1024: the same scan writing every vector's composite to its slot of the candidate rows
+void dfx_launch_scan_pq_il2_mat(dfx_index* idx, const float* xq, int64_t qc, const int32_t* keys, int nprobe, int G,
+                                int ngroups, uint64_t* cand, const int64_t* coff, cudaStream_t st);
 
 // ---- dfx_tc.cu
 bool dfx_tc_supported(int d);

@@ -35,6 +35,9 @@
 //     memory (268 MB written + 268 MB read per 4096-query launch) and the K3 launch is gone.
 //   * A CTA that owns ALL probes of its query (ngroups == 1, the large-batch regime) writes the
 //     final (D, I) rows itself; the per-query reduction launch is skipped.
+//   * MAT (k > 1024, with !REG): no candidate set.  `part` is the candidate buffer: the composite of
+//     every vector goes to slot coff[q][p] + (position in list) (dfx_cand_store); padding slots of a
+//     list's last block lie past the list's end and are not written.  outD / outI are not used.
 #pragma once
 #include "dfx_internal.h"
 #include "dfx_topk.cuh"
@@ -97,16 +100,20 @@ __device__ __noinline__ Il2Flushed il2_flush(uint64_t kept, uint64_t* queue, int
 // REG: k <= 32, register-resident top-k;  !REG: WarpTopK buffers in shared memory (any k)
 // Q [nq][d] queries; cbT: transposed codebook PT[j][m][dsub]; cent [nlist][d]; d = 32 * dsub.
 // outD / outI != nullptr (requires ngroups == 1): final faiss-style rows are written directly.
-template <bool REG, int THREADS, int MINB>
+template <bool REG, int THREADS, int MINB, bool MAT = false>
 __global__ void __launch_bounds__(THREADS, MINB)
 scan_pq_il2_kernel(const float* __restrict__ Q, const float* __restrict__ cbT, const float* __restrict__ cent, int d,
                    int dsub, const int32_t* __restrict__ keys, int nprobe, int G, int ngroups,
                    const int64_t* __restrict__ blk_off, const uint4* __restrict__ il_codes,
                    const float* __restrict__ il_tvals, const int32_t* __restrict__ il_ids, int k, int cap,
-                   uint64_t* __restrict__ part, float* __restrict__ outD, int64_t* __restrict__ outI, int pf_ahead) {
+                   uint64_t* __restrict__ part, float* __restrict__ outD, int64_t* __restrict__ outI, int pf_ahead,
+                   const int64_t* __restrict__ coff) {
     DFX_DYN_SMEM(unsigned char, smem_raw, 128);
     float* s_lut = reinterpret_cast<float*>(smem_raw);                      // [256][64]
     uint64_t* s_buf = reinterpret_cast<uint64_t*>(smem_raw + IL2_LUT_BYTES);  // queues / WarpTopK buffers
+    // MAT: slot of block b, lane v of probe p is s_cb[p] + 32 b + v, the probe's slots end at s_ce[p]
+    int64_t* s_cb = reinterpret_cast<int64_t*>(s_buf);
+    int64_t* s_ce = s_cb + IL2_MAXG;
     __shared__ unsigned int s_cta_key;  // CTA-wide admission bound (order-preserving key)
     __shared__ int s_lb[IL2_MAXG], s_le[IL2_MAXG];  // first / end block of each probed list
     __shared__ float s_ld0[IL2_MAXG];               // |q - c|^2 of each probed list
@@ -130,6 +137,11 @@ scan_pq_il2_kernel(const float* __restrict__ Q, const float* __restrict__ cbT, c
         s_lkey[tid] = l;
         s_lb[tid] = (l < 0) ? 0 : (int)blk_off[l];
         s_le[tid] = (l < 0) ? 0 : (int)blk_off[l + 1];
+        if constexpr (MAT) {
+            const int64_t* cq = coff + q * (nprobe + 1) + g * G + tid;
+            s_cb[tid] = cq[0] - 32 * (int64_t)((l < 0) ? 0 : (int)blk_off[l]);
+            s_ce[tid] = cq[1];
+        }
     }
     // ---- K3, part 1: the query's table, rows j = warp, warp + 8, ...; lane = subquantizer m.
     // seq-k order (oracle): acc = fma(q0, p0, 0), fma(q1, p1, acc), ...; entry = -2 * acc.
@@ -196,7 +208,8 @@ scan_pq_il2_kernel(const float* __restrict__ Q, const float* __restrict__ cbT, c
     float thr = __int_as_float(0x7f800000);  // value of this warp's k-th best
     uint32_t thr_sec = DFX_SEC_NONE;         // and its id
     float bnd = __int_as_float(0x7f800000);  // register copy of the CTA bound (may lag: only looser)
-    if (!REG) wt.init(s_buf + (size_t)warp * cap, cap, k, &s_cta_key);
+    if (!REG && !MAT) wt.init(s_buf + (size_t)warp * cap, cap, k, &s_cta_key);
+    int mp = 0;  // MAT: probe of the warp's current block (the warp meets its probes in increasing order)
 
     // merge 32 queued candidates into `kept` (out of line: rare, and called from three places)
     auto flush = [&]() {
@@ -225,7 +238,11 @@ scan_pq_il2_kernel(const float* __restrict__ Q, const float* __restrict__ cbT, c
         dfx_halving_tree<16>(y);
         const float v = d0 + (tv + y[0]);  // padding has tv = +inf
 
-        if (REG) {
+        if constexpr (MAT) {
+            while (pos < s_lb[mp] || pos >= s_le[mp]) mp++;
+            const int64_t dst = s_cb[mp] + (int64_t)pos * 32 + lane;
+            if (dst < s_ce[mp]) dfx_cand_store(part, dst, v, dfx_ld_nc_u(il_ids + (int64_t)pos * 32 + lane));
+        } else if (REG) {
             bool pass = v <= bnd;
             if (__any_sync(0xffffffffu, pass)) {
                 bnd = dfx_key2f(*reinterpret_cast<volatile unsigned int*>(&s_cta_key));
@@ -341,6 +358,7 @@ scan_pq_il2_kernel(const float* __restrict__ Q, const float* __restrict__ cbT, c
     }
 #undef IL2_FETCH
 
+    if constexpr (MAT) return;
     uint64_t* out = part + ((int64_t)q * ngroups + g) * k;
     if (REG) {
         if (cnt > 0) flush();

@@ -28,18 +28,20 @@
 
 constexpr int PQ4_KSUB = 16;
 
-// shared memory of one CTA: 4 per-warp candidate buffers of `cap` composites
+// shared memory of one CTA: 4 per-warp candidate buffers of `cap` composites (MAT: none)
 static inline size_t dfx_pq4_smem(int cap) { return (size_t)4 * cap * 8; }
 
 // M = 40, 72, 88: under ptxas's default register budget one value is reloaded from local memory in
 // the per-vector loop; asking for one resident block lets it keep everything in registers.  The other
 // shapes keep the default (0), which spills only outside that loop and leaves more blocks per SM.
-template <int MT>
+// MAT (k > 1024): `part` is the candidate buffer; every vector's composite goes to slot
+// coff[q][p] + (position in list) (dfx_cand_store) instead of the per-warp queues.
+template <int MT, bool MAT = false>
 __global__ void __launch_bounds__(128, (MT == 40 || MT == 72 || MT == 88) ? 1 : 0)
 scan_pq4_kernel(const float* __restrict__ lut, const float* __restrict__ dis0, const int32_t* __restrict__ keys,
                 int nprobe, int G, int ngroups, const int64_t* __restrict__ list_off,
                 const uint8_t* __restrict__ codes, const float* __restrict__ tvals, const int32_t* __restrict__ ids,
-                int k, int cap, uint64_t* __restrict__ part) {
+                int k, int cap, uint64_t* __restrict__ part, const int64_t* __restrict__ coff) {
     static_assert(MT >= 8 && MT <= 128 && MT % 8 == 0, "4-bit codes: M % 8 == 0, 8 <= M <= 128");
     constexpr int NW = MT / 8;  // 32-bit code words per row
     constexpr int P = (MT <= 8) ? 8 : (MT <= 16) ? 16 : (MT <= 32) ? 32 : (MT <= 64) ? 64 : 128;
@@ -57,7 +59,7 @@ scan_pq4_kernel(const float* __restrict__ lut, const float* __restrict__ dis0, c
         for (int j = 0; j < MT / 2; j++) T[j] = __ldg(lq + 32 * j + lane);
     }
     WarpTopK wt;
-    wt.init(s_buf + (size_t)warp * cap, cap, k);
+    if constexpr (!MAT) wt.init(s_buf + (size_t)warp * cap, cap, k);
 
     const int p_end = min(nprobe, (g + 1) * G);
     for (int p = g * G; p < p_end; p++) {
@@ -65,6 +67,8 @@ scan_pq4_kernel(const float* __restrict__ lut, const float* __restrict__ dis0, c
         if (l < 0) continue;
         const float d0 = dis0[q * nprobe + p];
         const int64_t beg = list_off[l], end = list_off[l + 1];
+        int64_t cbase = 0;  // MAT: slot of row i is cbase + i
+        if constexpr (MAT) cbase = coff[q * (nprobe + 1) + p] - beg;
         for (int64_t base = beg + warp * 32; base < end; base += 128) {  // warp-uniform trip count
             const int64_t i = base + lane;
             const bool valid = i < end;
@@ -115,10 +119,14 @@ scan_pq4_kernel(const float* __restrict__ lut, const float* __restrict__ dis0, c
             }
             if constexpr (H > 1) dfx_halving_tree<H / 2>(s);
             const float v = d0 + (t + s[0]);
-            uint32_t sec = 0;
-            const bool want = valid && wt.admits(v, [&] { return my_id; }, sec);
-            wt.push_lanes(want, v, sec);
+            if constexpr (MAT) {
+                if (valid) dfx_cand_store(part, cbase + i, v, my_id);
+            } else {
+                uint32_t sec = 0;
+                const bool want = valid && wt.admits(v, [&] { return my_id; }, sec);
+                wt.push_lanes(want, v, sec);
+            }
         }
     }
-    cta_merge_and_write<128>(wt, s_buf, cap, k, part + ((int64_t)q * ngroups + g) * k);
+    if constexpr (!MAT) cta_merge_and_write<128>(wt, s_buf, cap, k, part + ((int64_t)q * ngroups + g) * k);
 }

@@ -20,6 +20,8 @@
 //     the row-major table is kept, so the arithmetic order is the oracle's without any remapping.
 //   * THREADS (128 / 256 / 512) is chosen by the driver so that the table and one WarpTopK queue
 //     per warp fit in the device's shared memory.
+//   * MAT (k > 1024): `part` is the candidate buffer; every vector's composite goes to slot
+//     coff[q][p] + (position in list) (dfx_cand_store), and the CTA's shared memory is the table only.
 #pragma once
 #include "dfx_common.cuh"
 #include "dfx_topk.cuh"
@@ -33,13 +35,13 @@ static inline size_t dfx_pq_wide_smem(int M, int threads, int cap) {
 }
 
 // MT: M when it is a multiple of 16 known at compile time (16-byte code loads), else 0 (any M % 4 == 0)
-template <int MT, int THREADS>
+template <int MT, int THREADS, bool MAT = false>
 __global__ void __launch_bounds__(THREADS)
 scan_pq_wide_kernel(const float* __restrict__ Q, int d, int Mrt, int dsub, const float* __restrict__ codebooks,
                     const float* __restrict__ dis0, const int32_t* __restrict__ keys, int nprobe, int G,
                     int ngroups, const int64_t* __restrict__ list_off, const uint8_t* __restrict__ codes,
                     const float* __restrict__ tvals, const int32_t* __restrict__ ids, int k, int cap,
-                    uint64_t* __restrict__ part) {
+                    uint64_t* __restrict__ part, const int64_t* __restrict__ coff) {
     DFX_DYN_SMEM(unsigned char, smem_raw, 16);
     const int M = (MT > 0) ? MT : Mrt;
     float* s_lut = reinterpret_cast<float*>(smem_raw);  // [M][256]
@@ -62,7 +64,7 @@ scan_pq_wide_kernel(const float* __restrict__ Q, int d, int Mrt, int dsub, const
         }
     }
     WarpTopK wt;
-    wt.init(s_buf + (size_t)warp * cap, cap, k);
+    if constexpr (!MAT) wt.init(s_buf + (size_t)warp * cap, cap, k);
     __syncthreads();
 
     const int p_end = min(nprobe, (g + 1) * G);
@@ -71,6 +73,8 @@ scan_pq_wide_kernel(const float* __restrict__ Q, int d, int Mrt, int dsub, const
         if (l < 0) continue;
         const float d0 = dis0[q * nprobe + p];
         const int64_t beg = list_off[l], end = list_off[l + 1];
+        int64_t cbase = 0;  // MAT: slot of row i is cbase + i
+        if constexpr (MAT) cbase = coff[q * (nprobe + 1) + p] - beg;
         for (int64_t base = beg + warp * 32; base < end; base += THREADS) {
             const int64_t i = base + lane;
             const bool valid = i < end;
@@ -118,10 +122,14 @@ scan_pq_wide_kernel(const float* __restrict__ Q, int d, int Mrt, int dsub, const
                 dfx_halving_tree<32>(s);
                 v = d0 + (__ldg(tvals + i) + s[0]);
             }
-            uint32_t sec = 0;
-            const bool want = valid && wt.admits(v, [&] { return my_id; }, sec);
-            wt.push_lanes(want, v, sec);
+            if constexpr (MAT) {
+                if (valid) dfx_cand_store(part, cbase + i, v, my_id);
+            } else {
+                uint32_t sec = 0;
+                const bool want = valid && wt.admits(v, [&] { return my_id; }, sec);
+                wt.push_lanes(want, v, sec);
+            }
         }
     }
-    cta_merge_and_write<THREADS>(wt, s_buf, cap, k, part + ((int64_t)q * ngroups + g) * k);
+    if constexpr (!MAT) cta_merge_and_write<THREADS>(wt, s_buf, cap, k, part + ((int64_t)q * ngroups + g) * k);
 }

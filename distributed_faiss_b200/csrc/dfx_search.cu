@@ -11,6 +11,8 @@
 //   K4w  scan_pq_wide     64 < M <= 128: table built in shared memory + scan (dfx_scan_pq_wide_dev.cuh)
 //   K4n  scan_pq4         4-bit codes: table in registers, lookups by warp shuffle (dfx_scan_pq4_dev.cuh)
 //   K2/5 scan_rows        inverted-list scan of fp32 rows / fp16 / 8-bit residual codes
+//   K_off cand_offsets    k > 1024: slots of each query's candidate row (the list scans then write
+//                         every vector's composite, MAT = true, and select_cand picks the k best)
 //   K6   merge            cross-shard merge (float_maxheap_array_t semantics)
 // Arithmetic orders are the canonical ones of oracle/dfx_oracle.c (bit-exact parity).
 #include "dfx_internal.h"
@@ -199,22 +201,22 @@ void dfx_launch_select_comp(const uint64_t* comp, int64_t nrows, int n, int64_t 
 #include "dfx_scan_pq_wide_dev.cuh"
 #include "dfx_scan_pq4_dev.cuh"
 
-// scan_pq4_kernel<M> for the runtime M (a multiple of 8 in [8, 128], checked by dfx_create)
-template <int MT = 8>
+// scan_pq4_kernel<M, MAT> for the runtime M (a multiple of 8 in [8, 128], checked by dfx_create)
+template <bool MAT, int MT = 8>
 static void dfx_launch_scan_pq4(int M, unsigned grid, size_t smem, cudaStream_t st, const float* lut,
                                 const float* dis0, const int32_t* keys, int nprobe, int G, int ngroups,
                                 const int64_t* list_off, const uint8_t* codes, const float* tvals,
-                                const int32_t* ids, int k, int cap, uint64_t* part) {
+                                const int32_t* ids, int k, int cap, uint64_t* part, const int64_t* coff) {
     if constexpr (MT <= 128) {
         if (M != MT) {
-            dfx_launch_scan_pq4<MT + 8>(M, grid, smem, st, lut, dis0, keys, nprobe, G, ngroups, list_off, codes,
-                                        tvals, ids, k, cap, part);
+            dfx_launch_scan_pq4<MAT, MT + 8>(M, grid, smem, st, lut, dis0, keys, nprobe, G, ngroups, list_off, codes,
+                                             tvals, ids, k, cap, part, coff);
             return;
         }
-        auto kern = scan_pq4_kernel<MT>;
+        auto kern = scan_pq4_kernel<MT, MAT>;
         DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         DFX_LAUNCH(kern, grid, 128, smem, st, lut, dis0, keys, nprobe, G, ngroups, list_off, codes, tvals, ids, k,
-                   cap, part);
+                   cap, part, coff);
     } else {
         throw DfxError{"IVF-PQ with 4-bit codes: no list scan for M=" + std::to_string(M)};
     }
@@ -224,13 +226,15 @@ static void dfx_launch_scan_pq4(int M, unsigned grid, size_t smem, cudaStream_t 
 // K4: scan_pq.  one CTA = (query, group of G consecutive probes).  lane-per-vector:
 //   v = dis0 + (t + S),  S = halving-tree sum of lut[m][code_m] (oracle pq_sum)
 // =====================================================================================
-template <int MT>
+// MAT (k > 1024): `part` is the candidate buffer and every vector's composite goes to slot
+// coff[q][p] + (position in list) (dfx_cand_store); no per-warp queues, no shared memory after the table
+template <int MT, bool MAT = false>
 __global__ void __launch_bounds__(128)
 scan_pq_kernel(const float* __restrict__ lut, const float* __restrict__ dis0,
                const int32_t* __restrict__ keys, int nprobe, int G, int ngroups,
                const int64_t* __restrict__ list_off, const uint8_t* __restrict__ codes,
                const float* __restrict__ tvals, const int32_t* __restrict__ ids, int Mrt, int ksub,
-               int k, int cap, uint64_t* __restrict__ part) {
+               int k, int cap, uint64_t* __restrict__ part, const int64_t* __restrict__ coff) {
     DFX_DYN_SMEM(unsigned char, smem_raw, 16);
     const int M = (MT > 0) ? MT : Mrt;
     float* s_lut = reinterpret_cast<float*>(smem_raw);
@@ -245,7 +249,7 @@ scan_pq_kernel(const float* __restrict__ lut, const float* __restrict__ dis0,
         for (int i = tid; i < (M * ksub) / 4; i += 128) dst[i] = src[i];
     }
     WarpTopK wt;
-    wt.init(s_buf + (size_t)warp * cap, cap, k);
+    if constexpr (!MAT) wt.init(s_buf + (size_t)warp * cap, cap, k);
     __syncthreads();
 
     const int p_end = min(nprobe, (g + 1) * G);
@@ -254,6 +258,8 @@ scan_pq_kernel(const float* __restrict__ lut, const float* __restrict__ dis0,
         if (l < 0) continue;
         const float d0 = dis0[q * nprobe + p];
         const int64_t beg = list_off[l], end = list_off[l + 1];
+        int64_t cbase = 0;  // MAT: slot of row i is cbase + i
+        if constexpr (MAT) cbase = coff[q * (nprobe + 1) + p] - beg;
         for (int64_t base = beg + warp * 32; base < end; base += 128) {
             const int64_t i = base + lane;
             const bool valid = i < end;
@@ -298,12 +304,16 @@ scan_pq_kernel(const float* __restrict__ lut, const float* __restrict__ dis0,
                 dfx_halving_tree<P / 2>(val);
                 v = d0 + (__ldg(tvals + i) + val[0]);
             }
-            uint32_t sec = 0;
-            const bool want = valid && wt.admits(v, [&] { return my_id; }, sec);
-            wt.push_lanes(want, v, sec);
+            if constexpr (MAT) {
+                if (valid) dfx_cand_store(part, cbase + i, v, my_id);
+            } else {
+                uint32_t sec = 0;
+                const bool want = valid && wt.admits(v, [&] { return my_id; }, sec);
+                wt.push_lanes(want, v, sec);
+            }
         }
     }
-    cta_merge_and_write<128>(wt, s_buf, cap, k, part + ((int64_t)q * ngroups + g) * k);
+    if constexpr (!MAT) cta_merge_and_write<128>(wt, s_buf, cap, k, part + ((int64_t)q * ngroups + g) * k);
 }
 
 // =====================================================================================
@@ -326,13 +336,14 @@ __device__ __forceinline__ float dfx_sq8_component(uint32_t w, uint32_t sel, flo
     return __fmaf_rn(__fmaf_rn(c, DFX_SQ8_SCALE, DFX_SQ8_BIAS), vdiff, vmin);
 }
 
-template <int MODE, int U = 4>
+// MAT (k > 1024): as scan_pq_kernel, every vector's composite goes to its slot of the candidate row
+template <int MODE, int U = 4, bool MAT = false>
 __global__ void __launch_bounds__(128)
 scan_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent,
                  const int32_t* __restrict__ keys, int nprobe, int G, int ngroups,
                  const int64_t* __restrict__ list_off, const void* __restrict__ rows,
                  const int32_t* __restrict__ ids, int k, int cap, uint64_t* __restrict__ part,
-                 const float* __restrict__ sq_trained) {
+                 const float* __restrict__ sq_trained, const int64_t* __restrict__ coff) {
     DFX_DYN_SMEM(unsigned char, smem_raw, 16);
     float* s_q = reinterpret_cast<float*>(smem_raw);   // query (MODE 2 / 3: residual q - c)
     float* s_q0 = s_q + d;                              // MODE 2 / 3: the raw query
@@ -354,7 +365,7 @@ scan_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ c
         }
     }
     WarpTopK wt;
-    wt.init(s_buf + (size_t)warp * cap, cap, k);
+    if constexpr (!MAT) wt.init(s_buf + (size_t)warp * cap, cap, k);
     __syncthreads();
 
     const int p_end = min(nprobe, (g + 1) * G);
@@ -367,6 +378,8 @@ scan_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ c
             __syncthreads();
         }
         const int64_t beg = list_off[l], end = list_off[l + 1];
+        int64_t cbase = 0;  // MAT: slot of row i is cbase + i
+        if constexpr (MAT) cbase = coff[q * (nprobe + 1) + p] - beg;
         for (int64_t base = beg + warp * U; base < end; base += 4 * U) {
             float acc[U];
             uint32_t vid[U];
@@ -439,13 +452,17 @@ scan_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ c
                 const int64_t i = base + u;
                 float v = dfx_warp_butterfly(acc[u]);
                 if (MODE == 0) v = -v;
-                uint32_t sec = 0;
-                if (i < end && wt.admits(v, [&] { return vid[u]; }, sec))
-                    wt.push_uniform(v, sec);
+                if constexpr (MAT) {
+                    if (lane == u && i < end) dfx_cand_store(part, cbase + i, v, vid[u]);
+                } else {
+                    uint32_t sec = 0;
+                    if (i < end && wt.admits(v, [&] { return vid[u]; }, sec))
+                        wt.push_uniform(v, sec);
+                }
             }
         }
     }
-    cta_merge_and_write<128>(wt, s_buf, cap, k, part + ((int64_t)q * ngroups + g) * k);
+    if constexpr (!MAT) cta_merge_and_write<128>(wt, s_buf, cap, k, part + ((int64_t)q * ngroups + g) * k);
 }
 
 // =====================================================================================
@@ -649,6 +666,59 @@ void dfx_stats_impl(dfx_index* idx, int64_t* ndis, cudaStream_t st) {
 }
 
 // =====================================================================================
+// k > 1024.  The per-warp queues of the list scans would need 4 x 2 KP x 8 B of shared memory per
+// CTA (256 KiB at k = 4096), so the scans write the composite of every probed vector instead
+// (MAT = true) and one k-selection per query picks the result.  Row q of a query chunk holds its
+// probed lists end to end from slot q * ld; ld, the nprobe longest lists of the index together,
+// bounds every row and is known on the host, so nothing is read back from the device.
+// =====================================================================================
+// coff[q][p] = q * ld + (vectors in the lists of probes < p), coff[q][nprobe] = q * ld + n_q; a
+// missing probe (key < 0) holds none.  One warp per query; lane j sums a contiguous run of probes.
+__global__ void __launch_bounds__(128)
+cand_offsets_kernel(const int32_t* __restrict__ keys, int64_t nq, int nprobe, const int64_t* __restrict__ list_off,
+                    int64_t ld, int64_t* __restrict__ coff) {
+    const int64_t q = (int64_t)blockIdx.x * 4 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (q >= nq) return;  // warp-uniform
+    const int per = (nprobe + 31) / 32;
+    const int p0 = min(nprobe, lane * per), p1 = min(nprobe, p0 + per);
+    const int32_t* kq = keys + q * nprobe;
+    auto len = [&](int p) -> long long {
+        const int l = kq[p];
+        return l < 0 ? 0ll : (long long)(list_off[l + 1] - list_off[l]);
+    };
+    long long s = 0;
+    for (int p = p0; p < p1; p++) s += len(p);
+    long long incl = s;  // inclusive prefix over the lanes
+    for (int off = 1; off < 32; off <<= 1) {
+        const long long o = __shfl_sync(0xffffffffu, incl, lane >= off ? lane - off : 0);
+        if (lane >= off) incl += o;
+    }
+    int64_t* out = coff + q * (nprobe + 1);
+    long long c = q * ld + (incl - s);
+    for (int p = p0; p < p1; p++) {
+        out[p] = c;
+        c += len(p);
+    }
+    if (lane == 31) out[nprobe] = q * ld + incl;
+}
+
+struct SlotLoader {  // one candidate row
+    const uint64_t* c;
+    __device__ __forceinline__ uint64_t operator()(int64_t, int e) const { return c[e]; }
+};
+// one CTA per query: the k best of its n_q candidates, each row with its own length
+template <int THREADS>
+__global__ void __launch_bounds__(THREADS)
+select_cand_kernel(const uint64_t* __restrict__ cand, const int64_t* __restrict__ coff, int nprobe, ResultWriter wr,
+                   int k, int P, int sort_cap) {
+    DFX_DYN_SMEM(unsigned char, smem_raw, 16);
+    const int64_t q = blockIdx.x;
+    const int64_t b = coff[q * (nprobe + 1)], n = coff[q * (nprobe + 1) + nprobe] - b;
+    dfx_select_row<THREADS>(SlotLoader{cand + b}, wr, q, (int)n, k, P, sort_cap, reinterpret_cast<uint64_t*>(smem_raw));
+}
+
+// =====================================================================================
 // the per-shard search driver
 // =====================================================================================
 static int choose_group(int64_t nq, int nprobe) {
@@ -738,10 +808,22 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
     }
 
     // ---------------- IVF kinds
-    DFX_REQUIRE(k64 <= 1024, "IVF search supports k <= 1024");
+    DFX_REQUIRE(k64 <= 4096, "IVF search supports k <= 4096");
     const int64_t nlist = idx->cfg.nlist;
     int nprobe = (int)std::min<int64_t>(std::max<int64_t>(idx->nprobe, 1), nlist);
     DFX_REQUIRE(nprobe <= 4096, "nprobe <= 4096");
+    // k > 1024: candidate rows instead of per-warp queues; ld = slots per row
+    const bool mat = k > 1024;
+    const int64_t part_max = (int64_t)1 << 24;  // composites of a chunk's partial results / candidates (128 MiB)
+    int64_t ld = 0;
+    if (mat) {
+        DFX_REQUIRE(idx->h_len_top.size() == (size_t)nlist + 1, "IVF search: list lengths are not known");
+        ld = std::max<int64_t>(idx->h_len_top[(size_t)nprobe], 1);
+        DFX_REQUIRE(ld <= part_max,
+                    "IVF search at k=" + std::to_string(k) + " with nprobe=" + std::to_string(nprobe) +
+                        ": one query's candidates can reach " + std::to_string(ld) +
+                        " vectors (the nprobe longest lists), more than the 16777216 (128 MiB) of a query chunk");
+    }
     const int cmetric = idx->cfg.metric;  // coarse quantizer metric
     const int smetric = (kind == DFX_IVF_FLAT) ? idx->cfg.metric : DFX_METRIC_L2;
 
@@ -753,10 +835,12 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
     if (QC > 8192) QC = 8192;
     // the chunk's partial results (qc x ngroups x k composites) stay within the values matrix's
     // 128 MiB: cap QC against ngroups <= nprobe, then once more against the ngroups choose_group
-    // gives at that cap (choose_group never gives a larger chunk more groups per query)
-    const int64_t part_max = (int64_t)1 << 24;
+    // gives at that cap (choose_group never gives a larger chunk more groups per query).
+    // k > 1024: the chunk's candidate rows (qc x ld composites) stay within the same 128 MiB.
     const int64_t q1 = std::max<int64_t>(1, part_max / ((int64_t)nprobe * k));
-    if (QC > q1) {
+    if (mat) {
+        QC = std::min(QC, part_max / ld);
+    } else if (QC > q1) {
         const int G1 = choose_group(q1, nprobe);
         const int64_t ng1 = (nprobe + G1 - 1) / G1;
         QC = std::min(QC, std::max(q1, part_max / (ng1 * k)));
@@ -767,15 +851,18 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
 
     // IVF-PQ with 64 < M <= 128 (scan_pq_wide_kernel): the widest CTA whose table and per-warp
     // queues fit in the device's shared memory, decided before anything is launched
+    // (k > 1024: no queues, the table alone; the 512-thread shape, the only one instantiated)
     int wide_threads = 0;
     if (kind == DFX_IVF_PQ && idx->M > 64) {
         const size_t optin = (size_t)dfx_smem_optin();
         for (int t : {512, 256, 128}) {
-            if (dfx_pq_wide_smem(idx->M, t, cap) <= optin) {
+            if (dfx_pq_wide_smem(idx->M, t, mat ? 0 : cap) <= optin) {
                 wide_threads = t;
                 break;
             }
         }
+        DFX_REQUIRE(!mat || wide_threads == 512, "IVF-PQ with " + std::to_string(idx->M) +
+                                                     " sub-quantizers: the table does not fit in shared memory");
         DFX_REQUIRE(wide_threads > 0,
                     "IVF-PQ with " + std::to_string(idx->M) + " sub-quantizers at k=" + std::to_string(k) +
                         ": the distance table and the candidate queues need " +
@@ -785,6 +872,11 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
 
     idx->w_keys.reserve((size_t)nq * nprobe * 4);
     int32_t* keys_all = idx->w_keys.as<int32_t>();
+    int64_t* coff = nullptr;  // k > 1024: [qc][nprobe + 1] slot offsets of the candidate rows
+    if (mat) {
+        idx->w_coff.reserve((size_t)QC * (nprobe + 1) * 8);
+        coff = idx->w_coff.as<int64_t>();
+    }
 
     for (int64_t q0 = 0; q0 < nq; q0 += QC) {
         const int64_t qc = (nq - q0 < QC) ? (nq - q0) : QC;
@@ -802,8 +894,12 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
         }
         const int G = choose_group(qc, nprobe);
         const int ngroups = (nprobe + G - 1) / G;
-        idx->w_part.reserve((size_t)qc * ngroups * k * 8);
+        // k > 1024: `part` holds the candidate rows
+        idx->w_part.reserve(mat ? (size_t)qc * ld * 8 : (size_t)qc * ngroups * k * 8);
         uint64_t* part = idx->w_part.as<uint64_t>();
+        if (mat)
+            DFX_LAUNCH(cand_offsets_kernel, (unsigned)dfx_ceil_div(qc, 4), 128, 0, st, keys, qc, nprobe,
+                       idx->list_off.as<int64_t>(), ld, coff);
         std::pair<cudaEvent_t, cudaEvent_t>* pev = nullptr;
         if (idx->prof_on) {
             if (idx->prof_used == idx->prof_events.size()) {
@@ -826,15 +922,16 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
             DFX_LAUNCH(pq_prep_kernel, (unsigned)qc, 256, prep_smem, st, xq, d, M, PQ4_KSUB, idx->dsub,
                        idx->codebooks.as<float>(), idx->centroids.as<float>(), keys, nprobe,
                        idx->w_lut.as<float>(), idx->w_dis0.as<float>());
-            dfx_launch_scan_pq4(M, (unsigned)(qc * ngroups), dfx_pq4_smem(cap), st, idx->w_lut.as<float>(),
-                                idx->w_dis0.as<float>(), keys, nprobe, G, ngroups, idx->list_off.as<int64_t>(),
-                                idx->payload.as<uint8_t>(), idx->tvals.as<float>(), idx->ids.as<int32_t>(), k, cap,
-                                part);
+            auto launch = mat ? dfx_launch_scan_pq4<true> : dfx_launch_scan_pq4<false>;
+            launch(M, (unsigned)(qc * ngroups), mat ? 0 : dfx_pq4_smem(cap), st, idx->w_lut.as<float>(),
+                   idx->w_dis0.as<float>(), keys, nprobe, G, ngroups, idx->list_off.as<int64_t>(),
+                   idx->payload.as<uint8_t>(), idx->tvals.as<float>(), idx->ids.as<int32_t>(), k, cap, part, coff);
         } else if (kind == DFX_IVF_PQ && idx->il) {
             // M == 32: table build + exact |q-c|^2 + block scan in ONE kernel; with a single probe
             // group per query it also writes the final rows (dfx_scan_il2.cu)
-            final_written = dfx_launch_scan_pq_il2(idx, xq, qc, keys, nprobe, G, ngroups, k, cap, part, d_D + q0 * k,
-                                                   d_I + q0 * k, st);
+            if (mat) dfx_launch_scan_pq_il2_mat(idx, xq, qc, keys, nprobe, G, ngroups, part, coff, st);
+            else final_written = dfx_launch_scan_pq_il2(idx, xq, qc, keys, nprobe, G, ngroups, k, cap, part,
+                                                        d_D + q0 * k, d_I + q0 * k, st);
         } else if (kind == DFX_IVF_PQ && idx->M > 64) {
             // 64 < M <= 128: the scan kernel builds the query's table in its own shared memory, so
             // only |q - c|^2 of the probed lists is prepared here (no w_lut)
@@ -844,10 +941,11 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
             DFX_LAUNCH(pq_prep_kernel, (unsigned)qc, 256, prep_smem, st, xq, d, M, idx->ksub, idx->dsub,
                        idx->codebooks.as<float>(), idx->centroids.as<float>(), keys, nprobe, (float*)nullptr,
                        idx->w_dis0.as<float>());
-            const size_t smem = dfx_pq_wide_smem(M, wide_threads, cap);
+            const size_t smem = dfx_pq_wide_smem(M, wide_threads, mat ? 0 : cap);
 #define DFX_SCAN_PQ_WIDE(MT)                                                                     \
     do {                                                                                         \
-        auto kern = (wide_threads == 512)   ? scan_pq_wide_kernel<MT, 512>                       \
+        auto kern = mat                     ? scan_pq_wide_kernel<MT, 512, true>                 \
+                    : (wide_threads == 512) ? scan_pq_wide_kernel<MT, 512>                       \
                     : (wide_threads == 256) ? scan_pq_wide_kernel<MT, 256>                       \
                                             : scan_pq_wide_kernel<MT, 128>;                      \
         DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,         \
@@ -855,7 +953,7 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
         DFX_LAUNCH(kern, (unsigned)(qc * ngroups), wide_threads, smem, st, xq, d, M, idx->dsub,  \
                    idx->codebooks.as<float>(), idx->w_dis0.as<float>(), keys, nprobe, G, ngroups, \
                    idx->list_off.as<int64_t>(), idx->payload.as<uint8_t>(), idx->tvals.as<float>(), \
-                   idx->ids.as<int32_t>(), k, cap, part);                                        \
+                   idx->ids.as<int32_t>(), k, cap, part, coff);                                  \
     } while (0)
             if (M == 128) DFX_SCAN_PQ_WIDE(128);
             else if (M == 96) DFX_SCAN_PQ_WIDE(96);
@@ -870,16 +968,16 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
                        idx->codebooks.as<float>(), idx->centroids.as<float>(), keys, nprobe,
                        idx->w_lut.as<float>(), idx->w_dis0.as<float>());
             {
-            const size_t smem = (size_t)M * ksub * 4 + (size_t)4 * cap * 8;
+            const size_t smem = (size_t)M * ksub * 4 + (mat ? 0 : (size_t)4 * cap * 8);
 #define DFX_SCAN_PQ(MT)                                                                          \
     do {                                                                                         \
-        auto kern = scan_pq_kernel<MT>;                                                          \
+        auto kern = mat ? scan_pq_kernel<MT, true> : scan_pq_kernel<MT>;                         \
         DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,         \
                                       (int)smem));                                               \
         DFX_LAUNCH(kern, (unsigned)(qc * ngroups), 128, smem, st, idx->w_lut.as<float>(),        \
                    idx->w_dis0.as<float>(), keys, nprobe, G, ngroups, idx->list_off.as<int64_t>(), \
                    idx->payload.as<uint8_t>(), idx->tvals.as<float>(), idx->ids.as<int32_t>(), M, \
-                   ksub, k, cap, part);                                                          \
+                   ksub, k, cap, part, coff);                                                    \
     } while (0)
             if (M == 32) DFX_SCAN_PQ(32);
             else if (M == 64) DFX_SCAN_PQ(64);
@@ -891,18 +989,19 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
         } else {
             // shared memory: the query; + the raw query (SQ16); + vmin and vdiff (SQ8)
             const int dq = (kind == DFX_IVF_SQ8) ? 4 * d : (kind == DFX_IVF_SQ16) ? 2 * d : d;
-            const size_t smem = (((size_t)dq * 4 + 15) / 16) * 16 + (size_t)4 * cap * 8;
+            const size_t smem = (((size_t)dq * 4 + 15) / 16) * 16 + (mat ? 0 : (size_t)4 * cap * 8);
             // vectors in flight per warp: rows of up to 1 KB need 8 to cover the DRAM latency,
             // longer rows keep 4 (rows_inflight overrides)
             const int inflight = idx->rows_inflight ? idx->rows_inflight : (idx->row_bytes() <= 1024 ? 8 : 4);
 #define DFX_SCAN_ROWS(MODE)                                                                      \
     do {                                                                                         \
-        auto kern = (inflight == 8) ? scan_rows_kernel<MODE, 8> : scan_rows_kernel<MODE, 4>; \
+        auto kern = (inflight == 8) ? (mat ? scan_rows_kernel<MODE, 8, true> : scan_rows_kernel<MODE, 8>) \
+                                    : (mat ? scan_rows_kernel<MODE, 4, true> : scan_rows_kernel<MODE, 4>); \
         DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,         \
                                       (int)smem));                                               \
         DFX_LAUNCH(kern, (unsigned)(qc * ngroups), 128, smem, st, xq, d, idx->centroids.as<float>(), \
                    keys, nprobe, G, ngroups, idx->list_off.as<int64_t>(), idx->payload.p,        \
-                   idx->ids.as<int32_t>(), k, cap, part, idx->sq_trained.as<float>());           \
+                   idx->ids.as<int32_t>(), k, cap, part, idx->sq_trained.as<float>(), coff);     \
     } while (0)
             if (kind == DFX_IVF_SQ8) DFX_SCAN_ROWS(3);
             else if (kind == DFX_IVF_SQ16) DFX_SCAN_ROWS(2);
@@ -911,7 +1010,13 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
 #undef DFX_SCAN_ROWS
         }
         if (pev) DFX_CUDA(cudaEventRecord(pev->second, st));
-        if (!final_written) {
+        if (mat) {
+            // P >= 2048 = sort_cap: a row of up to sort_cap candidates is sorted whole
+            const int P = dfx_next_pow2(k);
+            ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, smetric, nullptr};
+            DFX_LAUNCH(select_cand_kernel<256>, (unsigned)qc, 256, (size_t)P * 8, st, part, coff, nprobe, wr, k, P,
+                       2048);
+        } else if (!final_written) {
             CompLoader ldr{part, (int64_t)ngroups * k};
             ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, smetric, nullptr};
             dfx_launch_select<128>(ldr, wr, qc, ngroups * k, k, st);

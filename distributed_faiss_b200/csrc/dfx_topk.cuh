@@ -103,6 +103,13 @@ struct WarpTopK {
     }
 };
 
+// The other sink of the list scans (MAT = true, searches with k > 1024): the composite of every
+// scanned vector goes to its own slot of the query's candidate row, and one k-selection per query
+// picks the result (dfx_search.cu).  WarpTopK::admits never takes a NaN value; it is stored as "none".
+__device__ __forceinline__ void dfx_cand_store(uint64_t* cand, int64_t pos, float v, uint32_t id) {
+    cand[pos] = (v == v) ? dfx_comp(v, id) : DFX_COMP_NONE;
+}
+
 // merges the per-warp sets of a CTA and writes k composites (NONE padded) to out.
 // Each warp first sorts and cuts its own set to <= k entries; only those live entries
 // (NW*k of the NW*cap slots) are then packed densely and sorted by the CTA.

@@ -97,8 +97,8 @@ int dfx_set_param(dfx_index *idx, const char *name, double value);
  * next screening launch will use: 1 = FAST), "tc_stat_rows" / "tc_stat_overflow" /
  * "tc_stat_fast_would" (rows, rows re-done exactly, and rows FAST would have re-done, of the last
  * launch whose statistics came back; synchronises with that launch), "workspace_bytes" (bytes of
- * the partial-result workspace, the largest any search so far has needed; IVF searches keep it
- * within 128 MiB by their query chunk) */
+ * the partial-result workspace, the largest any search so far has needed, including the candidate
+ * rows of IVF searches with k > 1024; IVF searches keep it within 128 MiB by their query chunk) */
 int dfx_get_param(dfx_index *idx, const char *name, double *value);
 /* pre-size the shard for n_total vectors (optional; avoids regrowth while bulk loading) */
 int dfx_reserve(dfx_index *idx, int64_t n_total);
@@ -106,7 +106,9 @@ int dfx_reserve(dfx_index *idx, int64_t n_total);
 int dfx_finalize(dfx_index *idx, void *stream);
 
 /* ---- THE HOT PATH: faiss_index.search(query_batch, top_k) index.py:257 ----
- * D float32[nq,k], I int64[nq,k]. */
+ * D float32[nq,k], I int64[nq,k], 1 <= k <= 4096 for every kind.  An IVF search with k > 1024
+ * writes every probed vector's candidate and selects per query; it raises an error before launching
+ * anything when the nprobe longest lists together exceed 2^24 vectors (128 MiB of candidates). */
 int dfx_search(dfx_index *idx, int64_t nq, const float *x, int64_t k, float *D, int64_t *I);
 int dfx_search_dev(dfx_index *idx, int64_t nq, const float *d_x, int64_t k, float *d_D,
                    int64_t *d_I, void *stream);
