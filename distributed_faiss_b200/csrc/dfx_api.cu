@@ -102,7 +102,7 @@ int dfx_debug_tc_screen(dfx_index* idx, int64_t nq, const float* d_x, int npl, f
 int dfx_create(const dfx_cfg* cfg, dfx_index** out) {
     DFX_API_BEGIN
     DFX_REQUIRE(cfg && out, "null argument");
-    DFX_REQUIRE(cfg->kind >= DFX_FLAT && cfg->kind <= DFX_IVF_SQ8, "unknown index kind");
+    DFX_REQUIRE(cfg->kind >= DFX_FLAT && cfg->kind <= DFX_IVF_PQ_FS, "unknown index kind");
     DFX_REQUIRE(cfg->metric == DFX_METRIC_IP || cfg->metric == DFX_METRIC_L2,
                 "Only dot and l2 metrics are supported.");
     DFX_REQUIRE(cfg->d > 0 && cfg->d <= 4096, "dimension must be in [1, 4096]");
@@ -133,6 +133,19 @@ int dfx_create(const dfx_cfg* cfg, dfx_index** out) {
         }
         idx->M = cfg->pq_m;
         idx->ksub = 1 << cfg->pq_nbits;
+        idx->dsub = cfg->d / cfg->pq_m;
+    }
+    if (cfg->kind == DFX_IVF_PQ_FS) {
+        // the list scan sums 8-bit quantized L2 tables; there is no inner-product table
+        DFX_REQUIRE(cfg->metric == DFX_METRIC_L2,
+                    "IVF-PQ FastScan: only the L2 metric is supported (for the index and its coarse quantizer)");
+        DFX_REQUIRE(cfg->pq_nbits == 4,
+                    "IVF-PQ FastScan: 4 bits per sub-quantizer, got " + std::to_string(cfg->pq_nbits));
+        DFX_REQUIRE(cfg->pq_m >= 8 && cfg->pq_m <= 128 && cfg->pq_m % 8 == 0 && cfg->d % cfg->pq_m == 0,
+                    "IVF-PQ FastScan: the number of sub-quantizers must be a multiple of 8 in [8, 128] that "
+                    "divides d, got M=" + std::to_string(cfg->pq_m) + ", d=" + std::to_string(cfg->d));
+        idx->M = cfg->pq_m;
+        idx->ksub = 16;
         idx->dsub = cfg->d / cfg->pq_m;
     }
     DeviceGuard g(cfg->device);
@@ -480,6 +493,7 @@ static const char* payload_name(int kind) {
         case DFX_IVF_PQ: return "codes";
         case DFX_IVF_SQ16: return "codes16";
         case DFX_IVF_SQ8: return "codes8";
+        case DFX_IVF_PQ_FS: return "codes";
     }
     return "";
 }
@@ -512,9 +526,9 @@ int dfx_get_array(dfx_index* idx, const char* name, void* out, int64_t max_bytes
     int64_t bytes = 0;
     bool widen_ids = false;
     // 4-bit IVF-PQ codes are stored packed (two per byte) and exchanged one code per byte
-    const bool unpack4 = n == "codes" && idx->cfg.kind == DFX_IVF_PQ && idx->ksub == 16;
+    const bool unpack4 = n == "codes" && idx->has_pq() && idx->ksub == 16;
     if (n == "centroids" && idx->is_ivf() && idx->trained) { src = idx->centroids.p; bytes = nlist * d * 4; }
-    else if (n == "codebooks" && idx->cfg.kind == DFX_IVF_PQ && idx->trained) { src = idx->codebooks.p; bytes = (int64_t)idx->M * idx->ksub * idx->dsub * 4; }
+    else if (n == "codebooks" && idx->has_pq() && idx->trained) { src = idx->codebooks.p; bytes = (int64_t)idx->M * idx->ksub * idx->dsub * 4; }
     else if (n == "sq_trained" && idx->cfg.kind == DFX_IVF_SQ8 && idx->trained) { src = idx->sq_trained.p; bytes = 2 * d * 4; }
     else if (n == "list_off" && idx->is_ivf() && idx->trained) { src = idx->list_off.p; bytes = (nlist + 1) * 8; }
     else if (n == "ids" && idx->is_ivf()) { widen_ids = true; bytes = nt * 8; }
@@ -564,7 +578,7 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
         idx->cnorm.reserve((size_t)nlist * 4);
         dfx_launch_row_norms(idx->centroids.as<float>(), nlist, (int)d, idx->cnorm.as<float>(), idx->stream);
         DFX_CUDA(cudaStreamSynchronize(idx->stream));
-    } else if (n == "codebooks" && idx->cfg.kind == DFX_IVF_PQ) {
+    } else if (n == "codebooks" && idx->has_pq()) {
         DFX_REQUIRE(nbytes == (int64_t)idx->M * idx->ksub * idx->dsub * 4, "codebooks: wrong size");
         upload(idx->codebooks, nbytes);
         idx->cbT_valid = false;
@@ -601,7 +615,7 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
                 dfx_launch_row_norms(idx->payload.as<float>(), idx->n_sorted, (int)d, idx->xnorm.as<float>(), idx->stream);
                 DFX_CUDA(cudaStreamSynchronize(idx->stream));
             }
-        } else if (idx->cfg.kind == DFX_IVF_PQ && idx->ksub == 16) {
+        } else if (idx->has_pq() && idx->ksub == 16) {
             DFX_REQUIRE(nbytes == idx->n_sorted * (int64_t)idx->M,
                         "codes: wrong size (one byte per code, u8[ntotal, M]; set list_off first)");
             const uint8_t* s = (const uint8_t*)in;
@@ -637,6 +651,7 @@ int dfx_import_done(dfx_index* idx) {
             dfx_compute_tvals_sorted(idx, idx->stream);  // K7 recomputes the per-vector term
             dfx_pq_rm_to_il(idx, idx->stream);
         }
+        if (idx->cfg.kind == DFX_IVF_PQ_FS) DFX_REQUIRE(idx->codebooks.p, "import: codebooks are required");
         if (idx->cfg.kind == DFX_IVF_SQ8) DFX_REQUIRE(idx->sq_trained.p, "import: sq_trained is required");
         dfx_tc_prepare_centroids(idx, idx->stream);
         DFX_CUDA(cudaStreamSynchronize(idx->stream));

@@ -79,7 +79,8 @@ __global__ void split_cluster_kernel(float* cent, int d, int empty, int big) {
 
 // PQ encode: grid (ceil(n/256), M); code_m = argmin_j l2_seq(r_m, P[m][j]), ties -> smaller j.
 // The residual sub-vector lives in registers (DS = dsub when it is one of the common sizes).
-template <int DS>
+// RES = false (IVF-PQ FastScan, not by_residual): r = x itself; cent and assign are not read.
+template <int DS, bool RES = true>
 __global__ void __launch_bounds__(256)
 pq_encode_kernel(const float* __restrict__ x, const float* __restrict__ cent,
                  const int32_t* __restrict__ assign, int64_t n, int d, int M, int ksub, int dsub,
@@ -92,13 +93,13 @@ pq_encode_kernel(const float* __restrict__ x, const float* __restrict__ cent,
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     const float* xi = x + i * d + m * dsub;
-    const float* c = cent + (size_t)assign[i] * d + m * dsub;
+    const float* c = RES ? cent + (size_t)assign[i] * d + m * dsub : nullptr;
     float best = FLT_MAX;
     int bj = 0;
     if (DS > 0) {
         float r[DS > 0 ? DS : 1];
 #pragma unroll
-        for (int t = 0; t < DS; t++) r[t] = xi[t] - c[t];
+        for (int t = 0; t < DS; t++) r[t] = RES ? xi[t] - c[t] : xi[t];
         for (int j = 0; j < ksub; j++) {
             float acc = 0.f;
 #pragma unroll
@@ -115,7 +116,7 @@ pq_encode_kernel(const float* __restrict__ x, const float* __restrict__ cent,
         for (int j = 0; j < ksub; j++) {
             float acc = 0.f;
             for (int t = 0; t < dsub; t++) {
-                float df = (xi[t] - c[t]) - s_cb[j * dsub + t];
+                float df = (RES ? xi[t] - c[t] : xi[t]) - s_cb[j * dsub + t];
                 acc = __fmaf_rn(df, df, acc);
             }
             if (acc < best) {
@@ -175,15 +176,6 @@ __global__ void sq_encode_kernel(const float* __restrict__ x, const float* __res
     int64_t i = t / d;
     int c = (int)(t - i * d);
     codes[t] = __float2half_rn(x[t] - cent[(size_t)assign[i] * d + c]);
-}
-
-// IEEE division, round to nearest (spelled out so that no compiler setting can relax it)
-__device__ __forceinline__ float dfx_div_rn(float a, float b) {
-#ifdef DFX_EMU
-    return a / b;
-#else
-    return __fdiv_rn(a, b);
-#endif
 }
 
 // IVF-SQ8 encode (faiss QT_8bit, non-uniform, by_residual; DESIGN.md section 2): per component
@@ -427,6 +419,22 @@ void dfx_train_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st
                           idx->codebooks.as<float>() + (size_t)m * ksub * dsub, st);
         }
     }
+    if (kind == DFX_IVF_PQ_FS) {
+        // FastScan is not by_residual: the 16-centroid sub-quantizers are trained on the raw
+        // sub-vectors of the first min(nt, 256 * ksub) rows of the k-means sample
+        const int M = idx->M, ksub = idx->ksub, dsub = idx->dsub;
+        const int64_t ns = std::min<int64_t>(nt, 256ll * ksub);
+        DFX_REQUIRE(ns >= ksub, "train: need at least " + std::to_string(ksub) + " vectors for PQ");
+        DevBuf d_subv;
+        d_subv.reserve((size_t)ns * dsub * 4);
+        idx->codebooks.reserve((size_t)M * ksub * dsub * 4);
+        for (int m = 0; m < M; m++) {
+            DFX_LAUNCH(gather_rows_kernel, blocks_for(ns * dsub, 256), 256, 0, st, xt, (const int32_t*)nullptr, ns,
+                       dsub, m * dsub, d, d_subv.as<float>());
+            kmeans_device(idx, dsub, ns, d_subv.as<float>(), ksub, niter, seed + 1 + m,
+                          idx->codebooks.as<float>() + (size_t)m * ksub * dsub, st);
+        }
+    }
     if (kind == DFX_IVF_SQ8) {
         // faiss ScalarQuantizer (QT_8bit, RS_minmax) on the residuals of the first min(nt, 100000)
         // rows of the k-means sample, the way the PQ above takes a prefix of it
@@ -535,6 +543,27 @@ void dfx_add_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) 
             DFX_LAUNCH(pq_pack4_kernel, blocks_for(n * M / 2, 256), 256, 0, st, (const uint8_t*)enc,
                        n * M / 2, (uint8_t*)prow);
         // (`unpacked` is freed on return: cudaFree waits for the kernels above)
+    } else if (kind == DFX_IVF_PQ_FS) {
+        // the codes of the raw vector (no residual, no t-value), one per byte, then packed
+        const int M = idx->M, ksub = idx->ksub, dsub = idx->dsub;
+        DevBuf unpacked;
+        unpacked.reserve((size_t)n * M);
+        dim3 grid(blocks_for(n, 256), (unsigned)M);
+#define DFX_PQ_ENCODE_RAW(DS)                                                                   \
+    do {                                                                                        \
+        auto kern = pq_encode_kernel<DS, false>;                                                \
+        DFX_LAUNCH(kern, grid, 256, (size_t)ksub * dsub * 4, st, d_x, (const float*)nullptr,    \
+                   (const int32_t*)nullptr, n, d, M, ksub, dsub, idx->codebooks.as<float>(),    \
+                   unpacked.as<uint8_t>());                                                     \
+    } while (0)
+        if (dsub == 2) DFX_PQ_ENCODE_RAW(2);
+        else if (dsub == 4) DFX_PQ_ENCODE_RAW(4);
+        else if (dsub == 8) DFX_PQ_ENCODE_RAW(8);
+        else if (dsub == 16) DFX_PQ_ENCODE_RAW(16);
+        else DFX_PQ_ENCODE_RAW(0);
+#undef DFX_PQ_ENCODE_RAW
+        DFX_LAUNCH(pq_pack4_kernel, blocks_for(n * M / 2, 256), 256, 0, st, (const uint8_t*)unpacked.as<uint8_t>(),
+                   n * M / 2, (uint8_t*)prow);
     } else if (kind == DFX_IVF_SQ16) {
         DFX_LAUNCH(sq_encode_kernel, blocks_for(n * d, 256), 256, 0, st, d_x, idx->centroids.as<float>(),
                    plist, n, d, (__half*)prow);
@@ -721,6 +750,28 @@ __global__ void sq8_reconstruct_kernel(int d, int64_t ntotal, int64_t nlist, con
     }
 }
 
+// IVF-PQ FastScan: x_m = P[m][code_m], no centroid (the codes are of the raw vector).  Ids as
+// reconstruct_kernel.
+__global__ void pq_fs_reconstruct_kernel(int d, int M, int dsub, int64_t ntotal, const int64_t* __restrict__ want,
+                                         const int32_t* __restrict__ inv, const uint8_t* __restrict__ codes,
+                                         const float* __restrict__ codebooks, float* __restrict__ out, int64_t tag) {
+    const int64_t r = blockIdx.x;
+    int64_t id = want[r];
+    if (tag >= 0) {
+        if (id < 0 || ((id >> 40) & 0xfffff) != tag) return;
+        id &= (1ll << 40) - 1;
+    }
+    if (id < 0 || id >= ntotal) {
+        for (int k = threadIdx.x; k < d; k += blockDim.x) out[r * d + k] = __int_as_float(0x7fc00000);
+        return;
+    }
+    const int64_t pos = inv[id];
+    for (int k = threadIdx.x; k < d; k += blockDim.x) {
+        const int m = k / dsub;
+        out[r * d + k] = codebooks[((size_t)m * 16 + dfx_pq_code<4>(codes, pos, M, m)) * dsub + (k - m * dsub)];
+    }
+}
+
 void dfx_reconstruct_impl(dfx_index* idx, int64_t n, const int64_t* d_ids, float* d_out,
                           cudaStream_t st, int64_t tag) {
     if (n <= 0) return;
@@ -739,6 +790,11 @@ void dfx_reconstruct_impl(dfx_index* idx, int64_t n, const int64_t* d_ids, float
         DFX_LAUNCH(sq8_reconstruct_kernel, (unsigned)n, 128, 0, st, idx->cfg.d, nt, idx->cfg.nlist, d_ids,
                    idx->inv.as<int32_t>(), idx->payload.as<uint8_t>(), idx->list_off.as<int64_t>(),
                    idx->centroids.as<float>(), idx->sq_trained.as<float>(), d_out, tag);
+        return;
+    }
+    if (idx->cfg.kind == DFX_IVF_PQ_FS) {
+        DFX_LAUNCH(pq_fs_reconstruct_kernel, (unsigned)n, 128, 0, st, idx->cfg.d, idx->M, idx->dsub, nt, d_ids,
+                   idx->inv.as<int32_t>(), idx->payload.as<uint8_t>(), idx->codebooks.as<float>(), d_out, tag);
         return;
     }
     auto kern = (idx->cfg.kind == DFX_IVF_PQ && idx->ksub == 16) ? reconstruct_kernel<4> : reconstruct_kernel<8>;

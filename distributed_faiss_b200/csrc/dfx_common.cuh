@@ -172,6 +172,15 @@ __device__ __forceinline__ float dfx_rank_value(float ip, int metric, const floa
     return (metric == DFX_METRIC_IP) ? -ip : __fmaf_rn(-2.f, ip, xnorm[col]);
 }
 
+// IEEE division, round to nearest (spelled out so that no compiler setting can relax it)
+__device__ __forceinline__ float dfx_div_rn(float a, float b) {
+#ifdef DFX_EMU
+    return a / b;
+#else
+    return __fdiv_rn(a, b);
+#endif
+}
+
 // code of sub-quantizer m of row i of IVF-PQ codes stored with NB bits per code: NB = 8, one byte
 // per code (u8[n][M]); NB = 4, packed as faiss does (u8[n][M / 2], code m in nibble m & 1 of byte
 // m >> 1, low nibble first)

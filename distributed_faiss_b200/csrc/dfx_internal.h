@@ -40,7 +40,7 @@ struct dfx_index {
     std::vector<int64_t> h_len_top;
     DevBuf ids;                         // int32[n_sorted] shard-local ids, list-sorted
     DevBuf payload;                     // kind-specific rows, list-sorted (FLAT: arrival order)
-    DevBuf tvals;                       // IVF_PQ: f32[n_sorted]
+    DevBuf tvals;                       // IVF_PQ: f32[n_sorted] (IVF_PQ_FS has none)
     DevBuf xnorm;                       // FLAT + L2: f32[n]
     DevBuf p_list, p_payload, p_tvals;  // pending: int32 list per row, payload rows, tvals
     int64_t p_cap = 0;
@@ -146,6 +146,7 @@ struct dfx_index {
             case DFX_FLAT:
             case DFX_IVF_FLAT: return (size_t)cfg.d * 4;
             case DFX_IVF_PQ: return ksub == 16 ? (size_t)M / 2 : (size_t)M;  // 4-bit codes: two per byte
+            case DFX_IVF_PQ_FS: return (size_t)M / 2;
             case DFX_IVF_SQ16: return (size_t)cfg.d * 2;
             case DFX_IVF_SQ8: return (size_t)cfg.d;
         }
@@ -162,6 +163,8 @@ struct dfx_index {
         for (size_t l = 0; l < nl; l++) h_len_top[l + 1] = h_len_top[l] + len[l];
     }
     bool is_ivf() const { return cfg.kind != DFX_FLAT; }
+    // the kinds with PQ codebooks (IVF_PQ: residual codes, IVF_PQ_FS: codes of the raw vectors)
+    bool has_pq() const { return cfg.kind == DFX_IVF_PQ || cfg.kind == DFX_IVF_PQ_FS; }
 };
 
 // ---- dfx_search.cu

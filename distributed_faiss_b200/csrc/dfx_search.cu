@@ -10,6 +10,8 @@
 //   K4   scan_pq          inverted-list scan of PQ codes, per-warp k-selection
 //   K4w  scan_pq_wide     64 < M <= 128: table built in shared memory + scan (dfx_scan_pq_wide_dev.cuh)
 //   K4n  scan_pq4         4-bit codes: table in registers, lookups by warp shuffle (dfx_scan_pq4_dev.cuh)
+//   K_fs pq_fs_lut / scan_pq_fs / fs_dequant   IVF-PQ FastScan: u8 quantized table, integer sums
+//                         (dfx_scan_pq_fs_dev.cuh)
 //   K2/5 scan_rows        inverted-list scan of fp32 rows / fp16 / 8-bit residual codes
 //   K_off cand_offsets    k > 1024: slots of each query's candidate row (the list scans then write
 //                         every vector's composite, MAT = true, and select_cand picks the k best)
@@ -200,6 +202,28 @@ void dfx_launch_select_comp(const uint64_t* comp, int64_t nrows, int n, int64_t 
 #include "dfx_pq_prep_dev.cuh"
 #include "dfx_scan_pq_wide_dev.cuh"
 #include "dfx_scan_pq4_dev.cuh"
+#include "dfx_scan_pq_fs_dev.cuh"
+
+// scan_pq_fs_kernel<M, MAT> for the runtime M (a multiple of 8 in [8, 128], checked by dfx_create)
+template <bool MAT, int MT = 8>
+static void dfx_launch_scan_pq_fs(int M, unsigned grid, size_t smem, cudaStream_t st, const uint8_t* lutq,
+                                  const int32_t* keys, int nprobe, int G, int ngroups, const int64_t* list_off,
+                                  const uint8_t* codes, const int32_t* ids, int k, int cap, uint64_t* part,
+                                  const int64_t* coff) {
+    if constexpr (MT <= 128) {
+        if (M != MT) {
+            dfx_launch_scan_pq_fs<MAT, MT + 8>(M, grid, smem, st, lutq, keys, nprobe, G, ngroups, list_off, codes,
+                                               ids, k, cap, part, coff);
+            return;
+        }
+        auto kern = scan_pq_fs_kernel<MT, MAT>;
+        DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        DFX_LAUNCH(kern, grid, 128, smem, st, lutq, keys, nprobe, G, ngroups, list_off, codes, ids, k, cap, part,
+                   coff);
+    } else {
+        throw DfxError{"IVF-PQ FastScan: no list scan for M=" + std::to_string(M)};
+    }
+}
 
 // scan_pq4_kernel<M, MAT> for the runtime M (a multiple of 8 in [8, 128], checked by dfx_create)
 template <bool MAT, int MT = 8>
@@ -913,7 +937,19 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
         }
 
         bool final_written = false;
-        if (kind == DFX_IVF_PQ && idx->ksub == 16) {
+        if (kind == DFX_IVF_PQ_FS) {
+            // FastScan: each query's table quantized to u8 (w_lut) with its (1 / a, b) (w_dis0), then
+            // the integer scan; fs_dequant_kernel maps the selected distances below
+            const int M = idx->M;
+            idx->w_lut.reserve((size_t)qc * M * 16);
+            idx->w_dis0.reserve((size_t)qc * 8);
+            DFX_LAUNCH(pq_fs_lut_kernel, (unsigned)qc, 256, dfx_pq_fs_lut_smem(d, M), st, xq, d, M, idx->dsub,
+                       idx->codebooks.as<float>(), idx->w_lut.as<uint8_t>(), idx->w_dis0.as<float2>());
+            auto launch = mat ? dfx_launch_scan_pq_fs<true> : dfx_launch_scan_pq_fs<false>;
+            launch(M, (unsigned)(qc * ngroups), mat ? 0 : dfx_pq_fs_smem(cap), st, idx->w_lut.as<uint8_t>(), keys,
+                   nprobe, G, ngroups, idx->list_off.as<int64_t>(), idx->payload.as<uint8_t>(),
+                   idx->ids.as<int32_t>(), k, cap, part, coff);
+        } else if (kind == DFX_IVF_PQ && idx->ksub == 16) {
             // 4-bit codes: the [M][16] table of each query goes to registers (dfx_scan_pq4_dev.cuh)
             const int M = idx->M;
             idx->w_lut.reserve((size_t)qc * M * PQ4_KSUB * 4);
@@ -1021,6 +1057,9 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
             ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, smetric, nullptr};
             dfx_launch_select<128>(ldr, wr, qc, ngroups * k, k, st);
         }
+        if (kind == DFX_IVF_PQ_FS)
+            DFX_LAUNCH(fs_dequant_kernel, (unsigned)dfx_ceil_div(qc * k, 256), 256, 0, st, d_D + q0 * k, d_I + q0 * k,
+                       qc * k, k, idx->w_dis0.as<float2>());
     }
     idx->last_nq = nq;
     idx->last_nprobe = nprobe;

@@ -23,10 +23,10 @@ import numpy as np
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdfx.so")
 
-KIND_FLAT, KIND_IVF_FLAT, KIND_IVF_PQ, KIND_IVF_SQ16, KIND_IVF_SQ8 = 0, 1, 2, 3, 4
+KIND_FLAT, KIND_IVF_FLAT, KIND_IVF_PQ, KIND_IVF_SQ16, KIND_IVF_SQ8, KIND_IVF_PQ_FS = 0, 1, 2, 3, 4, 5
 METRIC_INNER_PRODUCT, METRIC_L2 = 0, 1  # faiss enum values (reference index_cfg.py:44-52)
 KIND_NAMES = {KIND_FLAT: "flat", KIND_IVF_FLAT: "ivf_flat", KIND_IVF_PQ: "ivf_pq", KIND_IVF_SQ16: "ivf_sq",
-              KIND_IVF_SQ8: "ivf_sq8"}
+              KIND_IVF_SQ8: "ivf_sq8", KIND_IVF_PQ_FS: "ivf_pq_fs"}
 
 # every symbol include/dfx.h declares (tests check that the library exports each one)
 EXPORTED_SYMBOLS = [
@@ -126,7 +126,7 @@ class GpuIndex:
             self.quantizer = _Quantizer(self)
         self.pq_m = int(pq_m)
         self.pq_nbits = int(pq_nbits)
-        self.ksub = 1 << self.pq_nbits if self.kind == KIND_IVF_PQ else 0
+        self.ksub = 1 << self.pq_nbits if self.kind in (KIND_IVF_PQ, KIND_IVF_PQ_FS) else 0
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -287,7 +287,7 @@ class GpuIndex:
 
     def payload_name(self):
         return {KIND_FLAT: "xb", KIND_IVF_FLAT: "vecs", KIND_IVF_PQ: "codes", KIND_IVF_SQ16: "codes16",
-                KIND_IVF_SQ8: "codes8"}[self.kind]
+                KIND_IVF_SQ8: "codes8", KIND_IVF_PQ_FS: "codes"}[self.kind]
 
     def get_state(self):
         """Same dict layout as oracle.get_state() (list-sorted storage order)."""
@@ -307,6 +307,10 @@ class GpuIndex:
             st["codebooks"] = self.get_array("codebooks").reshape(self.pq_m, self.ksub, d // self.pq_m)
             st["codes"] = self.get_array("codes").reshape(-1, self.pq_m)
             st["tvals"] = self.get_array("tvals")
+        if self.kind == KIND_IVF_PQ_FS:  # codes of the raw vectors: no t-values
+            st["M"], st["ksub"] = self.pq_m, self.ksub
+            st["codebooks"] = self.get_array("codebooks").reshape(self.pq_m, self.ksub, d // self.pq_m)
+            st["codes"] = self.get_array("codes").reshape(-1, self.pq_m)
         if self.kind == KIND_IVF_SQ16:
             st["codes16"] = self.get_array("codes16").reshape(-1, d)
         if self.kind == KIND_IVF_SQ8:
@@ -319,7 +323,7 @@ class GpuIndex:
             self.set_array("xb", st["xb"])
         else:
             self.set_array("centroids", st["centroids"])
-            if self.kind == KIND_IVF_PQ:
+            if self.kind in (KIND_IVF_PQ, KIND_IVF_PQ_FS):
                 self.set_array("codebooks", st["codebooks"])
             if self.kind == KIND_IVF_SQ8:
                 self.set_array("sq_trained", st["sq_trained"])

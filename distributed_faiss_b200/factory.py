@@ -14,24 +14,29 @@ Tokens are case-sensitive, as in faiss:
                                               at most 128, that divides d)
   "IVF{n},SQfp16"                 -> ivf_sq    (IndexIVFScalarQuantizer QT_fp16, L2 only)
   "IVF{n},SQ8"                    -> ivf_sq8   (IndexIVFScalarQuantizer QT_8bit, L2 only)
+  "IVF{n},PQ{M}x4fs"              -> ivf_pq_fs (IndexIVFPQFastScan, 4-bit codes of the raw vectors
+                                              (not by_residual), searched through 8-bit quantized
+                                              distance tables; L2 only; M a multiple of 8 in
+                                              [8, 128] that divides d)
 Everything else (OPQ / PCA prefixes, HNSW, IVF{n}_HNSW quantizers, RFlat / Refine, IDMap, PQ{M}x4,
-SQ4 / SQ6, malformed n or M) raises RuntimeError.
+PQ{M}x4fsr, a FastScan block size suffix "_{bbs}", SQ4 / SQ6, malformed n or M) raises RuntimeError.
 """
 import re
 from typing import NamedTuple
 
 METRIC_INNER_PRODUCT, METRIC_L2 = 0, 1  # faiss enum values
 
-ACCEPTED_FORMS = ("Flat", "IVF{n},Flat", "IVF{n},PQ{M}", "IVF{n},PQ{M}x8", "IVF{n},SQfp16", "IVF{n},SQ8")
+ACCEPTED_FORMS = ("Flat", "IVF{n},Flat", "IVF{n},PQ{M}", "IVF{n},PQ{M}x8", "IVF{n},PQ{M}x4fs", "IVF{n},SQfp16",
+                  "IVF{n},SQ8")
 
-_IVF = re.compile(r"IVF([1-9][0-9]*),(Flat|PQ([1-9][0-9]*)(x8)?|SQfp16|SQ8)")
+_IVF = re.compile(r"IVF([1-9][0-9]*),(Flat|PQ([1-9][0-9]*)(x8|x4fs)?|SQfp16|SQ8)")
 # one query's fp32 PQ distance table (M x 256 x 4 bytes) must fit in one thread block's shared memory
 # (128 KB at M = 128); more would need split or fp16 tables, which are not bit-exact
 _PQ_M_MAX = 128
 
 
 class FactorySpec(NamedTuple):
-    """kind: a name of engine.KIND_NAMES ("flat", "ivf_flat", "ivf_pq", "ivf_sq", "ivf_sq8").
+    """kind: a name of engine.KIND_NAMES ("flat", "ivf_flat", "ivf_pq", "ivf_sq", "ivf_sq8", "ivf_pq_fs").
     metric: flat / ivf_flat: the search metric; the codecs: the coarse quantizer's metric (their
     search is L2)."""
     kind: str
@@ -67,6 +72,13 @@ def parse_factory(dim: int, factory_string: str, metric: int) -> FactorySpec:
             f"faiss_factory {factory_string!r} with the inner-product metric is not supported: a PQ or SQ "
             "codec searched by inner product needs inner-product distance tables, which no list scan here "
             "has (use metric='l2', or IVF{n},Flat for inner product)")
+    if codec.startswith("PQ") and m.group(4) == "x4fs":
+        M = int(m.group(3))
+        if M % 8 != 0 or M > _PQ_M_MAX or dim % M != 0:
+            raise RuntimeError(
+                f"faiss_factory {factory_string!r}: the number of FastScan sub-quantizers must be a multiple of 8 "
+                f"in [8, {_PQ_M_MAX}] that divides d={dim} (a row of 4-bit codes is whole 32-bit words)")
+        return FactorySpec("ivf_pq_fs", int(metric), nlist, M)
     if codec.startswith("PQ"):
         M = int(m.group(3))
         if M % 4 != 0 or M > _PQ_M_MAX or dim % M != 0:

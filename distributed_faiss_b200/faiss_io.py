@@ -14,6 +14,8 @@ STATUS: written from the layout of faiss 1.7.x `impl/index_write.cpp` / `index_r
 itself is not available in this environment (SURVEY.md section 8c), so the format is checked for
 self-consistency only (tests/test_faiss_io.py), never against a file written by faiss.  The same
 holds for the 4-bit IndexIVFPQ codes [faiss-upstream], restated from faiss's PQEncoderGeneric.
+IndexIVFPQFastScan ("IwPf", the factory string "IVF{n},PQ{M}x4fs") is neither read nor written: its
+block-interleaved code layout could not be checked without faiss; such shards use the npz format.
 
 Layout (little endian, no padding; `vec<T>` = u64 count + raw elements):
   header   : i32 d, i64 ntotal, i64 1<<20, i64 1<<20, u8 is_trained, i32 metric (0 IP, 1 L2)
@@ -243,6 +245,11 @@ def write_index(state: Dict, path: str, nprobe: int = 1) -> None:
             _w(f, "QQQ", int(state["d"]), M, nbits)
             _wvec(f, state["codebooks"], np.float32)
             _write_invlists(f, state["list_off"], state["ids"], codes, codes.shape[1])
+        elif kind == "ivf_pq_fs":
+            # faiss stores FastScan codes (IwPf) in blocks of bbs vectors with the nibbles permuted for
+            # its SIMD lookups; that layout has never been checked against faiss, so it is not written
+            raise FaissFormatError("IndexIVFPQFastScan (IVF{n},PQ{M}x4fs) shards cannot be written in the faiss "
+                                   "format; save them with the default npz format (index_format='dfx')")
         elif kind == "ivf_sq":
             d = int(state["d"])
             f.write(b"IwSq")

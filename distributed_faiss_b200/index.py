@@ -21,8 +21,10 @@ Builders (reference index.py:93-100):
   no builder, `faiss_factory` set -> the factory string with {centroids} substituted, the cfg metric
                   for the index and its quantizer, nprobe = the faiss default 1 (index.py:385-396)
 Factory strings are parsed by factory.parse_factory ("Flat", "IVF{n},Flat", "IVF{n},PQ{M}[x8]",
+"IVF{n},PQ{M}x4fs" (FastScan: 4-bit codes of the raw vectors, 8-bit quantized distance tables),
 "IVF{n},SQfp16", "IVF{n},SQ8"); any other string raises, and so does "hnswsq" (a graph index,
-outside the hot path this package rebuilds, SURVEY.md section 8).
+outside the hot path this package rebuilds, SURVEY.md section 8).  A stored shard is only loaded
+under a cfg that builds the same kind (and, for the PQ kinds, the same (M, ksub)).
 """
 import _thread
 import logging
@@ -76,7 +78,9 @@ def default_engine_factory(cfg: IndexCfg, device: Optional[int] = None):
     spec = factory_spec(cfg)
     if spec is not None:
         kind = {name: k for k, name in engine.KIND_NAMES.items()}[spec.kind]
-        idx = engine.GpuIndex(kind, cfg.dim, spec.metric, nlist=spec.nlist, pq_m=spec.pq_m, device=device)
+        nbits = 4 if spec.kind == "ivf_pq_fs" else 8  # FastScan: 4-bit codes
+        idx = engine.GpuIndex(kind, cfg.dim, spec.metric, nlist=spec.nlist, pq_m=spec.pq_m, pq_nbits=nbits,
+                              device=device)
         if cfg.index_builder_type == "ivf_gpu":
             idx.nprobe = cfg.nprobe  # index.py:84
         # the factory path keeps faiss's default nprobe (1) and leaves cfg.nprobe alone, unlike
@@ -561,7 +565,7 @@ class Index:
             # e.g. an SQfp16 file under a cfg that builds IVF-SQ8: never reinterpret the codes
             raise RuntimeError(f"the stored index is of kind {state.get('kind')!r} but the cfg builds "
                                f"{want!r}; refusing to load it")
-        if want == "ivf_pq":
+        if want in ("ivf_pq", "ivf_pq_fs"):
             # e.g. 4-bit codes under a cfg that builds 8-bit ones: the codebooks would not fit either
             stored = (int(state["M"]), int(state["ksub"]))
             built = (int(getattr(engine, "pq_m", getattr(engine, "M", 0))), int(engine.ksub))

@@ -41,8 +41,12 @@ enum {
     DFX_IVF_FLAT = 1, /* faiss.IndexIVFFlat                       index.py:36-40     */
     DFX_IVF_PQ = 2,   /* faiss.IndexIVFPQ (L2, by_residual)       index.py:43-48     */
     DFX_IVF_SQ16 = 3, /* faiss.IndexIVFScalarQuantizer(QT_fp16)   index.py:63-68     */
-    DFX_IVF_SQ8 = 4   /* faiss.IndexIVFScalarQuantizer(QT_8bit), by_residual: the factory string
+    DFX_IVF_SQ8 = 4,  /* faiss.IndexIVFScalarQuantizer(QT_8bit), by_residual: the factory string
                          "IVF{n},SQ8" (index.py:380-396) -- one byte per dimension */
+    DFX_IVF_PQ_FS = 5 /* faiss.IndexIVFPQFastScan(nbits = 4), NOT by_residual: the factory string
+                         "IVF{n},PQ{M}x4fs" (index.py:380-396).  4-bit codes packed two per byte; the
+                         search quantizes each query's distance table to 8 bits and sums it in
+                         integers (DESIGN.md section 2).  L2 only, for the index and its quantizer */
 };
 
 /* faiss.METRIC_INNER_PRODUCT / faiss.METRIC_L2 (index_cfg.py:44-52) */
@@ -52,15 +56,16 @@ typedef struct dfx_cfg {
     int32_t kind;     /* DFX_FLAT ... */
     int32_t metric;   /* FLAT / IVF_FLAT: search metric.  IVF_PQ / IVF_SQ16 / IVF_SQ8: metric of
                          the coarse quantizer only -- the reference never forwards it to the
-                         index, which is therefore always L2 (index.py:44-46, 64-66). */
+                         index, which is therefore always L2 (index.py:44-46, 64-66).
+                         IVF_PQ_FS: must be L2 (an inner-product metric is refused). */
     int32_t d;        /* vector dimension (cfg.dim) */
     int32_t pq_m;     /* IVF_PQ: sub-quantizers  (cfg.extra["code_size"], index.py:44).  8-bit codes:
                          4 <= M <= 128, M % 4 == 0, d % M == 0 (128: one query's fp32 table,
-                         M x 256 x 4 B, must fit in one thread block's shared memory).  4-bit codes:
-                         8 <= M <= 128, M % 8 == 0, d % M == 0 */
+                         M x 256 x 4 B, must fit in one thread block's shared memory).  4-bit codes
+                         and IVF_PQ_FS: 8 <= M <= 128, M % 8 == 0, d % M == 0 */
     int32_t pq_nbits; /* IVF_PQ: bits per code   (cfg.extra["bits_per_vector"], index.py:45): 8, or 4
                          (ksub = 16; codes stored two per byte, low nibble first, as faiss packs
-                         them) */
+                         them).  IVF_PQ_FS: must be 4 */
     int32_t device;   /* CUDA device ordinal this shard lives on */
     int64_t nlist;    /* IVF_*: number of inverted lists (cfg.centroids); IVF kinds need d % 4 == 0 */
 } dfx_cfg;
@@ -182,11 +187,13 @@ int dfx_map_ids_dev(int64_t n, const int64_t *d_ids, const int64_t *d_table, int
  *   (IVF_PQ: "codes" holds one code per byte whatever pq_nbits is, and "codebooks" has ksub =
  *   1 << pq_nbits; 4-bit codes are packed and unpacked on the way, and an imported code >= 16 is
  *   refused)
+ *   (IVF_PQ_FS: "centroids", "codebooks" f32[M,16,dsub], "list_off", "ids" and "codes" u8[ntotal,M],
+ *   one 4-bit code per byte as for IVF_PQ; no "tvals", since the codes are not residuals)
  *   "vecs" f32[ntotal,d] (IVF_FLAT)   "codes16" u16[ntotal,d]   "xb" f32[ntotal,d] (FLAT)
  *   "sq_trained" f32[2,d] (IVF_SQ8: vmin, then vdiff -- faiss's ScalarQuantizer::trained)
  *   "codes8" u8[ntotal,d] (IVF_SQ8)
  * dfx_get_array with out == NULL only reports the size.  Import order: centroids,
- * codebooks (IVF_PQ) or sq_trained (IVF_SQ8), then list_off, ids and the payload, then
+ * codebooks (IVF_PQ, IVF_PQ_FS) or sq_trained (IVF_SQ8), then list_off, ids and the payload, then
  * dfx_import_done(). */
 int dfx_get_array(dfx_index *idx, const char *name, void *out, int64_t max_bytes,
                   int64_t *nbytes);
