@@ -102,7 +102,8 @@ int dfx_debug_tc_screen(dfx_index* idx, int64_t nq, const float* d_x, int npl, f
 int dfx_create(const dfx_cfg* cfg, dfx_index** out) {
     DFX_API_BEGIN
     DFX_REQUIRE(cfg && out, "null argument");
-    DFX_REQUIRE(cfg->kind >= DFX_FLAT && cfg->kind <= DFX_IVF_PQ_FS, "unknown index kind");
+    DFX_REQUIRE(cfg->kind >= DFX_FLAT && cfg->kind <= DFX_IVF_PQR, "unknown index kind");
+    DFX_REQUIRE(cfg->kind == DFX_IVF_PQR || cfg->refine_m == 0, "refine_m must be 0 for every kind but IVF_PQR");
     DFX_REQUIRE(cfg->metric == DFX_METRIC_IP || cfg->metric == DFX_METRIC_L2,
                 "Only dot and l2 metrics are supported.");
     DFX_REQUIRE(cfg->d > 0 && cfg->d <= 4096, "dimension must be in [1, 4096]");
@@ -148,6 +149,23 @@ int dfx_create(const dfx_cfg* cfg, dfx_index** out) {
         idx->ksub = 16;
         idx->dsub = cfg->d / cfg->pq_m;
     }
+    if (cfg->kind == DFX_IVF_PQR) {
+        // faiss's factory refuses IVFPQR for inner product; the first stage is the 8-bit IVF-PQ scan
+        DFX_REQUIRE(cfg->metric == DFX_METRIC_L2,
+                    "IVF-PQR: only the L2 metric is supported (for the index and its coarse quantizer)");
+        DFX_REQUIRE(cfg->pq_nbits == 8, "IVF-PQR: 8 bits per sub-quantizer, got " + std::to_string(cfg->pq_nbits));
+        DFX_REQUIRE(cfg->pq_m >= 4 && cfg->pq_m <= 128 && cfg->pq_m % 4 == 0 && cfg->d % cfg->pq_m == 0,
+                    "IVF-PQR: the number of sub-quantizers must be a multiple of 4, at most 128, that divides d, "
+                    "got M=" + std::to_string(cfg->pq_m) + ", d=" + std::to_string(cfg->d));
+        DFX_REQUIRE(cfg->refine_m >= 4 && cfg->refine_m <= 128 && cfg->refine_m % 4 == 0 && cfg->d % cfg->refine_m == 0,
+                    "IVF-PQR: the number of refinement sub-quantizers must be a multiple of 4, at most 128, that "
+                    "divides d, got M2=" + std::to_string(cfg->refine_m) + ", d=" + std::to_string(cfg->d));
+        idx->M = cfg->pq_m;
+        idx->ksub = 256;
+        idx->dsub = cfg->d / cfg->pq_m;
+        idx->M2 = cfg->refine_m;
+        idx->dsub2 = cfg->d / cfg->refine_m;
+    }
     DeviceGuard g(cfg->device);
     DFX_CUDA(cudaStreamCreateWithFlags(&idx->stream, cudaStreamNonBlocking));
     *out = idx.release();
@@ -163,6 +181,10 @@ void dfx_destroy(dfx_index* idx) {
             cudaStreamDestroy(idx->stream);
         }
         for (auto& e : idx->prof_events) {
+            cudaEventDestroy(e.first);
+            cudaEventDestroy(e.second);
+        }
+        for (auto& e : idx->prof_refine_events) {
             cudaEventDestroy(e.first);
             cudaEventDestroy(e.second);
         }
@@ -214,8 +236,25 @@ int dfx_set_param(dfx_index* idx, const char* name, double value) {
         DFX_REQUIRE(value >= -1 && value <= 32, "il2_prefetch must be -1 (default) or 0..32 blocks");
         idx->il2_prefetch = (int)value;
     }
+    else if (n == "k_factor") {
+        DFX_REQUIRE(idx->cfg.kind == DFX_IVF_PQR, "k_factor is a parameter of IVF-PQR indexes");
+        DFX_REQUIRE(value >= 1 && value <= 16384, "k_factor must be in [1, 16384]");
+        idx->k_factor = (float)value;
+    }
     else throw DfxError{"unknown parameter " + n};
     DFX_API_END
+}
+
+// summed device time of one list of bracketing events (synchronises)
+static double prof_sum_ms(std::vector<std::pair<cudaEvent_t, cudaEvent_t>>& ev, size_t used) {
+    double ms = 0;
+    for (size_t i = 0; i < used; i++) {
+        DFX_CUDA(cudaEventSynchronize(ev[i].second));
+        float t = 0;
+        DFX_CUDA(cudaEventElapsedTime(&t, ev[i].first, ev[i].second));
+        ms += t;
+    }
+    return ms;
 }
 
 int dfx_get_param(dfx_index* idx, const char* name, double* value) {
@@ -244,6 +283,14 @@ int dfx_get_param(dfx_index* idx, const char* name, double* value) {
     else if (n == "il2_prefetch") *value = idx->il2_prefetch;
     else if (n == "rows_inflight") *value = idx->rows_inflight;
     else if (n == "workspace_bytes") *value = (double)idx->w_part.cap;  // read-only
+    else if (n == "k_factor" && idx->cfg.kind == DFX_IVF_PQR) *value = idx->k_factor;
+    else if (n == "refine_ms" || n == "refine_launches") {  // read-only
+        std::lock_guard<std::mutex> lk(idx->mu);
+        DeviceGuard g(idx->cfg.device);
+        idx->join_dev();
+        *value = n == "refine_launches" ? (double)idx->prof_refine_used
+                                        : prof_sum_ms(idx->prof_refine_events, idx->prof_refine_used);
+    }
     else throw DfxError{"unknown parameter " + n};
     DFX_API_END
 }
@@ -472,16 +519,10 @@ int dfx_profile_read(dfx_index* idx, double* scan_ms, int64_t* scan_launches, in
     std::lock_guard<std::mutex> lk(idx->mu);
     DeviceGuard g(idx->cfg.device);
     idx->join_dev();
-    double ms = 0;
-    for (size_t i = 0; i < idx->prof_used; i++) {
-        DFX_CUDA(cudaEventSynchronize(idx->prof_events[i].second));
-        float t = 0;
-        DFX_CUDA(cudaEventElapsedTime(&t, idx->prof_events[i].first, idx->prof_events[i].second));
-        ms += t;
-    }
+    const double ms = prof_sum_ms(idx->prof_events, idx->prof_used);
     if (scan_ms) *scan_ms = ms;
     if (scan_launches) *scan_launches = (int64_t)idx->prof_used;
-    if (reset) idx->prof_used = 0;
+    if (reset) idx->prof_used = idx->prof_refine_used = 0;
     DFX_API_END
 }
 
@@ -494,6 +535,7 @@ static const char* payload_name(int kind) {
         case DFX_IVF_SQ16: return "codes16";
         case DFX_IVF_SQ8: return "codes8";
         case DFX_IVF_PQ_FS: return "codes";
+        case DFX_IVF_PQR: return "codes";
     }
     return "";
 }
@@ -532,7 +574,9 @@ int dfx_get_array(dfx_index* idx, const char* name, void* out, int64_t max_bytes
     else if (n == "sq_trained" && idx->cfg.kind == DFX_IVF_SQ8 && idx->trained) { src = idx->sq_trained.p; bytes = 2 * d * 4; }
     else if (n == "list_off" && idx->is_ivf() && idx->trained) { src = idx->list_off.p; bytes = (nlist + 1) * 8; }
     else if (n == "ids" && idx->is_ivf()) { widen_ids = true; bytes = nt * 8; }
-    else if (n == "tvals" && idx->cfg.kind == DFX_IVF_PQ) { src = idx->tvals.p; bytes = nt * 4; }
+    else if (n == "tvals" && idx->pq_res()) { src = idx->tvals.p; bytes = nt * 4; }
+    else if (n == "refine_codebooks" && idx->cfg.kind == DFX_IVF_PQR && idx->trained) { src = idx->refine_cb.p; bytes = (int64_t)idx->M2 * 256 * idx->dsub2 * 4; }
+    else if (n == "refine_codes" && idx->cfg.kind == DFX_IVF_PQR) { src = idx->refine_codes.p; bytes = nt * idx->M2; }
     else if (unpack4) { bytes = nt * idx->M; }
     else if (n == payload_name(idx->cfg.kind)) { src = idx->payload.p; bytes = nt * (int64_t)idx->row_bytes(); }
     else throw DfxError{"no array named '" + n + "' in this index"};
@@ -585,6 +629,14 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
     } else if (n == "sq_trained" && idx->cfg.kind == DFX_IVF_SQ8) {
         DFX_REQUIRE(nbytes == 2 * d * 4, "sq_trained: wrong size (2 * d floats: vmin, then vdiff)");
         upload(idx->sq_trained, nbytes);
+    } else if (n == "refine_codebooks" && idx->cfg.kind == DFX_IVF_PQR) {
+        DFX_REQUIRE(nbytes == (int64_t)idx->M2 * 256 * idx->dsub2 * 4, "refine_codebooks: wrong size");
+        upload(idx->refine_cb, nbytes);
+    } else if (n == "refine_codes" && idx->cfg.kind == DFX_IVF_PQR) {
+        DFX_REQUIRE(nbytes == idx->n_sorted * (int64_t)idx->M2,
+                    "refine_codes: wrong size (u8[ntotal, M2] in id order; set list_off first)");
+        upload(idx->refine_codes, nbytes);
+        idx->refine_cap = idx->refine_rows = idx->n_sorted;
     } else if (n == "list_off" && idx->is_ivf()) {
         DFX_REQUIRE(nbytes == (nlist + 1) * 8, "list_off: wrong size");
         upload(idx->list_off, nbytes);
@@ -600,6 +652,15 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
         for (int64_t i = 0; i < idx->n_sorted; i++) {
             DFX_REQUIRE(s[i] >= 0 && s[i] < (1ll << 31), "ids must be in [0, 2^31)");
             tmp[(size_t)i] = (int32_t)s[i];
+        }
+        if (idx->cfg.kind == DFX_IVF_PQR) {
+            // the refine codes are addressed by id (faiss asserts the same of IndexIVFPQR)
+            std::vector<char> seen((size_t)idx->n_sorted, 0);
+            for (int64_t i = 0; i < idx->n_sorted; i++) {
+                DFX_REQUIRE(s[i] < idx->n_sorted && !seen[(size_t)s[i]],
+                            "ids: an IVF-PQR index needs ids that are a permutation of 0 .. ntotal-1");
+                seen[(size_t)s[i]] = 1;
+            }
         }
         idx->ids.reserve((size_t)std::max<int64_t>(idx->n_sorted, 1) * 4);
         if (idx->n_sorted)
@@ -646,11 +707,16 @@ int dfx_import_done(dfx_index* idx) {
     idx->join_dev();
     if (idx->is_ivf()) {
         DFX_REQUIRE(idx->centroids.p && idx->list_off.p, "import: centroids and list_off are required");
-        if (idx->cfg.kind == DFX_IVF_PQ) {
+        if (idx->cfg.kind == DFX_IVF_PQR) {
+            DFX_REQUIRE(idx->refine_cb.p, "import: refine_codebooks are required");
+            DFX_REQUIRE(idx->refine_rows == idx->n_sorted, "import: refine_codes of every vector are required");
+        }
+        if (idx->pq_res()) {
             DFX_REQUIRE(idx->codebooks.p, "import: codebooks are required");
             dfx_compute_tvals_sorted(idx, idx->stream);  // K7 recomputes the per-vector term
             dfx_pq_rm_to_il(idx, idx->stream);
         }
+        if (idx->cfg.kind == DFX_IVF_PQR) dfx_refresh_inv(idx, idx->stream);
         if (idx->cfg.kind == DFX_IVF_PQ_FS) DFX_REQUIRE(idx->codebooks.p, "import: codebooks are required");
         if (idx->cfg.kind == DFX_IVF_SQ8) DFX_REQUIRE(idx->sq_trained.p, "import: sq_trained is required");
         dfx_tc_prepare_centroids(idx, idx->stream);

@@ -128,6 +128,21 @@ pq_encode_kernel(const float* __restrict__ x, const float* __restrict__ cent,
     codes[i * M + m] = (uint8_t)bj;
 }
 
+// IVF-PQR: the residual left after PQ1, r2 = (x - c) - P1[m][code_m], one fp32 rounding per
+// subtraction.  cent == nullptr: x already holds the residuals x - c (training).
+__global__ void pq_residual2_kernel(const float* __restrict__ x, const float* __restrict__ cent,
+                                    const int32_t* __restrict__ assign, const uint8_t* __restrict__ codes, int64_t n,
+                                    int d, int M, int dsub, const float* __restrict__ codebooks,
+                                    float* __restrict__ out) {
+    int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t >= n * d) return;
+    int64_t i = t / d;
+    int c = (int)(t - i * d);
+    const int m = c / dsub;
+    const float r1 = cent ? x[t] - cent[(size_t)assign[i] * d + c] : x[t];
+    out[t] = r1 - codebooks[((size_t)m * 256 + codes[i * M + m]) * dsub + (c - m * dsub)];
+}
+
 // 4-bit codes: u8[n][M] (one code per byte, from pq_encode_kernel) -> the packed rows u8[n][M / 2].
 // One thread per output byte, so no two threads write the same byte.
 __global__ void pq_pack4_kernel(const uint8_t* __restrict__ in, int64_t nbytes, uint8_t* __restrict__ out) {
@@ -269,6 +284,25 @@ __global__ void widen_kernel(const int32_t* __restrict__ in, int64_t n, int64_t*
 
 static inline unsigned blocks_for(int64_t n, int t) { return (unsigned)dfx_ceil_div(n, t); }
 
+// codes u8[n][M] of the rows x themselves (pq_encode_kernel<DS, false>: no centroid subtracted)
+static void launch_pq_encode_raw(const float* x, int64_t n, int d, int M, int ksub, int dsub, const float* codebooks,
+                                 uint8_t* codes, cudaStream_t st) {
+    if (n <= 0) return;
+    dim3 grid(blocks_for(n, 256), (unsigned)M);
+#define DFX_PQ_ENCODE_RAW(DS)                                                                          \
+    do {                                                                                               \
+        auto kern = pq_encode_kernel<DS, false>;                                                       \
+        DFX_LAUNCH(kern, grid, 256, (size_t)ksub * dsub * 4, st, x, (const float*)nullptr,             \
+                   (const int32_t*)nullptr, n, d, M, ksub, dsub, codebooks, codes);                    \
+    } while (0)
+    if (dsub == 2) DFX_PQ_ENCODE_RAW(2);
+    else if (dsub == 4) DFX_PQ_ENCODE_RAW(4);
+    else if (dsub == 8) DFX_PQ_ENCODE_RAW(8);
+    else if (dsub == 16) DFX_PQ_ENCODE_RAW(16);
+    else DFX_PQ_ENCODE_RAW(0);
+#undef DFX_PQ_ENCODE_RAW
+}
+
 // ------------------------------------------------------------------ assign
 void dfx_assign_impl(dfx_index* idx, const float* d_cent, const float* d_cnorm, int64_t nlist,
                      int metric, int d, int64_t n, const float* d_x, int32_t* d_assign,
@@ -398,7 +432,7 @@ void dfx_train_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st
     dfx_launch_row_norms(idx->centroids.as<float>(), nlist, d, idx->cnorm.as<float>(), st);
     dfx_tc_prepare_centroids(idx, st);
 
-    if (kind == DFX_IVF_PQ) {
+    if (idx->pq_res()) {
         const int M = idx->M, ksub = idx->ksub, dsub = idx->dsub;
         int64_t ns = std::min<int64_t>(nt, 256ll * ksub);
         DFX_REQUIRE(ns >= ksub, "train: need at least " + std::to_string(ksub) + " vectors for PQ");
@@ -417,6 +451,27 @@ void dfx_train_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st
                        (const int32_t*)nullptr, ns, dsub, m * dsub, d, d_subv.as<float>());
             kmeans_device(idx, dsub, ns, d_subv.as<float>(), ksub, niter, seed + 1 + m,
                           idx->codebooks.as<float>() + (size_t)m * ksub * dsub, st);
+        }
+        if (kind == DFX_IVF_PQR) {
+            // faiss IndexIVFPQR::train_encoder: the refinement PQ is trained on what PQ1 leaves of the
+            // same residuals, r2 = r - decode(encode(r)); seeds seed + 1 + M + m2 (PQ1 has seed + 1 + m)
+            const int M2 = idx->M2, dsub2 = idx->dsub2;
+            DevBuf d_codes, d_r2;
+            d_codes.reserve((size_t)ns * M);
+            d_r2.reserve((size_t)ns * d * 4);
+            launch_pq_encode_raw(d_res.as<float>(), ns, d, M, ksub, dsub, idx->codebooks.as<float>(),
+                                 d_codes.as<uint8_t>(), st);
+            DFX_LAUNCH(pq_residual2_kernel, blocks_for(ns * d, 256), 256, 0, st, d_res.as<float>(), (const float*)nullptr,
+                       (const int32_t*)nullptr, d_codes.as<uint8_t>(), ns, d, M, dsub, idx->codebooks.as<float>(),
+                       d_r2.as<float>());
+            d_subv.reserve((size_t)ns * dsub2 * 4);
+            idx->refine_cb.reserve((size_t)M2 * 256 * dsub2 * 4);
+            for (int m2 = 0; m2 < M2; m2++) {
+                DFX_LAUNCH(gather_rows_kernel, blocks_for(ns * dsub2, 256), 256, 0, st, d_r2.as<float>(),
+                           (const int32_t*)nullptr, ns, dsub2, m2 * dsub2, d, d_subv.as<float>());
+                kmeans_device(idx, dsub2, ns, d_subv.as<float>(), 256, niter, seed + 1 + M + m2,
+                              idx->refine_cb.as<float>() + (size_t)m2 * 256 * dsub2, st);
+            }
         }
     }
     if (kind == DFX_IVF_PQ_FS) {
@@ -467,6 +522,10 @@ void dfx_train_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st
     idx->n_sorted = 0;
     idx->n_pending = 0;
     idx->trained = true;
+    if (kind == DFX_IVF_PQR) {
+        idx->inv_valid = false;
+        dfx_refresh_inv(idx, st);
+    }
 }
 
 // ------------------------------------------------------------------ add
@@ -478,7 +537,7 @@ static void ensure_pending(dfx_index* idx, int64_t need, cudaStream_t st) {
     const size_t rb = idx->row_bytes();
     idx->p_list.reserve((size_t)cap * 4, (size_t)idx->n_pending * 4, st);
     idx->p_payload.reserve((size_t)cap * rb, (size_t)idx->n_pending * rb, st);
-    if (idx->cfg.kind == DFX_IVF_PQ)
+    if (idx->pq_res())
         idx->p_tvals.reserve((size_t)cap * 4, (size_t)idx->n_pending * 4, st);
     idx->p_cap = cap;
 }
@@ -512,7 +571,7 @@ void dfx_add_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) 
     unsigned char* prow = idx->p_payload.as<unsigned char>() + (size_t)idx->n_pending * rb;
     if (kind == DFX_IVF_FLAT) {
         DFX_CUDA(cudaMemcpyAsync(prow, d_x, (size_t)n * rb, cudaMemcpyDeviceToDevice, st));
-    } else if (kind == DFX_IVF_PQ) {
+    } else if (idx->pq_res()) {
         const int M = idx->M, ksub = idx->ksub, dsub = idx->dsub;
         // one code per byte first; 4-bit codes are packed afterwards (two sub-quantizers share a
         // byte, so the per-sub-quantizer encode launch cannot write nibbles in place)
@@ -542,7 +601,24 @@ void dfx_add_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) 
         if (ksub == 16)
             DFX_LAUNCH(pq_pack4_kernel, blocks_for(n * M / 2, 256), 256, 0, st, (const uint8_t*)enc,
                        n * M / 2, (uint8_t*)prow);
-        // (`unpacked` is freed on return: cudaFree waits for the kernels above)
+        if (kind == DFX_IVF_PQR) {
+            // refine_codes[id] = refine_pq.encode((x - c) - PQ1(code)); the new rows get the ids
+            // ntotal .. ntotal + n - 1, their arrival order, so they append
+            const int64_t id0 = idx->ntotal();
+            if (id0 + n > idx->refine_cap) {
+                const int64_t cap = std::max<int64_t>({id0 + n, 2 * idx->refine_cap, idx->reserve_hint});
+                idx->refine_codes.reserve((size_t)cap * idx->M2, (size_t)id0 * idx->M2, st);
+                idx->refine_cap = cap;
+            }
+            DevBuf r2;
+            r2.reserve((size_t)n * d * 4);
+            DFX_LAUNCH(pq_residual2_kernel, blocks_for(n * d, 256), 256, 0, st, d_x, idx->centroids.as<float>(),
+                       (const int32_t*)plist, (const uint8_t*)enc, n, d, M, dsub, idx->codebooks.as<float>(),
+                       r2.as<float>());
+            launch_pq_encode_raw(r2.as<float>(), n, d, idx->M2, 256, idx->dsub2, idx->refine_cb.as<float>(),
+                                 idx->refine_codes.as<uint8_t>() + (size_t)id0 * idx->M2, st);
+        }
+        // (`unpacked` and `r2` are freed on return: cudaFree waits for the kernels above)
     } else if (kind == DFX_IVF_PQ_FS) {
         // the codes of the raw vector (no residual, no t-value), one per byte, then packed
         const int M = idx->M, ksub = idx->ksub, dsub = idx->dsub;
@@ -638,7 +714,7 @@ void dfx_finalize_impl(dfx_index* idx, cudaStream_t st) {
                new_payload.as<uint32_t>());
     DFX_LAUNCH(gather_ids_kernel, blocks_for(n, 256), 256, 0, st, idx->ids.as<int32_t>(), na,
                order.as<int32_t>(), n, new_ids.as<int32_t>());
-    if (idx->cfg.kind == DFX_IVF_PQ) {
+    if (idx->pq_res()) {
         new_tvals.reserve((size_t)n * 4);
         DFX_LAUNCH(gather_words_kernel, blocks_for(n, 256), 256, 0, st, idx->tvals.as<uint32_t>(),
                    idx->p_tvals.as<uint32_t>(), na, order.as<int32_t>(), n, 1, new_tvals.as<uint32_t>());
@@ -653,7 +729,7 @@ void dfx_finalize_impl(dfx_index* idx, cudaStream_t st) {
     idx->update_list_lengths();
     std::swap(idx->payload, new_payload);
     std::swap(idx->ids, new_ids);
-    if (idx->cfg.kind == DFX_IVF_PQ) std::swap(idx->tvals, new_tvals);
+    if (idx->pq_res()) std::swap(idx->tvals, new_tvals);
     idx->p_list.release();
     idx->p_payload.release();
     idx->p_tvals.release();
@@ -662,6 +738,7 @@ void dfx_finalize_impl(dfx_index* idx, cudaStream_t st) {
     idx->n_pending = 0;
     idx->inv_valid = false;
     dfx_pq_rm_to_il(idx, st);  // IVF-PQ, M == 32: interleaved blocks for the scan (no-op otherwise)
+    if (idx->cfg.kind == DFX_IVF_PQR) dfx_refresh_inv(idx, st);
 }
 
 // ------------------------------------------------------------------ reconstruct
@@ -772,19 +849,67 @@ __global__ void pq_fs_reconstruct_kernel(int d, int M, int dsub, int64_t ntotal,
     }
 }
 
+// IVF-PQR: (c + P1[m][code_m]) + P2[m2][refine_code_m2], the reconstruction of faiss's
+// IndexIVFPQR.  Ids as reconstruct_kernel; il != 0: `inv` holds padded block positions, `off` is
+// blk_off and the codes are the interleaved blocks, else `off` is list_off.
+__global__ void pqr_reconstruct_kernel(int d, int M, int dsub, int M2, int dsub2, int64_t ntotal, int64_t nlist,
+                                       const int64_t* __restrict__ want, const int32_t* __restrict__ inv,
+                                       const uint8_t* __restrict__ codes, int il, const int64_t* __restrict__ off,
+                                       const float* __restrict__ cent, const float* __restrict__ codebooks,
+                                       const uint8_t* __restrict__ rcodes, const float* __restrict__ rcb,
+                                       float* __restrict__ out, int64_t tag) {
+    const int64_t r = blockIdx.x;
+    int64_t id = want[r];
+    if (tag >= 0) {
+        if (id < 0 || ((id >> 40) & 0xfffff) != tag) return;
+        id &= (1ll << 40) - 1;
+    }
+    if (id < 0 || id >= ntotal) {
+        for (int k = threadIdx.x; k < d; k += blockDim.x) out[r * d + k] = __int_as_float(0x7fc00000);
+        return;
+    }
+    const int64_t pos = inv[id];
+    const int64_t key = il ? (pos >> 5) : pos;
+    int64_t lo = 0, hi = nlist;
+    while (hi - lo > 1) {
+        int64_t mid = (lo + hi) >> 1;
+        if (off[mid] <= key) lo = mid; else hi = mid;
+    }
+    for (int k = threadIdx.x; k < d; k += blockDim.x) {
+        const int m = k / dsub, m2 = k / dsub2;
+        const int code = il ? codes[(pos >> 5) * 1024 + dfx_il2_byte((int)(pos & 31), m)] : codes[pos * M + m];
+        const float p1 = codebooks[((size_t)m * 256 + code) * dsub + (k - m * dsub)];
+        const float p2 = rcb[((size_t)m2 * 256 + rcodes[id * M2 + m2]) * dsub2 + (k - m2 * dsub2)];
+        out[r * d + k] = (cent[(size_t)lo * d + k] + p1) + p2;
+    }
+}
+
+void dfx_refresh_inv(dfx_index* idx, cudaStream_t st) {
+    if (!idx->is_ivf() || idx->inv_valid) return;
+    const int64_t nt = idx->n_sorted;
+    const int il = idx->il ? 2 : 0;
+    idx->inv.reserve((size_t)std::max<int64_t>(nt, 1) * 4);
+    const int64_t npos = il ? idx->nblk * 32 : nt;
+    if (npos > 0)
+        DFX_LAUNCH(invert_ids_kernel, blocks_for(npos, 256), 256, 0, st,
+                   il ? idx->il_ids.as<int32_t>() : idx->ids.as<int32_t>(), npos, idx->inv.as<int32_t>());
+    idx->inv_valid = true;
+}
+
 void dfx_reconstruct_impl(dfx_index* idx, int64_t n, const int64_t* d_ids, float* d_out,
                           cudaStream_t st, int64_t tag) {
     if (n <= 0) return;
     if (idx->n_pending > 0) dfx_finalize_impl(idx, st);
     const int64_t nt = idx->n_sorted;
     const int il = idx->il ? 2 : 0;  // 0 = row-major, else the block layout
-    if (idx->is_ivf() && !idx->inv_valid) {
-        idx->inv.reserve((size_t)std::max<int64_t>(nt, 1) * 4);
-        const int64_t npos = il ? idx->nblk * 32 : nt;
-        if (npos > 0)
-            DFX_LAUNCH(invert_ids_kernel, blocks_for(npos, 256), 256, 0, st,
-                       il ? idx->il_ids.as<int32_t>() : idx->ids.as<int32_t>(), npos, idx->inv.as<int32_t>());
-        idx->inv_valid = true;
+    dfx_refresh_inv(idx, st);
+    if (idx->cfg.kind == DFX_IVF_PQR) {
+        DFX_LAUNCH(pqr_reconstruct_kernel, (unsigned)n, 128, 0, st, idx->cfg.d, idx->M, idx->dsub, idx->M2, idx->dsub2,
+                   nt, idx->cfg.nlist, d_ids, idx->inv.as<int32_t>(),
+                   il ? (const uint8_t*)idx->il_codes.p : (const uint8_t*)idx->payload.p, il,
+                   il ? idx->blk_off.as<int64_t>() : idx->list_off.as<int64_t>(), idx->centroids.as<float>(),
+                   idx->codebooks.as<float>(), idx->refine_codes.as<uint8_t>(), idx->refine_cb.as<float>(), d_out, tag);
+        return;
     }
     if (idx->cfg.kind == DFX_IVF_SQ8) {
         DFX_LAUNCH(sq8_reconstruct_kernel, (unsigned)n, 128, 0, st, idx->cfg.d, nt, idx->cfg.nlist, d_ids,

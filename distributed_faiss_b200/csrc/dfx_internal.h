@@ -89,10 +89,21 @@ struct dfx_index {
     bool flat_tc = true;        // FLAT: search through the tensor-core screening (dfx_tc_flat_candidates)
     int64_t tc_flat_rows = -1;  // rows covered by the fp16 copy of a FLAT index (-1: none)
 
+    // IVF_PQR: the refinement PQ (M2 sub-quantizers of 256 centroids, dsub2 = d / M2), its codes by
+    // id (u8[ntotal][M2], arrival order; refine_cap rows allocated), k' = k * k_factor, and the
+    // per-chunk workspace of the re-ranking (first-stage D' / I' and the refined composites)
+    int M2 = 0, dsub2 = 0;
+    float k_factor = 4.f;  // faiss IndexIVFPQR default
+    DevBuf refine_cb, refine_codes;
+    int64_t refine_cap = 0, refine_rows = 0;  // rows allocated / rows imported (dfx_set_array)
+    DevBuf w_rD, w_rI, w_rcomp;
+
     // scan-kernel profiling (dfx_profile_enable)
     bool prof_on = false;
     std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_events;
     size_t prof_used = 0;
+    std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_refine_events;  // IVF_PQR re-ranking stage
+    size_t prof_refine_used = 0;
 
     // last-search bookkeeping
     int64_t last_nq = 0, last_nprobe = 0;
@@ -147,6 +158,7 @@ struct dfx_index {
             case DFX_IVF_FLAT: return (size_t)cfg.d * 4;
             case DFX_IVF_PQ: return ksub == 16 ? (size_t)M / 2 : (size_t)M;  // 4-bit codes: two per byte
             case DFX_IVF_PQ_FS: return (size_t)M / 2;
+            case DFX_IVF_PQR: return (size_t)M;  // the refine codes live outside the lists
             case DFX_IVF_SQ16: return (size_t)cfg.d * 2;
             case DFX_IVF_SQ8: return (size_t)cfg.d;
         }
@@ -163,8 +175,10 @@ struct dfx_index {
         for (size_t l = 0; l < nl; l++) h_len_top[l + 1] = h_len_top[l] + len[l];
     }
     bool is_ivf() const { return cfg.kind != DFX_FLAT; }
-    // the kinds with PQ codebooks (IVF_PQ: residual codes, IVF_PQ_FS: codes of the raw vectors)
-    bool has_pq() const { return cfg.kind == DFX_IVF_PQ || cfg.kind == DFX_IVF_PQ_FS; }
+    // the kinds with PQ codebooks (IVF_PQ / IVF_PQR: residual codes, IVF_PQ_FS: codes of the raw vectors)
+    bool has_pq() const { return cfg.kind == DFX_IVF_PQ || cfg.kind == DFX_IVF_PQ_FS || cfg.kind == DFX_IVF_PQR; }
+    // the kinds whose lists hold IVF-PQ residual codes with t-values (IVF_PQR: its first stage)
+    bool pq_res() const { return cfg.kind == DFX_IVF_PQ || cfg.kind == DFX_IVF_PQR; }
 };
 
 // ---- dfx_search.cu
@@ -250,3 +264,7 @@ void dfx_assign_impl(dfx_index* idx, const float* d_cent, const float* d_cnorm, 
                      int metric, int d, int64_t n, const float* d_x, int32_t* d_assign,
                      cudaStream_t st);
 void dfx_compute_tvals_sorted(dfx_index* idx, cudaStream_t st);
+// `inv` (shard-local id -> storage position, padded block position when interleaved) for the
+// current layout; a no-op while it is valid.  IVF_PQR searches read it, so every change of the
+// layout rebuilds it right away (finalize, import, the interleaved conversions).
+void dfx_refresh_inv(dfx_index* idx, cudaStream_t st);

@@ -4,7 +4,7 @@
 
 bool dfx_il_wanted(const dfx_index* idx) {
     // the interleaved blocks hold one byte per code: 4-bit codes always stay row-major
-    return idx->cfg.kind == DFX_IVF_PQ && idx->M == 32 && idx->ksub == 256 && idx->il_enabled;
+    return idx->pq_res() && idx->M == 32 && idx->ksub == 256 && idx->il_enabled;
 }
 
 // payload/tvals/ids (row-major, list-sorted) -> il_* ; frees the row-major arrays
@@ -34,6 +34,7 @@ void dfx_pq_rm_to_il(dfx_index* idx, cudaStream_t st) {
     idx->nblk = nblk;
     idx->il = true;
     idx->inv_valid = false;
+    if (idx->cfg.kind == DFX_IVF_PQR) dfx_refresh_inv(idx, st);
 }
 
 // il_* -> payload/tvals/ids (row-major); frees the interleaved arrays
@@ -55,5 +56,6 @@ void dfx_pq_il_to_rm(dfx_index* idx, cudaStream_t st) {
     idx->nblk = 0;
     idx->il = false;
     idx->inv_valid = false;
+    if (idx->cfg.kind == DFX_IVF_PQR) dfx_refresh_inv(idx, st);
 }
 

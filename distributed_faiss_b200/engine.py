@@ -24,9 +24,10 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libdfx.so")
 
 KIND_FLAT, KIND_IVF_FLAT, KIND_IVF_PQ, KIND_IVF_SQ16, KIND_IVF_SQ8, KIND_IVF_PQ_FS = 0, 1, 2, 3, 4, 5
+KIND_IVF_PQR = 6
 METRIC_INNER_PRODUCT, METRIC_L2 = 0, 1  # faiss enum values (reference index_cfg.py:44-52)
 KIND_NAMES = {KIND_FLAT: "flat", KIND_IVF_FLAT: "ivf_flat", KIND_IVF_PQ: "ivf_pq", KIND_IVF_SQ16: "ivf_sq",
-              KIND_IVF_SQ8: "ivf_sq8", KIND_IVF_PQ_FS: "ivf_pq_fs"}
+              KIND_IVF_SQ8: "ivf_sq8", KIND_IVF_PQ_FS: "ivf_pq_fs", KIND_IVF_PQR: "ivf_pqr"}
 
 # every symbol include/dfx.h declares (tests check that the library exports each one)
 EXPORTED_SYMBOLS = [
@@ -42,7 +43,7 @@ EXPORTED_SYMBOLS = [
 
 class DfxCfg(C.Structure):
     _fields_ = [("kind", C.c_int32), ("metric", C.c_int32), ("d", C.c_int32), ("pq_m", C.c_int32),
-                ("pq_nbits", C.c_int32), ("device", C.c_int32), ("nlist", C.c_int64)]
+                ("pq_nbits", C.c_int32), ("device", C.c_int32), ("nlist", C.c_int64), ("refine_m", C.c_int32)]
 
 
 class DfxSynth(C.Structure):
@@ -112,21 +113,23 @@ class _Quantizer:
 class GpuIndex:
     """One shard resident in the HBM of one H100, behind the faiss-object surface."""
 
-    def __init__(self, kind, d, metric=METRIC_INNER_PRODUCT, nlist=0, pq_m=0, pq_nbits=8, device=None):
+    def __init__(self, kind, d, metric=METRIC_INNER_PRODUCT, nlist=0, pq_m=0, pq_nbits=8, device=None, refine_m=0):
         import torch  # device bookkeeping only
 
         if device is None:
             device = torch.cuda.current_device() if torch.cuda.is_available() else 0
         self.kind, self.d, self.metric = int(kind), int(d), int(metric)
         self.device = int(device)
-        self._cfg = DfxCfg(self.kind, self.metric, self.d, int(pq_m), int(pq_nbits), self.device, int(nlist))
+        self._cfg = DfxCfg(self.kind, self.metric, self.d, int(pq_m), int(pq_nbits), self.device, int(nlist),
+                           int(refine_m))
         self._h = C.c_void_p()
         _check(lib().dfx_create(C.byref(self._cfg), C.byref(self._h)))
         if self.kind != KIND_FLAT:
             self.quantizer = _Quantizer(self)
         self.pq_m = int(pq_m)
         self.pq_nbits = int(pq_nbits)
-        self.ksub = 1 << self.pq_nbits if self.kind in (KIND_IVF_PQ, KIND_IVF_PQ_FS) else 0
+        self.ksub = 1 << self.pq_nbits if self.kind in (KIND_IVF_PQ, KIND_IVF_PQ_FS, KIND_IVF_PQR) else 0
+        self.refine_m = int(refine_m)  # IVF-PQR: M2, the bytes of the refinement code
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -271,7 +274,8 @@ class GpuIndex:
     # ---- state exchange (tests / persistence)
     _DTYPES = {"centroids": np.float32, "codebooks": np.float32, "list_off": np.int64, "ids": np.int64,
                "codes": np.uint8, "tvals": np.float32, "vecs": np.float32, "codes16": np.uint16,
-               "xb": np.float32, "sq_trained": np.float32, "codes8": np.uint8}
+               "xb": np.float32, "sq_trained": np.float32, "codes8": np.uint8, "refine_codebooks": np.float32,
+               "refine_codes": np.uint8}
 
     def get_array(self, name):
         nb = C.c_int64(0)
@@ -287,7 +291,7 @@ class GpuIndex:
 
     def payload_name(self):
         return {KIND_FLAT: "xb", KIND_IVF_FLAT: "vecs", KIND_IVF_PQ: "codes", KIND_IVF_SQ16: "codes16",
-                KIND_IVF_SQ8: "codes8", KIND_IVF_PQ_FS: "codes"}[self.kind]
+                KIND_IVF_SQ8: "codes8", KIND_IVF_PQ_FS: "codes", KIND_IVF_PQR: "codes"}[self.kind]
 
     def get_state(self):
         """Same dict layout as oracle.get_state() (list-sorted storage order)."""
@@ -302,11 +306,17 @@ class GpuIndex:
             st["vecs"] = self.get_array("vecs").reshape(-1, d)
         else:
             st["coarse_metric"] = self.metric
-        if self.kind == KIND_IVF_PQ:
+        if self.kind in (KIND_IVF_PQ, KIND_IVF_PQR):
             st["M"], st["ksub"] = self.pq_m, self.ksub
             st["codebooks"] = self.get_array("codebooks").reshape(self.pq_m, self.ksub, d // self.pq_m)
             st["codes"] = self.get_array("codes").reshape(-1, self.pq_m)
             st["tvals"] = self.get_array("tvals")
+        if self.kind == KIND_IVF_PQR:  # the refinement PQ; its codes are in id order
+            M2 = self.refine_m
+            st["M2"] = M2
+            st["refine_codebooks"] = self.get_array("refine_codebooks").reshape(M2, 256, d // M2)
+            st["refine_codes"] = self.get_array("refine_codes").reshape(-1, M2)
+            st["k_factor"] = self.get_param("k_factor")
         if self.kind == KIND_IVF_PQ_FS:  # codes of the raw vectors: no t-values
             st["M"], st["ksub"] = self.pq_m, self.ksub
             st["codebooks"] = self.get_array("codebooks").reshape(self.pq_m, self.ksub, d // self.pq_m)
@@ -323,13 +333,19 @@ class GpuIndex:
             self.set_array("xb", st["xb"])
         else:
             self.set_array("centroids", st["centroids"])
-            if self.kind in (KIND_IVF_PQ, KIND_IVF_PQ_FS):
+            if self.kind in (KIND_IVF_PQ, KIND_IVF_PQ_FS, KIND_IVF_PQR):
                 self.set_array("codebooks", st["codebooks"])
             if self.kind == KIND_IVF_SQ8:
                 self.set_array("sq_trained", st["sq_trained"])
+            if self.kind == KIND_IVF_PQR:
+                self.set_array("refine_codebooks", st["refine_codebooks"])
             self.set_array("list_off", st["list_off"])
             self.set_array("ids", st["ids"])
             self.set_array(self.payload_name(), st[self.payload_name()])
+            if self.kind == KIND_IVF_PQR:
+                self.set_array("refine_codes", st["refine_codes"])
+                if "k_factor" in st:
+                    self.set_param("k_factor", float(st["k_factor"]))
         _check(lib().dfx_import_done(self._h))
 
 

@@ -18,6 +18,11 @@ Tokens are case-sensitive, as in faiss:
                                               (not by_residual), searched through 8-bit quantized
                                               distance tables; L2 only; M a multiple of 8 in
                                               [8, 128] that divides d)
+  "IVF{n},PQ{M}+{M2}"             -> ivf_pqr   (IndexIVFPQR: 8-bit IVF-PQ whose residual error is encoded
+                                              again by a second 8-bit PQ of M2 bytes; a search re-ranks
+                                              the k * k_factor best IVF-PQ candidates on the finer
+                                              reconstruction; L2 only; M and M2 each a multiple of 4, at
+                                              most 128, that divides d)
 Everything else (OPQ / PCA prefixes, HNSW, IVF{n}_HNSW quantizers, RFlat / Refine, IDMap, PQ{M}x4,
 PQ{M}x4fsr, a FastScan block size suffix "_{bbs}", SQ4 / SQ6, malformed n or M) raises RuntimeError.
 """
@@ -26,23 +31,24 @@ from typing import NamedTuple
 
 METRIC_INNER_PRODUCT, METRIC_L2 = 0, 1  # faiss enum values
 
-ACCEPTED_FORMS = ("Flat", "IVF{n},Flat", "IVF{n},PQ{M}", "IVF{n},PQ{M}x8", "IVF{n},PQ{M}x4fs", "IVF{n},SQfp16",
-                  "IVF{n},SQ8")
+ACCEPTED_FORMS = ("Flat", "IVF{n},Flat", "IVF{n},PQ{M}", "IVF{n},PQ{M}x8", "IVF{n},PQ{M}x4fs", "IVF{n},PQ{M}+{M2}",
+                  "IVF{n},SQfp16", "IVF{n},SQ8")
 
-_IVF = re.compile(r"IVF([1-9][0-9]*),(Flat|PQ([1-9][0-9]*)(x8|x4fs)?|SQfp16|SQ8)")
+_IVF = re.compile(r"IVF([1-9][0-9]*),(Flat|PQ([1-9][0-9]*)(x8|x4fs|\+([1-9][0-9]*))?|SQfp16|SQ8)")
 # one query's fp32 PQ distance table (M x 256 x 4 bytes) must fit in one thread block's shared memory
 # (128 KB at M = 128); more would need split or fp16 tables, which are not bit-exact
 _PQ_M_MAX = 128
 
 
 class FactorySpec(NamedTuple):
-    """kind: a name of engine.KIND_NAMES ("flat", "ivf_flat", "ivf_pq", "ivf_sq", "ivf_sq8", "ivf_pq_fs").
-    metric: flat / ivf_flat: the search metric; the codecs: the coarse quantizer's metric (their
-    search is L2)."""
+    """kind: a name of engine.KIND_NAMES ("flat", "ivf_flat", "ivf_pq", "ivf_sq", "ivf_sq8", "ivf_pq_fs",
+    "ivf_pqr").  metric: flat / ivf_flat: the search metric; the codecs: the coarse quantizer's metric
+    (their search is L2).  refine_m: ivf_pqr's M2 (bytes of the refinement code), else 0."""
     kind: str
     metric: int
     nlist: int = 0
     pq_m: int = 0
+    refine_m: int = 0
 
 
 def substitute_centroids(factory_string: str, centroids: int) -> str:
@@ -79,6 +85,14 @@ def parse_factory(dim: int, factory_string: str, metric: int) -> FactorySpec:
                 f"faiss_factory {factory_string!r}: the number of FastScan sub-quantizers must be a multiple of 8 "
                 f"in [8, {_PQ_M_MAX}] that divides d={dim} (a row of 4-bit codes is whole 32-bit words)")
         return FactorySpec("ivf_pq_fs", int(metric), nlist, M)
+    if codec.startswith("PQ") and m.group(5) is not None:
+        M, M2 = int(m.group(3)), int(m.group(5))
+        for name, v in (("PQ", M), ("refinement PQ", M2)):
+            if v % 4 != 0 or v > _PQ_M_MAX or dim % v != 0:
+                raise RuntimeError(
+                    f"faiss_factory {factory_string!r}: the number of {name} sub-quantizers must be a multiple of 4, "
+                    f"at most {_PQ_M_MAX}, that divides d={dim}, got {v}")
+        return FactorySpec("ivf_pqr", int(metric), nlist, M, M2)
     if codec.startswith("PQ"):
         M = int(m.group(3))
         if M % 4 != 0 or M > _PQ_M_MAX or dim % M != 0:

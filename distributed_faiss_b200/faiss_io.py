@@ -29,6 +29,9 @@ Layout (little endian, no padding; `vec<T>` = u64 count + raw elements):
   IVFPQ    : "IwPQ", ivf hdr, u8 by_residual, u64 code_size, PQ (u64 d, u64 M, u64 nbits,
              vec<f32> centroids [M][ksub][dsub]), invlists (code = M bytes; nbits 4: ceil(M / 2)
              bytes, two codes per byte, low nibble first [faiss-upstream: PQEncoderGeneric])
+  IVFPQR   : "IwQR", the IVFPQ body (8-bit codes), then the refinement PQ (u64 d, u64 M2, u64 nbits = 8,
+             vec<f32> centroids [M2][256][d / M2]), vec<u8> refine codes [ntotal][M2] in id order,
+             f32 k_factor [faiss-upstream: IndexIVFPQR, index_write.cpp]
   IVFSQ    : "IwSq", ivf hdr, SQ (i32 qtype, i32 rangestat, f32 rangestat_arg, u64 d,
              u64 code_size, vec<f32> trained), u64 code_size, u8 by_residual, invlists
              qtype 4 (fp16): trained empty, code = d little-endian fp16 of the residual
@@ -232,19 +235,27 @@ def write_index(state: Dict, path: str, nprobe: int = 1) -> None:
             _write_ivf_header(f, state, int(state["metric"]), int(state["metric"]), nprobe)
             vecs = np.ascontiguousarray(state["vecs"], dtype=np.float32)
             _write_invlists(f, state["list_off"], state["ids"], vecs, 4 * int(state["d"]))
-        elif kind == "ivf_pq":
+        elif kind in ("ivf_pq", "ivf_pqr"):
             M, ksub = int(state["M"]), int(state["ksub"])
             nbits = {256: 8, 16: 4}.get(ksub)
             if nbits is None:
                 raise FaissFormatError(f"only 8-bit and 4-bit product quantizers are supported, got ksub={ksub}")
             codes = _pack_pq_codes(np.asarray(state["codes"], dtype=np.uint8).reshape(-1, M), nbits)
-            f.write(b"IwPQ")
+            if kind == "ivf_pqr" and nbits != 8:
+                raise FaissFormatError(f"IndexIVFPQR: 8-bit codes only, got ksub={ksub}")
+            f.write(b"IwPQ" if kind == "ivf_pq" else b"IwQR")
             _write_ivf_header(f, state, METRIC_L2, int(state["coarse_metric"]), nprobe)
             _w(f, "B", 1)  # by_residual
             _w(f, "Q", codes.shape[1])  # code_size
             _w(f, "QQQ", int(state["d"]), M, nbits)
             _wvec(f, state["codebooks"], np.float32)
             _write_invlists(f, state["list_off"], state["ids"], codes, codes.shape[1])
+            if kind == "ivf_pqr":
+                M2 = int(state["M2"])
+                _w(f, "QQQ", int(state["d"]), M2, 8)
+                _wvec(f, state["refine_codebooks"], np.float32)
+                _wvec(f, np.asarray(state["refine_codes"], dtype=np.uint8).reshape(-1, M2), np.uint8)
+                _w(f, "f", float(state.get("k_factor", 4.0)))
         elif kind == "ivf_pq_fs":
             # faiss stores FastScan codes (IwPf) in blocks of bbs vectors with the nibbles permuted for
             # its SIMD lookups; that layout has never been checked against faiss, so it is not written
@@ -282,10 +293,10 @@ def read_index(path: str) -> Tuple[Dict, int]:
         if cc in ("IxFI", "IxF2", "IxFl"):
             st = _read_flat_body(f, cc)
             return st, 1
-        if cc not in ("IwFl", "IwPQ", "IwSq"):
+        if cc not in ("IwFl", "IwPQ", "IwQR", "IwSq"):
             raise FaissFormatError(
                 f"faiss index type {cc!r} is not one of the types the GPU search path serves "
-                "(IndexFlat, IndexIVFFlat, IndexIVFPQ, IndexIVFScalarQuantizer fp16 / 8bit)")
+                "(IndexFlat, IndexIVFFlat, IndexIVFPQ, IndexIVFPQR, IndexIVFScalarQuantizer fp16 / 8bit)")
         d, ntotal, metric, nlist, nprobe, cent, cmetric = _read_ivf_header(f)
         st = {"d": d, "nlist": nlist, "centroids": cent}
         if cc == "IwFl":
@@ -293,7 +304,7 @@ def read_index(path: str) -> Tuple[Dict, int]:
             if cs != 4 * d:
                 raise FaissFormatError("IndexIVFFlat code size is not 4 * d")
             st.update(kind="ivf_flat", metric=metric, vecs=rows.view(np.float32).reshape(-1, d))
-        elif cc == "IwPQ":
+        elif cc in ("IwPQ", "IwQR"):
             (by_res,) = _r(f, "B")
             (code_size,) = _r(f, "Q")
             pd, M, nbits = _r(f, "QQQ")
@@ -309,6 +320,18 @@ def read_index(path: str) -> Tuple[Dict, int]:
             ksub = 1 << nbits
             st.update(kind="ivf_pq", coarse_metric=cmetric, M=M, ksub=ksub,
                       codebooks=cb.reshape(M, ksub, d // M), codes=_unpack_pq_codes(rows, M, nbits))
+            if cc == "IwQR":
+                rd, M2, nbits2 = _r(f, "QQQ")
+                rcb = _rvec(f, np.float32)
+                rcodes = _rvec(f, np.uint8)
+                (k_factor,) = _r(f, "f")
+                if nbits != 8 or nbits2 != 8 or rd != d or M2 == 0 or d % M2 != 0 or rcb.size != M2 * 256 * (d // M2):
+                    raise FaissFormatError(f"IndexIVFPQR: only 8-bit codes in both product quantizers are supported "
+                                           f"(nbits={nbits}, refine nbits={nbits2}, M2={M2}, d={d})")
+                if rcodes.size != ntotal * M2:
+                    raise FaissFormatError("IndexIVFPQR: the refine codes do not hold ntotal vectors")
+                st.update(kind="ivf_pqr", M2=int(M2), refine_codebooks=rcb.reshape(M2, 256, d // M2),
+                          refine_codes=rcodes.reshape(ntotal, M2), k_factor=float(k_factor))
         else:
             qtype, rangestat, _ = _r(f, "iif")
             sd, scs = _r(f, "QQ")

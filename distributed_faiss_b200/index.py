@@ -22,9 +22,11 @@ Builders (reference index.py:93-100):
                   for the index and its quantizer, nprobe = the faiss default 1 (index.py:385-396)
 Factory strings are parsed by factory.parse_factory ("Flat", "IVF{n},Flat", "IVF{n},PQ{M}[x8]",
 "IVF{n},PQ{M}x4fs" (FastScan: 4-bit codes of the raw vectors, 8-bit quantized distance tables),
+"IVF{n},PQ{M}+{M2}" (IndexIVFPQR: IVF-PQ candidates re-ranked on a second, M2-byte residual code),
 "IVF{n},SQfp16", "IVF{n},SQ8"); any other string raises, and so does "hnswsq" (a graph index,
 outside the hot path this package rebuilds, SURVEY.md section 8).  A stored shard is only loaded
-under a cfg that builds the same kind (and, for the PQ kinds, the same (M, ksub)).
+under a cfg that builds the same kind (and, for the PQ kinds, the same (M, ksub), and for
+IVF-PQR the same M2).
 """
 import _thread
 import logging
@@ -80,7 +82,7 @@ def default_engine_factory(cfg: IndexCfg, device: Optional[int] = None):
         kind = {name: k for k, name in engine.KIND_NAMES.items()}[spec.kind]
         nbits = 4 if spec.kind == "ivf_pq_fs" else 8  # FastScan: 4-bit codes
         idx = engine.GpuIndex(kind, cfg.dim, spec.metric, nlist=spec.nlist, pq_m=spec.pq_m, pq_nbits=nbits,
-                              device=device)
+                              device=device, refine_m=spec.refine_m)
         if cfg.index_builder_type == "ivf_gpu":
             idx.nprobe = cfg.nprobe  # index.py:84
         # the factory path keeps faiss's default nprobe (1) and leaves cfg.nprobe alone, unlike
@@ -572,6 +574,14 @@ class Index:
             if stored != built:
                 raise RuntimeError(f"the stored IVF-PQ index has (M, ksub) = {stored} but the cfg builds {built}; "
                                    "refusing to load it")
+        if want == "ivf_pqr":
+            # the refinement codes are M2 bytes per vector: another M2 would misread every one of them
+            stored = (int(state["M"]), int(state["ksub"]), int(state["M2"]))
+            built = (int(getattr(engine, "pq_m", getattr(engine, "M", 0))), int(engine.ksub),
+                     int(getattr(engine, "refine_m", getattr(engine, "M2", 0))))
+            if stored != built:
+                raise RuntimeError(f"the stored IVF-PQR index has (M, ksub, M2) = {stored} but the cfg builds "
+                                   f"{built}; refusing to load it")
         engine.set_state(state)
         assert len(meta) >= engine.ntotal, "Deserialized meta list should be at least of index size"
         result.faiss_index = engine

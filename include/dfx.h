@@ -43,10 +43,15 @@ enum {
     DFX_IVF_SQ16 = 3, /* faiss.IndexIVFScalarQuantizer(QT_fp16)   index.py:63-68     */
     DFX_IVF_SQ8 = 4,  /* faiss.IndexIVFScalarQuantizer(QT_8bit), by_residual: the factory string
                          "IVF{n},SQ8" (index.py:380-396) -- one byte per dimension */
-    DFX_IVF_PQ_FS = 5 /* faiss.IndexIVFPQFastScan(nbits = 4), NOT by_residual: the factory string
+    DFX_IVF_PQ_FS = 5, /* faiss.IndexIVFPQFastScan(nbits = 4), NOT by_residual: the factory string
                          "IVF{n},PQ{M}x4fs" (index.py:380-396).  4-bit codes packed two per byte; the
                          search quantizes each query's distance table to 8 bits and sums it in
                          integers (DESIGN.md section 2).  L2 only, for the index and its quantizer */
+    DFX_IVF_PQR = 6   /* faiss.IndexIVFPQR: the factory string "IVF{n},PQ{M}+{M2}" (index.py:380-396).
+                         An 8-bit IVF-PQ (by_residual) whose residual error is encoded again by a second
+                         8-bit PQ of M2 bytes, stored by id outside the lists.  A search runs the IVF-PQ
+                         search for k' = k * k_factor candidates and re-ranks them on the reconstruction
+                         c + PQ1 + PQ2 (DESIGN.md section 2).  L2 only, for the index and its quantizer */
 };
 
 /* faiss.METRIC_INNER_PRODUCT / faiss.METRIC_L2 (index_cfg.py:44-52) */
@@ -59,15 +64,17 @@ typedef struct dfx_cfg {
                          index, which is therefore always L2 (index.py:44-46, 64-66).
                          IVF_PQ_FS: must be L2 (an inner-product metric is refused). */
     int32_t d;        /* vector dimension (cfg.dim) */
-    int32_t pq_m;     /* IVF_PQ: sub-quantizers  (cfg.extra["code_size"], index.py:44).  8-bit codes:
-                         4 <= M <= 128, M % 4 == 0, d % M == 0 (128: one query's fp32 table,
-                         M x 256 x 4 B, must fit in one thread block's shared memory).  4-bit codes
-                         and IVF_PQ_FS: 8 <= M <= 128, M % 8 == 0, d % M == 0 */
+    int32_t pq_m;     /* IVF_PQ: sub-quantizers  (cfg.extra["code_size"], index.py:44).  8-bit codes
+                         (and IVF_PQR): 4 <= M <= 128, M % 4 == 0, d % M == 0 (128: one query's fp32
+                         table, M x 256 x 4 B, must fit in one thread block's shared memory).  4-bit
+                         codes and IVF_PQ_FS: 8 <= M <= 128, M % 8 == 0, d % M == 0 */
     int32_t pq_nbits; /* IVF_PQ: bits per code   (cfg.extra["bits_per_vector"], index.py:45): 8, or 4
                          (ksub = 16; codes stored two per byte, low nibble first, as faiss packs
-                         them).  IVF_PQ_FS: must be 4 */
+                         them).  IVF_PQ_FS: must be 4.  IVF_PQR: must be 8 */
     int32_t device;   /* CUDA device ordinal this shard lives on */
     int64_t nlist;    /* IVF_*: number of inverted lists (cfg.centroids); IVF kinds need d % 4 == 0 */
+    int32_t refine_m; /* IVF_PQR: sub-quantizers of the refinement PQ (M2; 8 bits each): 4 <= M2 <= 128,
+                         M2 % 4 == 0, d % M2 == 0.  Must be 0 for every other kind */
 } dfx_cfg;
 
 /* ---- lifetime: replaces the faiss constructors at index.py:25-48,63-68,94 ---- */
@@ -96,14 +103,21 @@ int dfx_add_dev(dfx_index *idx, int64_t n, const float *d_x, void *stream);
  * "il2_threads" (0 = 256) / "il2_prefetch" (-1 = 4 blocks): CTA shape and L2 prefetch distance of
  *   that scan (tuning; 512 threads at k > 512 do not fit in shared memory and run with 256);
  * "rows_inflight" (0 = by row size): 4 or 8 vectors per warp in flight in the IVF-Flat / IVF-SQ
- *   list scan */
+ *   list scan;
+ * "k_factor" (4, IVF_PQR only; this knob DOES change results): a search for k results re-ranks the
+ *   k' = (int64)((float)k * k_factor) best candidates of the IVF-PQ stage, as faiss's
+ *   IndexIVFPQR::k_factor; values below 1 are refused, and a search whose k' exceeds 16384 raises
+ *   before launching anything */
 int dfx_set_param(dfx_index *idx, const char *name, double value);
 /* read back a knob or a counter: the names of dfx_set_param, plus "tc_fast" (the precision the
  * next screening launch will use: 1 = FAST), "tc_stat_rows" / "tc_stat_overflow" /
  * "tc_stat_fast_would" (rows, rows re-done exactly, and rows FAST would have re-done, of the last
  * launch whose statistics came back; synchronises with that launch), "workspace_bytes" (bytes of
  * the partial-result workspace, the largest any search so far has needed, including the candidate
- * rows of IVF searches with k > 1024; IVF searches keep it within 128 MiB by their query chunk) */
+ * rows of IVF searches with k > 1024; IVF searches keep it within 128 MiB by their query chunk),
+ * "refine_ms" / "refine_launches" (IVF_PQR with profiling on: summed device time and number of
+ * the refinement stages -- re-rank kernel and final selection -- since the last reset of
+ * dfx_profile_read; synchronises) */
 int dfx_get_param(dfx_index *idx, const char *name, double *value);
 /* pre-size the shard for n_total vectors (optional; avoids regrowth while bulk loading) */
 int dfx_reserve(dfx_index *idx, int64_t n_total);
@@ -113,7 +127,9 @@ int dfx_finalize(dfx_index *idx, void *stream);
 /* ---- THE HOT PATH: faiss_index.search(query_batch, top_k) index.py:257 ----
  * D float32[nq,k], I int64[nq,k], 1 <= k <= 4096 for every kind.  An IVF search with k > 1024
  * writes every probed vector's candidate and selects per query; it raises an error before launching
- * anything when the nprobe longest lists together exceed 2^24 vectors (128 MiB of candidates). */
+ * anything when the nprobe longest lists together exceed 2^24 vectors (128 MiB of candidates).
+ * IVF_PQR: the IVF-PQ stage runs at k' = k * k_factor (at most 16384; k' > 1024 takes the candidate
+ * rows), and the k' candidates are re-ranked and selected down to k. */
 int dfx_search(dfx_index *idx, int64_t nq, const float *x, int64_t k, float *D, int64_t *I);
 int dfx_search_dev(dfx_index *idx, int64_t nq, const float *d_x, int64_t k, float *d_D,
                    int64_t *d_I, void *stream);
@@ -192,16 +208,20 @@ int dfx_map_ids_dev(int64_t n, const int64_t *d_ids, const int64_t *d_table, int
  *   "vecs" f32[ntotal,d] (IVF_FLAT)   "codes16" u16[ntotal,d]   "xb" f32[ntotal,d] (FLAT)
  *   "sq_trained" f32[2,d] (IVF_SQ8: vmin, then vdiff -- faiss's ScalarQuantizer::trained)
  *   "codes8" u8[ntotal,d] (IVF_SQ8)
+ *   (IVF_PQR: the IVF_PQ arrays with 8-bit codes, plus "refine_codebooks" f32[M2,256,d/M2] and
+ *   "refine_codes" u8[ntotal,M2] in ID order, not list order; its "ids" must be a permutation of
+ *   0 .. ntotal-1, and "tvals" is recomputed on import)
  * dfx_get_array with out == NULL only reports the size.  Import order: centroids,
- * codebooks (IVF_PQ, IVF_PQ_FS) or sq_trained (IVF_SQ8), then list_off, ids and the payload, then
- * dfx_import_done(). */
+ * codebooks (IVF_PQ, IVF_PQ_FS, IVF_PQR) or sq_trained (IVF_SQ8), refine_codebooks (IVF_PQR), then
+ * list_off, ids and the payload, refine_codes (IVF_PQR), then dfx_import_done(). */
 int dfx_get_array(dfx_index *idx, const char *name, void *out, int64_t max_bytes,
                   int64_t *nbytes);
 int dfx_set_array(dfx_index *idx, const char *name, const void *in, int64_t nbytes);
 int dfx_import_done(dfx_index *idx);
 
 /* statistics of the most recent search (device work, synchronises):
- * ndis = sum over (query, probed list) of the list length -- faiss's `ndis`. */
+ * ndis = sum over (query, probed list) of the list length -- faiss's `ndis` (IVF_PQR: of the
+ * IVF-PQ stage; the re-ranked candidates are not counted). */
 int dfx_last_stats(dfx_index *idx, int64_t *ndis, int64_t *nq, int64_t *nprobe);
 /* per-kernel timing of the dominant kernel (the inverted-list scan): when enabled, every scan
  * launch is bracketed by CUDA events on the launching stream; dfx_profile_read synchronises
