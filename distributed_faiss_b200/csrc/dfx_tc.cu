@@ -143,11 +143,12 @@ constexpr int MAX_RESIDENT_KATOMS = 4;  // query tile resident in shared memory 
 //           k-step; error <= |q||c| 2^-17 (the dropped ql.cl term is 2^-22, hi + lo carries 22 bits)
 // shared-memory plan (offsets inside the 1024-aligned dynamic block)
 //   resident A (NPL x katoms <= 4): A = NPL x katoms x 16 KB, then a ring of B stages of 16 KB that
-//                          holds two tiles, at least 4 stages (FAST d <= 128: <= 99 KB, two CTAs per
-//                          SM; PRECISE d = 128 and FAST d = 256: 8 stages, 195 KB); the warpgroups run
+//                          holds two tiles, at least 4 stages (FAST d <= 128: <= 103 KB, two CTAs per
+//                          SM; PRECISE d = 128 and FAST d = 256: 8 stages, 199 KB); the warpgroups run
 //                          a tile apart, and the one behind still reads the stages of the tile before
 //   streamed A (larger d): a ring of 6 stages of (A atom + B atom) = 32 KB
-//   then 512 B of mbarriers and each warpgroup's copy of the tile's ranking offsets, [2][2][TILE] floats
+//   then 512 B of mbarriers, each warpgroup's copy of the tile's ranking offsets, [2][2][TILE] floats,
+//   and the held summary of an even tile, [CONSUMERS / 2][2] float4 (4 KB)
 struct Smem {
     static constexpr bool resident(int katoms, int npl) { return npl * katoms <= MAX_RESIDENT_KATOMS; }
     static constexpr int nstage(bool res, int katoms, int npl) {
@@ -156,7 +157,8 @@ struct Smem {
     static constexpr int stage_bytes(bool res) { return res ? ATOM_BYTES : 2 * ATOM_BYTES; }
     static constexpr int RING(bool res, int katoms, int npl) { return res ? npl * katoms * ATOM_BYTES : 0; }
     static constexpr int BARS(bool res, int katoms, int npl) { return RING(res, katoms, npl) + nstage(res, katoms, npl) * stage_bytes(res); }
-    static constexpr int total(bool res, int katoms, int npl) { return BARS(res, katoms, npl) + 512 + 4 * TILE * 4; }
+    static constexpr int HELD(bool res, int katoms, int npl) { return BARS(res, katoms, npl) + 512 + 4 * TILE * 4; }
+    static constexpr int total(bool res, int katoms, int npl) { return HELD(res, katoms, npl) + CONSUMERS / 2 * 32; }
     // CTAs that fit one SM (228 KB of shared memory): two when a CTA's block (+ 1 KB for the
     // alignment) stays within 113 KB, which only FAST shapes reach
     static constexpr int ctas_per_sm(bool res, int katoms, int npl) {
@@ -382,6 +384,7 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     uint64_t* empty = bars + NSTAGE;       // [NSTAGE]
     uint64_t* a_full = bars + 2 * NSTAGE;  // [1]
     float* s_cn = reinterpret_cast<float*>(smem + Smem::BARS(RES, KATOMS, NPL) + 512);  // [warpgroup][2][TN]
+    float4* s_held = reinterpret_cast<float4*>(smem + Smem::HELD(RES, KATOMS, NPL));   // [CONSUMERS / 2][2]
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int qt = blockIdx.y;
@@ -458,6 +461,14 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     if (RES) mbar_wait(a_full, 0);
     int stage = 0, phase = 0;
     float acc[64];
+    // The summary of an even centroid tile is held until the odd tile after it is done: lane q of
+    // a quad then writes row row0 + 8 (q >> 1) of tile parity q & 1, so that adjacent lanes fill one
+    // sector of each array in one store.  The stores, not the arithmetic, bounded the epilogue:
+    // one partial sector per array, row and tile.  Lanes of parity 0 hold (gmin, gmin2) of their
+    // row in shared memory (registers would spill under the two-CTA cap).
+    const int hq = quad >> 1, pq = quad & 1;
+    const int64_t grow_q = grow0 + 8 * hq;
+    float4* held = s_held + 2 * (threadIdx.x >> 1);  // parity-0 lanes: [gmin, gmin2]
     // one wgmma group stays in flight while the next stage is awaited: a stage is released once
     // the group after it has been issued and the group that read it has completed
     auto release = [&](int s) {
@@ -544,22 +555,35 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
                 ga[h] |= (__float_as_uint(m1) & 31u) << (8 * g);
             }
         }
-        // lane 0 of a quad writes row0, lane 1 row0 + 8
-        if (quad < 2) {
-            const bool h = quad == 1;
-            const int64_t grow = grow0 + (h ? 8 : 0);
-            if (grow < nq) {
-                const int64_t o = grow * ng + (col0 >> 5);
-                const float4 m = h ? make_float4(gm[1][0], gm[1][1], gm[1][2], gm[1][3])
-                                   : make_float4(gm[0][0], gm[0][1], gm[0][2], gm[0][3]);
-                const float4 m2 = h ? make_float4(gm2[1][0], gm2[1][1], gm2[1][2], gm2[1][3])
-                                    : make_float4(gm2[0][0], gm2[0][1], gm2[0][2], gm2[0][3]);
-                *reinterpret_cast<float4*>(gmin + o) = m;
-                *reinterpret_cast<float4*>(gmin2 + o) = m2;
-                *reinterpret_cast<uint32_t*>(gargc + o) = h ? ga[1] : ga[0];
-                // the tile's minimum: the first level of the group selection (topg_collect_kernel)
-                tmin[grow * (ng >> 2) + (col0 >> 7)] = fminf(fminf(m.x, m.y), fminf(m.z, m.w));
+        // every lane of a quad holds both rows' results; lane q takes row row0 + 8 (q >> 1)
+        const float4 m = hq ? make_float4(gm[1][0], gm[1][1], gm[1][2], gm[1][3])
+                            : make_float4(gm[0][0], gm[0][1], gm[0][2], gm[0][3]);
+        const float4 m2 = hq ? make_float4(gm2[1][0], gm2[1][1], gm2[1][2], gm2[1][3])
+                             : make_float4(gm2[0][0], gm2[0][1], gm2[0][2], gm2[0][3]);
+        const uint32_t a = hq ? ga[1] : ga[0];
+        const int ct = ct0 + t;                           // global index of this centroid tile
+        if (!(ct & 1) && t + 1 < ntiles) {                // even tile with its odd partner to come
+            if (pq == 0) {
+                held[0] = m;
+                held[1] = m2;
             }
+            continue;
+        }
+        const bool pair = (ct & 1) && t > 0;              // the held even tile goes out with this one
+        if ((pair || pq == 0) && grow_q < nq) {
+            const bool old = pair && pq == 0;             // lane writes the held tile ct - 1
+            const float4 wm = old ? held[0] : m, wm2 = old ? held[1] : m2;
+            const int wct = old ? ct - 1 : ct;
+            const int64_t o = grow_q * ng + 4 * wct;
+            *reinterpret_cast<float4*>(gmin + o) = wm;
+            *reinterpret_cast<float4*>(gmin2 + o) = wm2;
+            // gmin carries its arg-min column in its 5 low bits
+            *reinterpret_cast<uint32_t*>(gargc + o) =
+                old ? (__float_as_uint(wm.x) & 31u) | (__float_as_uint(wm.y) & 31u) << 8 |
+                          (__float_as_uint(wm.z) & 31u) << 16 | (__float_as_uint(wm.w) & 31u) << 24
+                    : a;
+            // the tile's minimum: the first level of the group selection (topg_collect_kernel)
+            tmin[grow_q * (ng >> 2) + wct] = fminf(fminf(wm.x, wm.y), fminf(wm.z, wm.w));
         }
     }
 }
