@@ -166,6 +166,17 @@ int dfx_create(const dfx_cfg* cfg, dfx_index** out) {
         idx->M2 = cfg->refine_m;
         idx->dsub2 = cfg->d / cfg->refine_m;
     }
+    if (cfg->refine_flat) {
+        // flat refinement (faiss IndexRefineFlat): exact re-ranking only makes sense over a lossy codec
+        DFX_REQUIRE(cfg->kind != DFX_FLAT && cfg->kind != DFX_IVF_FLAT,
+                    "refine_flat must be 0 for FLAT and IVF_FLAT: their distances are already exact");
+        DFX_REQUIRE(cfg->kind != DFX_IVF_PQR, "refine_flat must be 0 for IVF_PQR: it has its own refinement");
+        DFX_REQUIRE(cfg->kind != DFX_IVF_PQ || cfg->pq_nbits == 8,
+                    "refine_flat must be 0 for IVF-PQ with 4-bit codes (IVF-PQ FastScan takes it)");
+        DFX_REQUIRE(cfg->metric == DFX_METRIC_L2,
+                    "flat refinement: only the L2 metric is supported (for the index and its coarse quantizer)");
+        idx->k_factor = 1.f;  // faiss IndexRefine default
+    }
     DeviceGuard g(cfg->device);
     DFX_CUDA(cudaStreamCreateWithFlags(&idx->stream, cudaStreamNonBlocking));
     *out = idx.release();
@@ -237,7 +248,8 @@ int dfx_set_param(dfx_index* idx, const char* name, double value) {
         idx->il2_prefetch = (int)value;
     }
     else if (n == "k_factor") {
-        DFX_REQUIRE(idx->cfg.kind == DFX_IVF_PQR, "k_factor is a parameter of IVF-PQR indexes");
+        DFX_REQUIRE(idx->cfg.kind == DFX_IVF_PQR || idx->rflat(),
+                    "k_factor is a parameter of IVF-PQR indexes and of indexes with a flat refinement");
         DFX_REQUIRE(value >= 1 && value <= 16384, "k_factor must be in [1, 16384]");
         idx->k_factor = (float)value;
     }
@@ -283,7 +295,7 @@ int dfx_get_param(dfx_index* idx, const char* name, double* value) {
     else if (n == "il2_prefetch") *value = idx->il2_prefetch;
     else if (n == "rows_inflight") *value = idx->rows_inflight;
     else if (n == "workspace_bytes") *value = (double)idx->w_part.cap;  // read-only
-    else if (n == "k_factor" && idx->cfg.kind == DFX_IVF_PQR) *value = idx->k_factor;
+    else if (n == "k_factor" && (idx->cfg.kind == DFX_IVF_PQR || idx->rflat())) *value = idx->k_factor;
     else if (n == "refine_ms" || n == "refine_launches") {  // read-only
         std::lock_guard<std::mutex> lk(idx->mu);
         DeviceGuard g(idx->cfg.device);
@@ -577,6 +589,7 @@ int dfx_get_array(dfx_index* idx, const char* name, void* out, int64_t max_bytes
     else if (n == "tvals" && idx->pq_res()) { src = idx->tvals.p; bytes = nt * 4; }
     else if (n == "refine_codebooks" && idx->cfg.kind == DFX_IVF_PQR && idx->trained) { src = idx->refine_cb.p; bytes = (int64_t)idx->M2 * 256 * idx->dsub2 * 4; }
     else if (n == "refine_codes" && idx->cfg.kind == DFX_IVF_PQR) { src = idx->refine_codes.p; bytes = nt * idx->M2; }
+    else if (n == "refine_vecs" && idx->rflat()) { src = idx->refine_vecs.p; bytes = nt * d * 4; }
     else if (unpack4) { bytes = nt * idx->M; }
     else if (n == payload_name(idx->cfg.kind)) { src = idx->payload.p; bytes = nt * (int64_t)idx->row_bytes(); }
     else throw DfxError{"no array named '" + n + "' in this index"};
@@ -637,6 +650,11 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
                     "refine_codes: wrong size (u8[ntotal, M2] in id order; set list_off first)");
         upload(idx->refine_codes, nbytes);
         idx->refine_cap = idx->refine_rows = idx->n_sorted;
+    } else if (n == "refine_vecs" && idx->rflat()) {
+        DFX_REQUIRE(nbytes == idx->n_sorted * d * 4,
+                    "refine_vecs: wrong size (f32[ntotal, d] in id order; set list_off first)");
+        upload(idx->refine_vecs, nbytes);
+        idx->refine_cap = idx->refine_rows = idx->n_sorted;
     } else if (n == "list_off" && idx->is_ivf()) {
         DFX_REQUIRE(nbytes == (nlist + 1) * 8, "list_off: wrong size");
         upload(idx->list_off, nbytes);
@@ -653,12 +671,13 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
             DFX_REQUIRE(s[i] >= 0 && s[i] < (1ll << 31), "ids must be in [0, 2^31)");
             tmp[(size_t)i] = (int32_t)s[i];
         }
-        if (idx->cfg.kind == DFX_IVF_PQR) {
-            // the refine codes are addressed by id (faiss asserts the same of IndexIVFPQR)
+        if (idx->cfg.kind == DFX_IVF_PQR || idx->rflat()) {
+            // the refine codes / rows are addressed by id (faiss asserts the same of IndexIVFPQR)
             std::vector<char> seen((size_t)idx->n_sorted, 0);
             for (int64_t i = 0; i < idx->n_sorted; i++) {
                 DFX_REQUIRE(s[i] < idx->n_sorted && !seen[(size_t)s[i]],
-                            "ids: an IVF-PQR index needs ids that are a permutation of 0 .. ntotal-1");
+                            std::string("ids: ") + (idx->rflat() ? "a flat refinement" : "an IVF-PQR index") +
+                                " needs ids that are a permutation of 0 .. ntotal-1");
                 seen[(size_t)s[i]] = 1;
             }
         }
@@ -711,6 +730,8 @@ int dfx_import_done(dfx_index* idx) {
             DFX_REQUIRE(idx->refine_cb.p, "import: refine_codebooks are required");
             DFX_REQUIRE(idx->refine_rows == idx->n_sorted, "import: refine_codes of every vector are required");
         }
+        if (idx->rflat())
+            DFX_REQUIRE(idx->refine_rows == idx->n_sorted, "import: refine_vecs of every vector are required");
         if (idx->pq_res()) {
             DFX_REQUIRE(idx->codebooks.p, "import: codebooks are required");
             dfx_compute_tvals_sorted(idx, idx->stream);  // K7 recomputes the per-vector term

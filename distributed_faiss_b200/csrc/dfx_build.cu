@@ -647,6 +647,18 @@ void dfx_add_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) 
         DFX_LAUNCH(sq8_encode_kernel, blocks_for(n * d, 256), 256, 0, st, d_x, idx->centroids.as<float>(),
                    plist, n, d, idx->sq_trained.as<float>(), (uint8_t*)prow);
     }
+    if (idx->rflat()) {
+        // the raw rows by id: the new rows get the ids ntotal .. ntotal + n - 1, so they append
+        const int64_t id0 = idx->ntotal();
+        const size_t rowb = (size_t)d * 4;
+        if (id0 + n > idx->refine_cap) {
+            const int64_t cap = std::max<int64_t>({id0 + n, 2 * idx->refine_cap, idx->reserve_hint});
+            idx->refine_vecs.reserve((size_t)cap * rowb, (size_t)id0 * rowb, st);
+            idx->refine_cap = cap;
+        }
+        DFX_CUDA(cudaMemcpyAsync(idx->refine_vecs.as<unsigned char>() + (size_t)id0 * rowb, d_x, (size_t)n * rowb,
+                                 cudaMemcpyDeviceToDevice, st));
+    }
     idx->n_pending += n;
 }
 
@@ -902,6 +914,14 @@ void dfx_reconstruct_impl(dfx_index* idx, int64_t n, const int64_t* d_ids, float
     if (idx->n_pending > 0) dfx_finalize_impl(idx, st);
     const int64_t nt = idx->n_sorted;
     const int il = idx->il ? 2 : 0;  // 0 = row-major, else the block layout
+    if (idx->rflat()) {
+        // the stored row, addressed by id as a FLAT index addresses its rows
+        DFX_LAUNCH(reconstruct_kernel<8>, (unsigned)n, 128, 0, st, (int)DFX_FLAT, idx->cfg.d, 0, 0, 0, nt,
+                   (int64_t)0, d_ids, (const int32_t*)nullptr, (const void*)idx->refine_vecs.p,
+                   (const int64_t*)nullptr, (const float*)nullptr, (const float*)nullptr, 0,
+                   (const int64_t*)nullptr, d_out, tag);
+        return;
+    }
     dfx_refresh_inv(idx, st);
     if (idx->cfg.kind == DFX_IVF_PQR) {
         DFX_LAUNCH(pqr_reconstruct_kernel, (unsigned)n, 128, 0, st, idx->cfg.d, idx->M, idx->dsub, idx->M2, idx->dsub2,

@@ -97,6 +97,9 @@ struct dfx_index {
     DevBuf refine_cb, refine_codes;
     int64_t refine_cap = 0, refine_rows = 0;  // rows allocated / rows imported (dfx_set_array)
     DevBuf w_rD, w_rI, w_rcomp;
+    // flat refinement (cfg.refine_flat): the raw rows by id (f32[ntotal][d], arrival order), sharing
+    // refine_cap / refine_rows, k_factor (default 1, faiss IndexRefine) and the workspace above
+    DevBuf refine_vecs;
 
     // scan-kernel profiling (dfx_profile_enable)
     bool prof_on = false;
@@ -175,6 +178,7 @@ struct dfx_index {
         for (size_t l = 0; l < nl; l++) h_len_top[l + 1] = h_len_top[l] + len[l];
     }
     bool is_ivf() const { return cfg.kind != DFX_FLAT; }
+    bool rflat() const { return cfg.refine_flat != 0; }
     // the kinds with PQ codebooks (IVF_PQ / IVF_PQR: residual codes, IVF_PQ_FS: codes of the raw vectors)
     bool has_pq() const { return cfg.kind == DFX_IVF_PQ || cfg.kind == DFX_IVF_PQ_FS || cfg.kind == DFX_IVF_PQR; }
     // the kinds whose lists hold IVF-PQ residual codes with t-values (IVF_PQR: its first stage)

@@ -17,6 +17,8 @@
 //                         every vector's composite, MAT = true, and select_cand picks the k best)
 //   K_r  pqr_refine       IVF-PQR: re-ranks the k' = k * k_factor candidates of the IVF-PQ stage on
 //                         c + PQ1 + PQ2 (dfx_refine_dev.cuh), then K_sel picks the k best
+//   K_rf rflat_refine     flat refinement (",RFlat"): re-ranks the k' candidates of the base kind's stage
+//                         on the stored fp32 rows (dfx_rflat_dev.cuh), then K_sel picks the k best
 //   K6   merge            cross-shard merge (float_maxheap_array_t semantics)
 // Arithmetic orders are the canonical ones of oracle/dfx_oracle.c (bit-exact parity).
 #include "dfx_internal.h"
@@ -206,6 +208,7 @@ void dfx_launch_select_comp(const uint64_t* comp, int64_t nrows, int n, int64_t 
 #include "dfx_scan_pq4_dev.cuh"
 #include "dfx_scan_pq_fs_dev.cuh"
 #include "dfx_refine_dev.cuh"
+#include "dfx_rflat_dev.cuh"
 
 // scan_pq_fs_kernel<M, MAT> for the runtime M (a multiple of 8 in [8, 128], checked by dfx_create)
 template <bool MAT, int MT = 8>
@@ -746,12 +749,13 @@ select_cand_kernel(const uint64_t* __restrict__ cand, const int64_t* __restrict_
 }
 
 // =====================================================================================
-// IVF-PQR: re-rank the k1 = k' candidates of each query of a chunk (cand [qc][k1], the ids the
-// IVF-PQ stage selected) and select the k best into (D, I) -- the order and the padding are those
-// of every other kind.  Bracketed by the refine profiling events (dfx_get_param "refine_ms").
+// IVF-PQR and the flat refinement: re-rank the k1 = k' candidates of each query of a chunk (cand
+// [qc][k1], the ids the first stage selected) and select the k best into (D, I) -- the order and
+// the padding are those of every other kind.  Bracketed by the refine profiling events
+// (dfx_get_param "refine_ms").
 // =====================================================================================
-static void pqr_refine(dfx_index* idx, const float* xq, int64_t qc, int k1, int k, const int64_t* cand, float* D,
-                       int64_t* I, cudaStream_t st) {
+static void refine_candidates(dfx_index* idx, const float* xq, int64_t qc, int k1, int k, const int64_t* cand,
+                              float* D, int64_t* I, cudaStream_t st) {
     std::pair<cudaEvent_t, cudaEvent_t>* pev = nullptr;
     if (idx->prof_on) {
         if (idx->prof_refine_used == idx->prof_refine_events.size()) {
@@ -765,12 +769,22 @@ static void pqr_refine(dfx_index* idx, const float* xq, int64_t qc, int k1, int 
     }
     const int64_t nc = qc * k1;
     uint64_t* comp = idx->w_rcomp.as<uint64_t>();
-    const int il = idx->il ? 1 : 0;
-    DFX_LAUNCH(pqr_refine_kernel, (unsigned)dfx_ceil_div(nc, PQR_WARPS), 32 * PQR_WARPS, 0, st, xq, idx->cfg.d, nc, k1,
-               cand, idx->inv.as<int32_t>(), il ? idx->blk_off.as<int64_t>() : idx->list_off.as<int64_t>(),
-               idx->cfg.nlist, il, il ? idx->il_codes.as<uint8_t>() : idx->payload.as<uint8_t>(), idx->M, idx->dsub,
-               idx->codebooks.as<float>(), idx->refine_codes.as<uint8_t>(), idx->M2, idx->dsub2,
-               idx->refine_cb.as<float>(), idx->centroids.as<float>(), comp);
+    if (idx->rflat()) {
+        // exact distances on the stored fp32 rows; rows of up to 1 KB: two candidates per warp in flight
+        const int d = idx->cfg.d;
+        const int U = (size_t)d * 4 <= 1024 ? 2 : 1;
+        const int cpq = (k1 + RFLAT_WARPS * U - 1) / (RFLAT_WARPS * U);
+        auto kern = U == 2 ? rflat_refine_kernel<2> : rflat_refine_kernel<1>;
+        DFX_LAUNCH(kern, (unsigned)(qc * cpq), 32 * RFLAT_WARPS, (size_t)d * 4, st, xq, d, k1, cpq, cand,
+                   idx->refine_vecs.as<float>(), comp);
+    } else {
+        const int il = idx->il ? 1 : 0;
+        DFX_LAUNCH(pqr_refine_kernel, (unsigned)dfx_ceil_div(nc, PQR_WARPS), 32 * PQR_WARPS, 0, st, xq, idx->cfg.d, nc,
+                   k1, cand, idx->inv.as<int32_t>(), il ? idx->blk_off.as<int64_t>() : idx->list_off.as<int64_t>(),
+                   idx->cfg.nlist, il, il ? idx->il_codes.as<uint8_t>() : idx->payload.as<uint8_t>(), idx->M,
+                   idx->dsub, idx->codebooks.as<float>(), idx->refine_codes.as<uint8_t>(), idx->M2, idx->dsub2,
+                   idx->refine_cb.as<float>(), idx->centroids.as<float>(), comp);
+    }
     CompLoader ldr{comp, k1};
     ResultWriter wr{D, I, k, DFX_METRIC_L2, nullptr};
     dfx_launch_select<128>(ldr, wr, qc, k1, k, st);
@@ -798,14 +812,15 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
     if (nq <= 0) return;
     if (idx->n_pending > 0) dfx_finalize_impl(idx, st);
     const int d = idx->cfg.d;
-    // IVF-PQR: the IVF-PQ search for k' = (int64)(k * k_factor) candidates (faiss's float product)
-    // into workspace rows, re-ranked per query chunk down to kout = k; every sizing rule below
-    // sees k'
-    const bool refine = idx->cfg.kind == DFX_IVF_PQR;
+    // IVF-PQR and the flat refinement: the base kind's search for k' = (int64)(k * k_factor)
+    // candidates (faiss's float product) into workspace rows, re-ranked per query chunk down to
+    // kout = k; every sizing rule below sees k'
+    const bool rflat = idx->rflat();
+    const bool refine = idx->cfg.kind == DFX_IVF_PQR || rflat;
     const int64_t kfirst = refine ? (int64_t)((float)k64 * idx->k_factor) : k64;
     const int kout = (int)k64;
     const int k = (int)std::min<int64_t>(kfirst, 1 << 30);
-    const int kind = refine ? DFX_IVF_PQ : idx->cfg.kind;
+    const int kind = idx->cfg.kind == DFX_IVF_PQR ? DFX_IVF_PQ : idx->cfg.kind;
     idx->last_keys_valid = false;
 
     if (kind == DFX_FLAT) {
@@ -876,8 +891,8 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
     DFX_REQUIRE(k64 <= 4096, "IVF search supports k <= 4096");
     const int pqr_kmax = 16384;  // candidate rows selected by select_cand_kernel: P * 8 = 128 KiB of shared memory
     DFX_REQUIRE(!refine || kfirst <= pqr_kmax,
-                "IVF-PQR search at k=" + std::to_string(k64) + " with k_factor=" + std::to_string(idx->k_factor) +
-                    ": k' = " + std::to_string(kfirst) + " candidates to re-rank, more than " +
+                std::string(rflat ? "RFlat" : "IVF-PQR") + " search at k=" + std::to_string(k64) +
+                    " with k_factor=" + std::to_string(idx->k_factor) + ": k' = " + std::to_string(kfirst) + " candidates to re-rank, more than " +
                     std::to_string(pqr_kmax));
     const int64_t nlist = idx->cfg.nlist;
     int nprobe = (int)std::min<int64_t>(std::max<int64_t>(idx->nprobe, 1), nlist);
@@ -915,7 +930,7 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
         const int64_t ng1 = (nprobe + G1 - 1) / G1;
         QC = std::min(QC, std::max(q1, part_max / (ng1 * k)));
     }
-    // IVF-PQR: the chunk's first-stage rows and refined composites (qc x k' of each) stay within 2^22
+    // refinements: the chunk's first-stage rows and refined composites (qc x k' of each) stay within 2^22
     const int64_t pqr_cand_max = (int64_t)1 << 22;
     if (refine) QC = std::min(QC, std::max<int64_t>(1, pqr_cand_max / k));
     if (QC > nq) QC = nq;
@@ -951,7 +966,7 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
         coff = idx->w_coff.as<int64_t>();
     }
     if (refine) {
-        DFX_REQUIRE(idx->inv_valid, "IVF-PQR search: the id -> position map is not built");
+        DFX_REQUIRE(rflat || idx->inv_valid, "IVF-PQR search: the id -> position map is not built");
         idx->w_rD.reserve((size_t)QC * k * 4);
         idx->w_rI.reserve((size_t)QC * k * 8);
         idx->w_rcomp.reserve((size_t)QC * k * 8);
@@ -961,7 +976,7 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
         const int64_t qc = (nq - q0 < QC) ? (nq - q0) : QC;
         const float* xq = d_x + q0 * d;
         int32_t* keys = keys_all + q0 * nprobe;
-        // where the scan's selection writes: the result rows, or (IVF-PQR) the first-stage rows
+        // where the scan's selection writes: the result rows, or (refinements) the first-stage rows
         float* outD = refine ? idx->w_rD.as<float>() : d_D + q0 * k;
         int64_t* outI = refine ? idx->w_rI.as<int64_t>() : d_I + q0 * k;
         // K1: coarse quantizer -- tensor cores (screen) + canonical fp32 (decide), or plain FFMA
@@ -1108,7 +1123,7 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
             // P >= 2048 = sort_cap: a row of up to sort_cap candidates is sorted whole
             const int P = dfx_next_pow2(k);
             ResultWriter wr{outD, outI, k, smetric, nullptr};
-            if ((size_t)P * 8 > 48 * 1024)  // IVF-PQR's k' > 4096: opt in to more shared memory
+            if ((size_t)P * 8 > 48 * 1024)  // a refinement's k' > 4096: opt in to more shared memory
                 DFX_CUDA(cudaFuncSetAttribute(select_cand_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                               P * 8));
             DFX_LAUNCH(select_cand_kernel<256>, (unsigned)qc, 256, (size_t)P * 8, st, part, coff, nprobe, wr, k, P,
@@ -1118,10 +1133,10 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
             ResultWriter wr{outD, outI, k, smetric, nullptr};
             dfx_launch_select<128>(ldr, wr, qc, ngroups * k, k, st);
         }
-        if (kind == DFX_IVF_PQ_FS)
+        if (kind == DFX_IVF_PQ_FS && !rflat)  // the flat refinement reads the first stage's ids only
             DFX_LAUNCH(fs_dequant_kernel, (unsigned)dfx_ceil_div(qc * k, 256), 256, 0, st, outD, outI,
                        qc * k, k, idx->w_dis0.as<float2>());
-        if (refine) pqr_refine(idx, xq, qc, k, kout, outI, d_D + q0 * kout, d_I + q0 * kout, st);
+        if (refine) refine_candidates(idx, xq, qc, k, kout, outI, d_D + q0 * kout, d_I + q0 * kout, st);
     }
     idx->last_nq = nq;
     idx->last_nprobe = nprobe;

@@ -43,7 +43,8 @@ EXPORTED_SYMBOLS = [
 
 class DfxCfg(C.Structure):
     _fields_ = [("kind", C.c_int32), ("metric", C.c_int32), ("d", C.c_int32), ("pq_m", C.c_int32),
-                ("pq_nbits", C.c_int32), ("device", C.c_int32), ("nlist", C.c_int64), ("refine_m", C.c_int32)]
+                ("pq_nbits", C.c_int32), ("device", C.c_int32), ("nlist", C.c_int64), ("refine_m", C.c_int32),
+                ("refine_flat", C.c_int32)]
 
 
 class DfxSynth(C.Structure):
@@ -113,7 +114,8 @@ class _Quantizer:
 class GpuIndex:
     """One shard resident in the HBM of one H100, behind the faiss-object surface."""
 
-    def __init__(self, kind, d, metric=METRIC_INNER_PRODUCT, nlist=0, pq_m=0, pq_nbits=8, device=None, refine_m=0):
+    def __init__(self, kind, d, metric=METRIC_INNER_PRODUCT, nlist=0, pq_m=0, pq_nbits=8, device=None, refine_m=0,
+                 refine_flat=False):
         import torch  # device bookkeeping only
 
         if device is None:
@@ -121,7 +123,7 @@ class GpuIndex:
         self.kind, self.d, self.metric = int(kind), int(d), int(metric)
         self.device = int(device)
         self._cfg = DfxCfg(self.kind, self.metric, self.d, int(pq_m), int(pq_nbits), self.device, int(nlist),
-                           int(refine_m))
+                           int(refine_m), 1 if refine_flat else 0)
         self._h = C.c_void_p()
         _check(lib().dfx_create(C.byref(self._cfg), C.byref(self._h)))
         if self.kind != KIND_FLAT:
@@ -130,6 +132,8 @@ class GpuIndex:
         self.pq_nbits = int(pq_nbits)
         self.ksub = 1 << self.pq_nbits if self.kind in (KIND_IVF_PQ, KIND_IVF_PQ_FS, KIND_IVF_PQR) else 0
         self.refine_m = int(refine_m)  # IVF-PQR: M2, the bytes of the refinement code
+        # flat refinement (",RFlat"): the raw fp32 rows kept by id, k * k_factor candidates re-ranked exactly
+        self.refine_flat = bool(refine_flat)
 
     def __del__(self):
         h = getattr(self, "_h", None)
@@ -275,7 +279,7 @@ class GpuIndex:
     _DTYPES = {"centroids": np.float32, "codebooks": np.float32, "list_off": np.int64, "ids": np.int64,
                "codes": np.uint8, "tvals": np.float32, "vecs": np.float32, "codes16": np.uint16,
                "xb": np.float32, "sq_trained": np.float32, "codes8": np.uint8, "refine_codebooks": np.float32,
-               "refine_codes": np.uint8}
+               "refine_codes": np.uint8, "refine_vecs": np.float32}
 
     def get_array(self, name):
         nb = C.c_int64(0)
@@ -326,6 +330,10 @@ class GpuIndex:
         if self.kind == KIND_IVF_SQ8:
             st["sq_trained"] = self.get_array("sq_trained").reshape(2, d)
             st["codes8"] = self.get_array("codes8").reshape(-1, d)
+        if self.refine_flat:  # the raw rows, in id order
+            st["refine_flat"] = 1
+            st["refine_vecs"] = self.get_array("refine_vecs").reshape(-1, d)
+            st["k_factor"] = self.get_param("k_factor")
         return st
 
     def set_state(self, st):
@@ -344,8 +352,10 @@ class GpuIndex:
             self.set_array(self.payload_name(), st[self.payload_name()])
             if self.kind == KIND_IVF_PQR:
                 self.set_array("refine_codes", st["refine_codes"])
-                if "k_factor" in st:
-                    self.set_param("k_factor", float(st["k_factor"]))
+            if self.refine_flat:
+                self.set_array("refine_vecs", st["refine_vecs"])
+            if (self.kind == KIND_IVF_PQR or self.refine_flat) and "k_factor" in st:
+                self.set_param("k_factor", float(st["k_factor"]))
         _check(lib().dfx_import_done(self._h))
 
 

@@ -23,8 +23,15 @@ Tokens are case-sensitive, as in faiss:
                                               the k * k_factor best IVF-PQ candidates on the finer
                                               reconstruction; L2 only; M and M2 each a multiple of 4, at
                                               most 128, that divides d)
-Everything else (OPQ / PCA prefixes, HNSW, IVF{n}_HNSW quantizers, RFlat / Refine, IDMap, PQ{M}x4,
-PQ{M}x4fsr, a FastScan block size suffix "_{bbs}", SQ4 / SQ6, malformed n or M) raises RuntimeError.
+  "IVF{n},<codec>,RFlat"          -> the codec's kind with a flat refinement (IndexRefineFlat over the IVF
+                                              index): <codec> is PQ{M}, PQ{M}x8, PQ{M}x4fs, SQ8 or SQfp16 with
+                                              the limits above; the raw fp32 vectors are kept next to the
+                                              lists and a search re-ranks the k * k_factor best candidates
+                                              (k_factor 1 by default, as in faiss) on their exact distances;
+                                              L2 only
+Everything else (OPQ / PCA prefixes, HNSW, IVF{n}_HNSW quantizers, RFlat after Flat, IVF{n},Flat or
+PQ{M}+{M2}, every Refine(...) spelling, IDMap, PQ{M}x4, PQ{M}x4fsr, a FastScan block size suffix "_{bbs}",
+SQ4 / SQ6, malformed n or M) raises RuntimeError.
 """
 import re
 from typing import NamedTuple
@@ -32,9 +39,10 @@ from typing import NamedTuple
 METRIC_INNER_PRODUCT, METRIC_L2 = 0, 1  # faiss enum values
 
 ACCEPTED_FORMS = ("Flat", "IVF{n},Flat", "IVF{n},PQ{M}", "IVF{n},PQ{M}x8", "IVF{n},PQ{M}x4fs", "IVF{n},PQ{M}+{M2}",
-                  "IVF{n},SQfp16", "IVF{n},SQ8")
+                  "IVF{n},SQfp16", "IVF{n},SQ8", "IVF{n},PQ{M},RFlat", "IVF{n},PQ{M}x8,RFlat", "IVF{n},PQ{M}x4fs,RFlat",
+                  "IVF{n},SQfp16,RFlat", "IVF{n},SQ8,RFlat")
 
-_IVF = re.compile(r"IVF([1-9][0-9]*),(Flat|PQ([1-9][0-9]*)(x8|x4fs|\+([1-9][0-9]*))?|SQfp16|SQ8)")
+_IVF = re.compile(r"IVF([1-9][0-9]*),(Flat|PQ([1-9][0-9]*)(x8|x4fs|\+([1-9][0-9]*))?|SQfp16|SQ8)(,RFlat)?")
 # one query's fp32 PQ distance table (M x 256 x 4 bytes) must fit in one thread block's shared memory
 # (128 KB at M = 128); more would need split or fp16 tables, which are not bit-exact
 _PQ_M_MAX = 128
@@ -43,12 +51,14 @@ _PQ_M_MAX = 128
 class FactorySpec(NamedTuple):
     """kind: a name of engine.KIND_NAMES ("flat", "ivf_flat", "ivf_pq", "ivf_sq", "ivf_sq8", "ivf_pq_fs",
     "ivf_pqr").  metric: flat / ivf_flat: the search metric; the codecs: the coarse quantizer's metric
-    (their search is L2).  refine_m: ivf_pqr's M2 (bytes of the refinement code), else 0."""
+    (their search is L2).  refine_m: ivf_pqr's M2 (bytes of the refinement code), else 0.
+    refine_flat: the string ends in ",RFlat" (exact re-ranking on stored fp32 vectors)."""
     kind: str
     metric: int
     nlist: int = 0
     pq_m: int = 0
     refine_m: int = 0
+    refine_flat: bool = False
 
 
 def substitute_centroids(factory_string: str, centroids: int) -> str:
@@ -66,7 +76,9 @@ def parse_factory(dim: int, factory_string: str, metric: int) -> FactorySpec:
     if s == "Flat":
         return FactorySpec("flat", int(metric))
     m = _IVF.fullmatch(s)
-    if m is None:
+    # re-ranking an exact index is a no-op, and IVF-PQR has its own refinement: RFlat follows a codec only
+    rflat = m is not None and m.group(6) is not None
+    if m is None or (rflat and (m.group(2) == "Flat" or m.group(5) is not None)):
         raise RuntimeError(
             f"faiss_factory {factory_string!r} is not supported by the GPU search path; accepted forms: "
             + ", ".join(ACCEPTED_FORMS) + " (n: number of lists, M: PQ sub-quantizers; case-sensitive)")
@@ -84,7 +96,7 @@ def parse_factory(dim: int, factory_string: str, metric: int) -> FactorySpec:
             raise RuntimeError(
                 f"faiss_factory {factory_string!r}: the number of FastScan sub-quantizers must be a multiple of 8 "
                 f"in [8, {_PQ_M_MAX}] that divides d={dim} (a row of 4-bit codes is whole 32-bit words)")
-        return FactorySpec("ivf_pq_fs", int(metric), nlist, M)
+        return FactorySpec("ivf_pq_fs", int(metric), nlist, M, 0, rflat)
     if codec.startswith("PQ") and m.group(5) is not None:
         M, M2 = int(m.group(3)), int(m.group(5))
         for name, v in (("PQ", M), ("refinement PQ", M2)):
@@ -101,5 +113,5 @@ def parse_factory(dim: int, factory_string: str, metric: int) -> FactorySpec:
             raise RuntimeError(
                 f"faiss_factory {factory_string!r}: the number of PQ sub-quantizers must be a multiple of 4, "
                 f"at most {_PQ_M_MAX}, that divides d={dim}{why}")
-        return FactorySpec("ivf_pq", int(metric), nlist, M)
-    return FactorySpec("ivf_sq" if codec == "SQfp16" else "ivf_sq8", int(metric), nlist)
+        return FactorySpec("ivf_pq", int(metric), nlist, M, 0, rflat)
+    return FactorySpec("ivf_sq" if codec == "SQfp16" else "ivf_sq8", int(metric), nlist, 0, 0, rflat)

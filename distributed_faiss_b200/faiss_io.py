@@ -15,7 +15,8 @@ itself is not available in this environment (SURVEY.md section 8c), so the forma
 self-consistency only (tests/test_faiss_io.py), never against a file written by faiss.  The same
 holds for the 4-bit IndexIVFPQ codes [faiss-upstream], restated from faiss's PQEncoderGeneric.
 IndexIVFPQFastScan ("IwPf", the factory string "IVF{n},PQ{M}x4fs") is neither read nor written: its
-block-interleaved code layout could not be checked without faiss; such shards use the npz format.
+block-interleaved code layout could not be checked without faiss; such shards use the npz format,
+with or without a flat refinement.
 
 Layout (little endian, no padding; `vec<T>` = u64 count + raw elements):
   header   : i32 d, i64 ntotal, i64 1<<20, i64 1<<20, u8 is_trained, i32 metric (0 IP, 1 L2)
@@ -37,6 +38,9 @@ Layout (little endian, no padding; `vec<T>` = u64 count + raw elements):
              qtype 4 (fp16): trained empty, code = d little-endian fp16 of the residual
              qtype 0 (8bit): rangestat 0 (min-max), trained = [vmin (d), vdiff (d)],
                              code = d bytes of the residual
+  RefineFlat: "IxRF", header, the base index (IVFPQ with 8-bit codes or IVFSQ, as above), the refine
+             index (a flat "IxF2" index holding the raw rows in id order), f32 k_factor
+             [faiss-upstream: IndexRefineFlat, index_write.cpp]
 """
 import struct
 from typing import BinaryIO, Dict, Tuple
@@ -228,6 +232,16 @@ def write_index(state: Dict, path: str, nprobe: int = 1) -> None:
     """state: engine / oracle `get_state()` dict.  Writes a faiss index file."""
     kind = state["kind"]
     with open(path, "wb") as f:
+        if state.get("refine_flat"):
+            # IndexRefineFlat around the base index; the base's own refusals (FastScan) apply below
+            if kind not in ("ivf_pq", "ivf_pq_fs", "ivf_sq", "ivf_sq8") or (kind == "ivf_pq" and int(state["ksub"]) != 256):
+                raise FaissFormatError(f"IndexRefineFlat over an index of kind {kind!r} is not served")
+            vecs = np.ascontiguousarray(state["refine_vecs"], dtype=np.float32).reshape(-1, int(state["d"]))
+            if len(vecs) != len(state["ids"]):
+                raise FaissFormatError("IndexRefineFlat: the refine index does not hold ntotal vectors")
+            if kind != "ivf_pq_fs":
+                f.write(b"IxRF")
+                _wheader(f, state["d"], len(state["ids"]), METRIC_L2)
         if kind == "flat":
             _write_flat(f, state["xb"], int(state["metric"]))
         elif kind == "ivf_flat":
@@ -284,74 +298,98 @@ def write_index(state: Dict, path: str, nprobe: int = 1) -> None:
             _write_invlists(f, state["list_off"], state["ids"], np.ascontiguousarray(state["codes8"], np.uint8), d)
         else:
             raise FaissFormatError(f"unknown index kind {kind!r}")
+        if state.get("refine_flat"):
+            _write_flat(f, vecs, METRIC_L2)
+            _w(f, "f", float(state.get("k_factor", 1.0)))
 
 
 def read_index(path: str) -> Tuple[Dict, int]:
     """Returns (state dict for `set_state`, nprobe stored in the file)."""
     with open(path, "rb") as f:
         cc = _fourcc(f)
-        if cc in ("IxFI", "IxF2", "IxFl"):
-            st = _read_flat_body(f, cc)
-            return st, 1
-        if cc not in ("IwFl", "IwPQ", "IwQR", "IwSq"):
-            raise FaissFormatError(
-                f"faiss index type {cc!r} is not one of the types the GPU search path serves "
-                "(IndexFlat, IndexIVFFlat, IndexIVFPQ, IndexIVFPQR, IndexIVFScalarQuantizer fp16 / 8bit)")
-        d, ntotal, metric, nlist, nprobe, cent, cmetric = _read_ivf_header(f)
-        st = {"d": d, "nlist": nlist, "centroids": cent}
-        if cc == "IwFl":
+        if cc == "IxRF":
+            d, ntotal, _, metric = _rheader(f)
+            st, nprobe = _read_one(f, _fourcc(f))
+            four_bit = st["kind"] == "ivf_pq" and st["ksub"] != 256
+            if st["kind"] not in ("ivf_pq", "ivf_sq", "ivf_sq8") or four_bit or metric != METRIC_L2:
+                raise FaissFormatError(f"IndexRefineFlat over an index of kind {st['kind']!r}"
+                                       f"{' with 4-bit codes' if four_bit else ''} (metric {metric}) is not served")
+            rcc = _fourcc(f)
+            if rcc not in ("IxF2", "IxFl"):
+                raise FaissFormatError(f"IndexRefineFlat: the refine index {rcc!r} is not a flat L2 index")
+            flat = _read_flat_body(f, rcc)
+            (k_factor,) = _r(f, "f")
+            if flat["d"] != d or st["d"] != d or flat["xb"].shape[0] != ntotal or len(st["ids"]) != ntotal:
+                raise FaissFormatError("IndexRefineFlat: the refine index does not hold the base index's vectors")
+            st.update(refine_flat=1, refine_vecs=flat["xb"], k_factor=float(k_factor))
+            return st, nprobe
+        return _read_one(f, cc)
+
+
+def _read_one(f: BinaryIO, cc: str) -> Tuple[Dict, int]:
+    """one index whose fourcc `cc` has been read"""
+    if cc in ("IxFI", "IxF2", "IxFl"):
+        st = _read_flat_body(f, cc)
+        return st, 1
+    if cc not in ("IwFl", "IwPQ", "IwQR", "IwSq"):
+        raise FaissFormatError(
+            f"faiss index type {cc!r} is not one of the types the GPU search path serves "
+            "(IndexFlat, IndexIVFFlat, IndexIVFPQ, IndexIVFPQR, IndexIVFScalarQuantizer fp16 / 8bit)")
+    d, ntotal, metric, nlist, nprobe, cent, cmetric = _read_ivf_header(f)
+    st = {"d": d, "nlist": nlist, "centroids": cent}
+    if cc == "IwFl":
+        list_off, ids, rows, cs = _read_invlists(f, nlist)
+        if cs != 4 * d:
+            raise FaissFormatError("IndexIVFFlat code size is not 4 * d")
+        st.update(kind="ivf_flat", metric=metric, vecs=rows.view(np.float32).reshape(-1, d))
+    elif cc in ("IwPQ", "IwQR"):
+        (by_res,) = _r(f, "B")
+        (code_size,) = _r(f, "Q")
+        pd, M, nbits = _r(f, "QQQ")
+        cb = _rvec(f, np.float32)
+        if not by_res or nbits not in (8, 4) or pd != d or code_size != (M * nbits + 7) // 8:
+            raise FaissFormatError("IndexIVFPQ: only by_residual with 8 or 4 bits per sub-quantizer is "
+                                   f"supported (nbits={nbits}, M={M}, code_size={code_size})")
+        if metric != METRIC_L2:
+            raise FaissFormatError("IndexIVFPQ: only METRIC_L2 is supported")
+        list_off, ids, rows, cs = _read_invlists(f, nlist)
+        if cs != code_size:
+            raise FaissFormatError("IndexIVFPQ: inverted lists / header code_size mismatch")
+        ksub = 1 << nbits
+        st.update(kind="ivf_pq", coarse_metric=cmetric, M=M, ksub=ksub,
+                  codebooks=cb.reshape(M, ksub, d // M), codes=_unpack_pq_codes(rows, M, nbits))
+        if cc == "IwQR":
+            rd, M2, nbits2 = _r(f, "QQQ")
+            rcb = _rvec(f, np.float32)
+            rcodes = _rvec(f, np.uint8)
+            (k_factor,) = _r(f, "f")
+            if nbits != 8 or nbits2 != 8 or rd != d or M2 == 0 or d % M2 != 0 or rcb.size != M2 * 256 * (d // M2):
+                raise FaissFormatError(f"IndexIVFPQR: only 8-bit codes in both product quantizers are supported "
+                                       f"(nbits={nbits}, refine nbits={nbits2}, M2={M2}, d={d})")
+            if rcodes.size != ntotal * M2:
+                raise FaissFormatError("IndexIVFPQR: the refine codes do not hold ntotal vectors")
+            st.update(kind="ivf_pqr", M2=int(M2), refine_codebooks=rcb.reshape(M2, 256, d // M2),
+                      refine_codes=rcodes.reshape(ntotal, M2), k_factor=float(k_factor))
+    else:
+        qtype, rangestat, _ = _r(f, "iif")
+        sd, scs = _r(f, "QQ")
+        trained = _rvec(f, np.float32)
+        (code_size,) = _r(f, "Q")
+        (by_res,) = _r(f, "B")
+        if qtype == QT_8BIT:
+            if not by_res or code_size != d or trained.size != 2 * d:
+                raise FaissFormatError("IndexIVFScalarQuantizer QT_8bit: only by_residual with d codes "
+                                       "and a [vmin, vdiff] trained vector is supported")
             list_off, ids, rows, cs = _read_invlists(f, nlist)
-            if cs != 4 * d:
-                raise FaissFormatError("IndexIVFFlat code size is not 4 * d")
-            st.update(kind="ivf_flat", metric=metric, vecs=rows.view(np.float32).reshape(-1, d))
-        elif cc in ("IwPQ", "IwQR"):
-            (by_res,) = _r(f, "B")
-            (code_size,) = _r(f, "Q")
-            pd, M, nbits = _r(f, "QQQ")
-            cb = _rvec(f, np.float32)
-            if not by_res or nbits not in (8, 4) or pd != d or code_size != (M * nbits + 7) // 8:
-                raise FaissFormatError("IndexIVFPQ: only by_residual with 8 or 4 bits per sub-quantizer is "
-                                       f"supported (nbits={nbits}, M={M}, code_size={code_size})")
-            if metric != METRIC_L2:
-                raise FaissFormatError("IndexIVFPQ: only METRIC_L2 is supported")
-            list_off, ids, rows, cs = _read_invlists(f, nlist)
-            if cs != code_size:
-                raise FaissFormatError("IndexIVFPQ: inverted lists / header code_size mismatch")
-            ksub = 1 << nbits
-            st.update(kind="ivf_pq", coarse_metric=cmetric, M=M, ksub=ksub,
-                      codebooks=cb.reshape(M, ksub, d // M), codes=_unpack_pq_codes(rows, M, nbits))
-            if cc == "IwQR":
-                rd, M2, nbits2 = _r(f, "QQQ")
-                rcb = _rvec(f, np.float32)
-                rcodes = _rvec(f, np.uint8)
-                (k_factor,) = _r(f, "f")
-                if nbits != 8 or nbits2 != 8 or rd != d or M2 == 0 or d % M2 != 0 or rcb.size != M2 * 256 * (d // M2):
-                    raise FaissFormatError(f"IndexIVFPQR: only 8-bit codes in both product quantizers are supported "
-                                           f"(nbits={nbits}, refine nbits={nbits2}, M2={M2}, d={d})")
-                if rcodes.size != ntotal * M2:
-                    raise FaissFormatError("IndexIVFPQR: the refine codes do not hold ntotal vectors")
-                st.update(kind="ivf_pqr", M2=int(M2), refine_codebooks=rcb.reshape(M2, 256, d // M2),
-                          refine_codes=rcodes.reshape(ntotal, M2), k_factor=float(k_factor))
+            st.update(kind="ivf_sq8", coarse_metric=cmetric, sq_trained=trained.reshape(2, d),
+                      codes8=rows.reshape(-1, d))
         else:
-            qtype, rangestat, _ = _r(f, "iif")
-            sd, scs = _r(f, "QQ")
-            trained = _rvec(f, np.float32)
-            (code_size,) = _r(f, "Q")
-            (by_res,) = _r(f, "B")
-            if qtype == QT_8BIT:
-                if not by_res or code_size != d or trained.size != 2 * d:
-                    raise FaissFormatError("IndexIVFScalarQuantizer QT_8bit: only by_residual with d codes "
-                                           "and a [vmin, vdiff] trained vector is supported")
-                list_off, ids, rows, cs = _read_invlists(f, nlist)
-                st.update(kind="ivf_sq8", coarse_metric=cmetric, sq_trained=trained.reshape(2, d),
-                          codes8=rows.reshape(-1, d))
-            else:
-                if qtype != QT_FP16 or not by_res or code_size != 2 * d:
-                    raise FaissFormatError("IndexIVFScalarQuantizer: only QT_fp16 and QT_8bit, by_residual, "
-                                           "are supported")
-                list_off, ids, rows, cs = _read_invlists(f, nlist)
-                st.update(kind="ivf_sq", coarse_metric=cmetric, codes16=rows.view("<u2").reshape(-1, d))
-        if len(ids) != ntotal:
-            raise FaissFormatError("inverted lists do not hold ntotal vectors")
-        st.update(list_off=list_off, ids=ids)
-        return st, int(nprobe)
+            if qtype != QT_FP16 or not by_res or code_size != 2 * d:
+                raise FaissFormatError("IndexIVFScalarQuantizer: only QT_fp16 and QT_8bit, by_residual, "
+                                       "are supported")
+            list_off, ids, rows, cs = _read_invlists(f, nlist)
+            st.update(kind="ivf_sq", coarse_metric=cmetric, codes16=rows.view("<u2").reshape(-1, d))
+    if len(ids) != ntotal:
+        raise FaissFormatError("inverted lists do not hold ntotal vectors")
+    st.update(list_off=list_off, ids=ids)
+    return st, int(nprobe)

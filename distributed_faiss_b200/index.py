@@ -23,10 +23,13 @@ Builders (reference index.py:93-100):
 Factory strings are parsed by factory.parse_factory ("Flat", "IVF{n},Flat", "IVF{n},PQ{M}[x8]",
 "IVF{n},PQ{M}x4fs" (FastScan: 4-bit codes of the raw vectors, 8-bit quantized distance tables),
 "IVF{n},PQ{M}+{M2}" (IndexIVFPQR: IVF-PQ candidates re-ranked on a second, M2-byte residual code),
-"IVF{n},SQfp16", "IVF{n},SQ8"); any other string raises, and so does "hnswsq" (a graph index,
-outside the hot path this package rebuilds, SURVEY.md section 8).  A stored shard is only loaded
-under a cfg that builds the same kind (and, for the PQ kinds, the same (M, ksub), and for
-IVF-PQR the same M2).
+"IVF{n},SQfp16", "IVF{n},SQ8", and each codec form but PQ{M}+{M2} followed by ",RFlat" (IndexRefineFlat:
+the raw fp32 vectors are kept by id next to the lists, a search re-ranks the k * k_factor best
+candidates on their exact L2 distances, and `return_embeddings` gives the stored vectors; k_factor is
+1 unless the cfg carries `k_factor=...`)); any other string raises, and so does "hnswsq" (a graph
+index, outside the hot path this package rebuilds, SURVEY.md section 8).  A stored shard is only
+loaded under a cfg that builds the same kind with the same refinement (and, for the PQ kinds, the
+same (M, ksub), and for IVF-PQR the same M2).
 """
 import _thread
 import logging
@@ -82,7 +85,9 @@ def default_engine_factory(cfg: IndexCfg, device: Optional[int] = None):
         kind = {name: k for k, name in engine.KIND_NAMES.items()}[spec.kind]
         nbits = 4 if spec.kind == "ivf_pq_fs" else 8  # FastScan: 4-bit codes
         idx = engine.GpuIndex(kind, cfg.dim, spec.metric, nlist=spec.nlist, pq_m=spec.pq_m, pq_nbits=nbits,
-                              device=device, refine_m=spec.refine_m)
+                              device=device, refine_m=spec.refine_m, refine_flat=spec.refine_flat)
+        if spec.refine_flat and "k_factor" in cfg.extra:
+            idx.set_param("k_factor", float(cfg.extra["k_factor"]))
         if cfg.index_builder_type == "ivf_gpu":
             idx.nprobe = cfg.nprobe  # index.py:84
         # the factory path keeps faiss's default nprobe (1) and leaves cfg.nprobe alone, unlike
@@ -563,10 +568,13 @@ class Index:
         engine = result._engine_factory(build_cfg)
         cfg.nprobe = saved_nprobe
         want = _kind_name(engine)
-        if state.get("kind") != want:
-            # e.g. an SQfp16 file under a cfg that builds IVF-SQ8: never reinterpret the codes
-            raise RuntimeError(f"the stored index is of kind {state.get('kind')!r} but the cfg builds "
-                               f"{want!r}; refusing to load it")
+        stored_rf, built_rf = bool(state.get("refine_flat", 0)), bool(getattr(engine, "refine_flat", False))
+        if state.get("kind") != want or stored_rf != built_rf:
+            # e.g. an SQfp16 file under a cfg that builds IVF-SQ8: never reinterpret the codes; and a
+            # shard with a flat refinement is not one without (its answers and its stored rows differ)
+            rf = {True: " with a flat refinement (RFlat)", False: ""}
+            raise RuntimeError(f"the stored index is of kind {state.get('kind')!r}{rf[stored_rf]} but the cfg builds "
+                               f"{want!r}{rf[built_rf]}; refusing to load it")
         if want in ("ivf_pq", "ivf_pq_fs"):
             # e.g. 4-bit codes under a cfg that builds 8-bit ones: the codebooks would not fit either
             stored = (int(state["M"]), int(state["ksub"]))
@@ -583,6 +591,8 @@ class Index:
                 raise RuntimeError(f"the stored IVF-PQR index has (M, ksub, M2) = {stored} but the cfg builds "
                                    f"{built}; refusing to load it")
         engine.set_state(state)
+        if built_rf and "k_factor" in cfg.extra:  # the caller's cfg wins over the stored value
+            engine.set_param("k_factor", float(cfg.extra["k_factor"]))
         assert len(meta) >= engine.ntotal, "Deserialized meta list should be at least of index size"
         result.faiss_index = engine
         result.state = IndexState.TRAINED

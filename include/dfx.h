@@ -75,6 +75,13 @@ typedef struct dfx_cfg {
     int64_t nlist;    /* IVF_*: number of inverted lists (cfg.centroids); IVF kinds need d % 4 == 0 */
     int32_t refine_m; /* IVF_PQR: sub-quantizers of the refinement PQ (M2; 8 bits each): 4 <= M2 <= 128,
                          M2 % 4 == 0, d % M2 == 0.  Must be 0 for every other kind */
+    int32_t refine_flat; /* non-zero: flat refinement (faiss IndexRefineFlat, the ",RFlat" suffix of a
+                         factory string) on top of IVF_PQ with 8-bit codes, IVF_PQ_FS, IVF_SQ8 or IVF_SQ16:
+                         the raw fp32 rows are kept by id next to the lists ("refine_vecs", 4 d bytes per
+                         vector), a search runs the base kind's search for k' = k * k_factor candidates
+                         and re-ranks them on their exact L2 distances, and a reconstruction returns
+                         the stored row.  The metric must be L2.  Must be 0 for FLAT, IVF_FLAT, IVF_PQR
+                         and IVF_PQ with 4-bit codes */
 } dfx_cfg;
 
 /* ---- lifetime: replaces the faiss constructors at index.py:25-48,63-68,94 ---- */
@@ -104,10 +111,11 @@ int dfx_add_dev(dfx_index *idx, int64_t n, const float *d_x, void *stream);
  *   that scan (tuning; 512 threads at k > 512 do not fit in shared memory and run with 256);
  * "rows_inflight" (0 = by row size): 4 or 8 vectors per warp in flight in the IVF-Flat / IVF-SQ
  *   list scan;
- * "k_factor" (4, IVF_PQR only; this knob DOES change results): a search for k results re-ranks the
- *   k' = (int64)((float)k * k_factor) best candidates of the IVF-PQ stage, as faiss's
- *   IndexIVFPQR::k_factor; values below 1 are refused, and a search whose k' exceeds 16384 raises
- *   before launching anything */
+ * "k_factor" (IVF_PQR: 4; refine_flat: 1 -- the faiss defaults of IndexIVFPQR and IndexRefine; no
+ *   other index has it; this knob DOES change results): a search for k results re-ranks the
+ *   k' = (int64)((float)k * k_factor) best candidates of the first stage, as faiss's k_factor;
+ *   values outside [1, 16384] are refused, and a search whose k' exceeds 16384 raises before
+ *   launching anything */
 int dfx_set_param(dfx_index *idx, const char *name, double value);
 /* read back a knob or a counter: the names of dfx_set_param, plus "tc_fast" (the precision the
  * next screening launch will use: 1 = FAST), "tc_stat_rows" / "tc_stat_overflow" /
@@ -115,7 +123,7 @@ int dfx_set_param(dfx_index *idx, const char *name, double value);
  * launch whose statistics came back; synchronises with that launch), "workspace_bytes" (bytes of
  * the partial-result workspace, the largest any search so far has needed, including the candidate
  * rows of IVF searches with k > 1024; IVF searches keep it within 128 MiB by their query chunk),
- * "refine_ms" / "refine_launches" (IVF_PQR with profiling on: summed device time and number of
+ * "refine_ms" / "refine_launches" (IVF_PQR / refine_flat with profiling on: summed device time and number of
  * the refinement stages -- re-rank kernel and final selection -- since the last reset of
  * dfx_profile_read; synchronises) */
 int dfx_get_param(dfx_index *idx, const char *name, double *value);
@@ -129,12 +137,14 @@ int dfx_finalize(dfx_index *idx, void *stream);
  * writes every probed vector's candidate and selects per query; it raises an error before launching
  * anything when the nprobe longest lists together exceed 2^24 vectors (128 MiB of candidates).
  * IVF_PQR: the IVF-PQ stage runs at k' = k * k_factor (at most 16384; k' > 1024 takes the candidate
- * rows), and the k' candidates are re-ranked and selected down to k. */
+ * rows), and the k' candidates are re-ranked and selected down to k; the same holds for the base
+ * kind's stage of an index with refine_flat. */
 int dfx_search(dfx_index *idx, int64_t nq, const float *x, int64_t k, float *D, int64_t *I);
 int dfx_search_dev(dfx_index *idx, int64_t nq, const float *d_x, int64_t k, float *d_D,
                    int64_t *d_I, void *stream);
 
-/* faiss_index.search_and_reconstruct: decode rows by id (index.py:255); id -1 -> NaN row */
+/* faiss_index.search_and_reconstruct: decode rows by id (index.py:255); id -1 -> NaN row
+ * (refine_flat: the stored fp32 row, as faiss reconstructs from the refine index) */
 int dfx_reconstruct(dfx_index *idx, int64_t n, const int64_t *ids, float *out);
 
 /* device form, for winners that travelled through the all-gather + merge (client.py:287-289,
@@ -211,6 +221,8 @@ int dfx_map_ids_dev(int64_t n, const int64_t *d_ids, const int64_t *d_table, int
  *   (IVF_PQR: the IVF_PQ arrays with 8-bit codes, plus "refine_codebooks" f32[M2,256,d/M2] and
  *   "refine_codes" u8[ntotal,M2] in ID order, not list order; its "ids" must be a permutation of
  *   0 .. ntotal-1, and "tvals" is recomputed on import)
+ *   (refine_flat: the base kind's arrays, plus "refine_vecs" f32[ntotal,d] in ID order; "ids" must
+ *   be a permutation of 0 .. ntotal-1, and "refine_vecs" follows the payload on import)
  * dfx_get_array with out == NULL only reports the size.  Import order: centroids,
  * codebooks (IVF_PQ, IVF_PQ_FS, IVF_PQR) or sq_trained (IVF_SQ8), refine_codebooks (IVF_PQR), then
  * list_off, ids and the payload, refine_codes (IVF_PQR), then dfx_import_done(). */
@@ -221,7 +233,7 @@ int dfx_import_done(dfx_index *idx);
 
 /* statistics of the most recent search (device work, synchronises):
  * ndis = sum over (query, probed list) of the list length -- faiss's `ndis` (IVF_PQR: of the
- * IVF-PQ stage; the re-ranked candidates are not counted). */
+ * IVF-PQ stage, refine_flat: of the base kind's stage; the re-ranked candidates are not counted). */
 int dfx_last_stats(dfx_index *idx, int64_t *ndis, int64_t *nq, int64_t *nprobe);
 /* per-kernel timing of the dominant kernel (the inverted-list scan): when enabled, every scan
  * launch is bracketed by CUDA events on the launching stream; dfx_profile_read synchronises
