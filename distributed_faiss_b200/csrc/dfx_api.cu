@@ -191,14 +191,8 @@ void dfx_destroy(dfx_index* idx) {
             cudaStreamSynchronize(idx->stream);
             cudaStreamDestroy(idx->stream);
         }
-        for (auto& e : idx->prof_events) {
-            cudaEventDestroy(e.first);
-            cudaEventDestroy(e.second);
-        }
-        for (auto& e : idx->prof_refine_events) {
-            cudaEventDestroy(e.first);
-            cudaEventDestroy(e.second);
-        }
+        idx->prof_scan.destroy();
+        idx->prof_refine.destroy();
         if (idx->tc_stat_ev) cudaEventDestroy(idx->tc_stat_ev);
         if (idx->dev_done) cudaEventDestroy(idx->dev_done);
         if (idx->tc_stat_h) cudaFreeHost(idx->tc_stat_h);
@@ -257,18 +251,6 @@ int dfx_set_param(dfx_index* idx, const char* name, double value) {
     DFX_API_END
 }
 
-// summed device time of one list of bracketing events (synchronises)
-static double prof_sum_ms(std::vector<std::pair<cudaEvent_t, cudaEvent_t>>& ev, size_t used) {
-    double ms = 0;
-    for (size_t i = 0; i < used; i++) {
-        DFX_CUDA(cudaEventSynchronize(ev[i].second));
-        float t = 0;
-        DFX_CUDA(cudaEventElapsedTime(&t, ev[i].first, ev[i].second));
-        ms += t;
-    }
-    return ms;
-}
-
 int dfx_get_param(dfx_index* idx, const char* name, double* value) {
     DFX_API_BEGIN
     DFX_REQUIRE(idx && name && value, "null argument");
@@ -300,8 +282,7 @@ int dfx_get_param(dfx_index* idx, const char* name, double* value) {
         std::lock_guard<std::mutex> lk(idx->mu);
         DeviceGuard g(idx->cfg.device);
         idx->join_dev();
-        *value = n == "refine_launches" ? (double)idx->prof_refine_used
-                                        : prof_sum_ms(idx->prof_refine_events, idx->prof_refine_used);
+        *value = n == "refine_launches" ? (double)idx->prof_refine.used : idx->prof_refine.sum_ms();
     }
     else throw DfxError{"unknown parameter " + n};
     DFX_API_END
@@ -531,10 +512,13 @@ int dfx_profile_read(dfx_index* idx, double* scan_ms, int64_t* scan_launches, in
     std::lock_guard<std::mutex> lk(idx->mu);
     DeviceGuard g(idx->cfg.device);
     idx->join_dev();
-    const double ms = prof_sum_ms(idx->prof_events, idx->prof_used);
+    const double ms = idx->prof_scan.sum_ms();
     if (scan_ms) *scan_ms = ms;
-    if (scan_launches) *scan_launches = (int64_t)idx->prof_used;
-    if (reset) idx->prof_used = idx->prof_refine_used = 0;
+    if (scan_launches) *scan_launches = (int64_t)idx->prof_scan.used;
+    if (reset) {
+        idx->prof_scan.reset();
+        idx->prof_refine.reset();
+    }
     DFX_API_END
 }
 

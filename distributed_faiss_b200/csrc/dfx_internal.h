@@ -24,6 +24,40 @@ struct dfx_tc_table {
     float cmax2c = 0.f;   // max |c - m|^2
 };
 
+// Device time of one search stage (dfx_profile_enable): begin / end bracket its launches on a stream,
+// sum_ms adds up the ranges since the last reset.  Event pairs are created on first use, then reused.
+struct dfx_event_ranges {
+    std::vector<std::pair<cudaEvent_t, cudaEvent_t>> ev;
+    size_t used = 0;
+    void begin(cudaStream_t st) {
+        if (used == ev.size()) {
+            cudaEvent_t a, b;
+            DFX_CUDA(cudaEventCreate(&a));
+            DFX_CUDA(cudaEventCreate(&b));
+            ev.emplace_back(a, b);
+        }
+        DFX_CUDA(cudaEventRecord(ev[used++].first, st));
+    }
+    void end(cudaStream_t st) { DFX_CUDA(cudaEventRecord(ev[used - 1].second, st)); }
+    double sum_ms() {  // synchronises
+        double ms = 0;
+        for (size_t i = 0; i < used; i++) {
+            DFX_CUDA(cudaEventSynchronize(ev[i].second));
+            float t = 0;
+            DFX_CUDA(cudaEventElapsedTime(&t, ev[i].first, ev[i].second));
+            ms += t;
+        }
+        return ms;
+    }
+    void reset() { used = 0; }
+    void destroy() {
+        for (auto& e : ev) {
+            cudaEventDestroy(e.first);
+            cudaEventDestroy(e.second);
+        }
+    }
+};
+
 struct dfx_index {
     dfx_cfg cfg{};
     int M = 0, ksub = 0, dsub = 0;
@@ -101,12 +135,10 @@ struct dfx_index {
     // refine_cap / refine_rows, k_factor (default 1, faiss IndexRefine) and the workspace above
     DevBuf refine_vecs;
 
-    // scan-kernel profiling (dfx_profile_enable)
+    // profiling (dfx_profile_enable): each query chunk's table prep + list scan (dfx_profile_read),
+    // and the re-ranking stage of IVF_PQR and the flat refinement (dfx_get_param "refine_ms")
     bool prof_on = false;
-    std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_events;
-    size_t prof_used = 0;
-    std::vector<std::pair<cudaEvent_t, cudaEvent_t>> prof_refine_events;  // IVF_PQR re-ranking stage
-    size_t prof_refine_used = 0;
+    dfx_event_ranges prof_scan, prof_refine;
 
     // last-search bookkeeping
     int64_t last_nq = 0, last_nprobe = 0;

@@ -20,11 +20,14 @@
 //   K_rf rflat_refine     flat refinement (",RFlat"): re-ranks the k' candidates of the base kind's stage
 //                         on the stored fp32 rows (dfx_rflat_dev.cuh), then K_sel picks the k best
 //   K6   merge            cross-shard merge (float_maxheap_array_t semantics)
+// Driver (dfx_search_impl): search_flat, or plan_ivf once per search (every refusal, before any launch)
+// and per query chunk K1 -> launch_list_scan -> K_sel / select_cand -> fs_dequant -> refine_candidates.
 // Arithmetic orders are the canonical ones of oracle/dfx_oracle.c (bit-exact parity).
 #include "dfx_internal.h"
 #include "dfx_select.cuh"
 #include "dfx_topk.cuh"
 #include "dfx_ptx.cuh"
+#include <utility>
 
 // =====================================================================================
 // K1a: values GEMM (fp32 FFMA).  acc = fmaf(q[k], x[k], acc), k ascending.
@@ -209,48 +212,6 @@ void dfx_launch_select_comp(const uint64_t* comp, int64_t nrows, int n, int64_t 
 #include "dfx_scan_pq_fs_dev.cuh"
 #include "dfx_refine_dev.cuh"
 #include "dfx_rflat_dev.cuh"
-
-// scan_pq_fs_kernel<M, MAT> for the runtime M (a multiple of 8 in [8, 128], checked by dfx_create)
-template <bool MAT, int MT = 8>
-static void dfx_launch_scan_pq_fs(int M, unsigned grid, size_t smem, cudaStream_t st, const uint8_t* lutq,
-                                  const int32_t* keys, int nprobe, int G, int ngroups, const int64_t* list_off,
-                                  const uint8_t* codes, const int32_t* ids, int k, int cap, uint64_t* part,
-                                  const int64_t* coff) {
-    if constexpr (MT <= 128) {
-        if (M != MT) {
-            dfx_launch_scan_pq_fs<MAT, MT + 8>(M, grid, smem, st, lutq, keys, nprobe, G, ngroups, list_off, codes,
-                                               ids, k, cap, part, coff);
-            return;
-        }
-        auto kern = scan_pq_fs_kernel<MT, MAT>;
-        DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        DFX_LAUNCH(kern, grid, 128, smem, st, lutq, keys, nprobe, G, ngroups, list_off, codes, ids, k, cap, part,
-                   coff);
-    } else {
-        throw DfxError{"IVF-PQ FastScan: no list scan for M=" + std::to_string(M)};
-    }
-}
-
-// scan_pq4_kernel<M, MAT> for the runtime M (a multiple of 8 in [8, 128], checked by dfx_create)
-template <bool MAT, int MT = 8>
-static void dfx_launch_scan_pq4(int M, unsigned grid, size_t smem, cudaStream_t st, const float* lut,
-                                const float* dis0, const int32_t* keys, int nprobe, int G, int ngroups,
-                                const int64_t* list_off, const uint8_t* codes, const float* tvals,
-                                const int32_t* ids, int k, int cap, uint64_t* part, const int64_t* coff) {
-    if constexpr (MT <= 128) {
-        if (M != MT) {
-            dfx_launch_scan_pq4<MAT, MT + 8>(M, grid, smem, st, lut, dis0, keys, nprobe, G, ngroups, list_off, codes,
-                                             tvals, ids, k, cap, part, coff);
-            return;
-        }
-        auto kern = scan_pq4_kernel<MT, MAT>;
-        DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        DFX_LAUNCH(kern, grid, 128, smem, st, lut, dis0, keys, nprobe, G, ngroups, list_off, codes, tvals, ids, k,
-                   cap, part, coff);
-    } else {
-        throw DfxError{"IVF-PQ with 4-bit codes: no list scan for M=" + std::to_string(M)};
-    }
-}
 
 // =====================================================================================
 // K4: scan_pq.  one CTA = (query, group of G consecutive probes).  lane-per-vector:
@@ -751,22 +712,12 @@ select_cand_kernel(const uint64_t* __restrict__ cand, const int64_t* __restrict_
 // =====================================================================================
 // IVF-PQR and the flat refinement: re-rank the k1 = k' candidates of each query of a chunk (cand
 // [qc][k1], the ids the first stage selected) and select the k best into (D, I) -- the order and
-// the padding are those of every other kind.  Bracketed by the refine profiling events
+// the padding are those of every other kind.  Bracketed by the refine profiling range
 // (dfx_get_param "refine_ms").
 // =====================================================================================
 static void refine_candidates(dfx_index* idx, const float* xq, int64_t qc, int k1, int k, const int64_t* cand,
                               float* D, int64_t* I, cudaStream_t st) {
-    std::pair<cudaEvent_t, cudaEvent_t>* pev = nullptr;
-    if (idx->prof_on) {
-        if (idx->prof_refine_used == idx->prof_refine_events.size()) {
-            cudaEvent_t a, b;
-            DFX_CUDA(cudaEventCreate(&a));
-            DFX_CUDA(cudaEventCreate(&b));
-            idx->prof_refine_events.emplace_back(a, b);
-        }
-        pev = &idx->prof_refine_events[idx->prof_refine_used++];
-        DFX_CUDA(cudaEventRecord(pev->first, st));
-    }
+    if (idx->prof_on) idx->prof_refine.begin(st);
     const int64_t nc = qc * k1;
     uint64_t* comp = idx->w_rcomp.as<uint64_t>();
     if (idx->rflat()) {
@@ -788,7 +739,7 @@ static void refine_candidates(dfx_index* idx, const float* xq, int64_t qc, int k
     CompLoader ldr{comp, k1};
     ResultWriter wr{D, I, k, DFX_METRIC_L2, nullptr};
     dfx_launch_select<128>(ldr, wr, qc, k1, k, st);
-    if (pev) DFX_CUDA(cudaEventRecord(pev->second, st));
+    if (idx->prof_on) idx->prof_refine.end(st);
 }
 
 // =====================================================================================
@@ -805,117 +756,144 @@ static int choose_group(int64_t nq, int nprobe) {
     return (int)G;
 }
 
-void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, float* d_D,
-                     int64_t* d_I, cudaStream_t st) {
-    DFX_REQUIRE(idx->trained || idx->cfg.kind == DFX_FLAT, "index is not trained");
-    DFX_REQUIRE(k64 >= 1, "k must be >= 1");
-    if (nq <= 0) return;
-    if (idx->n_pending > 0) dfx_finalize_impl(idx, st);
+static void search_flat(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, float* d_D, int64_t* d_I,
+                        cudaStream_t st) {
+    DFX_REQUIRE(k64 <= 4096, "flat search supports k <= 4096");
     const int d = idx->cfg.d;
+    const int k = (int)k64;
+    const int64_t N = idx->n_sorted;
+    const int metric = idx->cfg.metric;
+    if (N == 0) {
+        ResultWriter wr{d_D, d_I, k, metric, nullptr};
+        CompLoader ldr{nullptr, 0};
+        dfx_launch_select<128>(ldr, wr, nq, 0, k, st);
+        return;
+    }
+    float* qnorm_tc = nullptr;
+    if (idx->flat_tc && idx->tc_enabled) {  // screening on tensor cores + exact re-rank
+        const int64_t ng = dfx_ceil_div(N, 128) * 4;
+        const int64_t QT = std::max<int64_t>(128, ((64ll << 20) / (ng * 4)) / 128 * 128);
+        bool handled = true;
+        for (int64_t q0 = 0; q0 < nq && handled; q0 += QT) {
+            const int64_t qc = std::min(QT, nq - q0);
+            const int ncand = dfx_tc_flat_candidates(idx, d_x + q0 * d, qc, k, st);
+            if (ncand == 0) {
+                handled = false;  // shape not covered (only possible on the first chunk)
+                break;
+            }
+            if (metric == DFX_METRIC_L2 && !qnorm_tc) {
+                idx->w_dis0.reserve((size_t)nq * 4);
+                qnorm_tc = idx->w_dis0.as<float>();
+                dfx_launch_row_norms(d_x, nq, d, qnorm_tc, st);
+            }
+            CompLoader ldr{idx->tc_cand.as<uint64_t>(), ncand};
+            ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, metric, qnorm_tc ? qnorm_tc + q0 : nullptr};
+            dfx_launch_select<128>(ldr, wr, qc, ncand, k, st);
+        }
+        if (handled) return;
+    }
+    const int64_t NT = 32768;
+    const int64_t ntiles = dfx_ceil_div(N, NT);
+    int64_t QC = (32ll << 20) / NT;  // 1024 queries per chunk (128 MB of values)
+    if (QC > nq) QC = nq;
+    idx->w_vals.reserve((size_t)QC * NT * 4);
+    idx->w_part.reserve((size_t)QC * ntiles * k * 8);
+    float* qnorm = nullptr;
+    if (metric == DFX_METRIC_L2) {
+        idx->w_dis0.reserve((size_t)nq * 4);
+        qnorm = idx->w_dis0.as<float>();
+        dfx_launch_row_norms(d_x, nq, d, qnorm, st);
+    }
+    for (int64_t q0 = 0; q0 < nq; q0 += QC) {
+        const int64_t qc = (nq - q0 < QC) ? (nq - q0) : QC;
+        for (int64_t t = 0; t < ntiles; t++) {
+            const int64_t c0 = t * NT;
+            const int64_t nc = (N - c0 < NT) ? (N - c0) : NT;
+            dfx_launch_gemm_values(d_x + q0 * d, qc, idx->payload.as<float>() + c0 * d,
+                                   idx->xnorm.as<float>() ? idx->xnorm.as<float>() + c0 : nullptr,
+                                   nc, d, metric, idx->w_vals.as<float>(), NT, st);
+            dfx_launch_select_cols(idx->w_vals.as<float>(), qc, (int)nc, NT, k, (uint32_t)c0,
+                                   nullptr, nullptr, idx->w_part.as<uint64_t>() + t * k,
+                                   ntiles * k, st);
+        }
+        CompLoader ldr{idx->w_part.as<uint64_t>(), ntiles * k};
+        ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, metric, qnorm ? qnorm + q0 : nullptr};
+        dfx_launch_select<128>(ldr, wr, qc, (int)(ntiles * k), k, st);
+    }
+}
+
+// the IVF list scans; plan_ivf picks one per search
+enum class ScanFamily {
+    Fs,      // IVF-PQ FastScan: u8 quantized table, integer sums (scan_pq_fs_kernel<M>)
+    Pq4,     // IVF-PQ, 4-bit codes: table in registers (scan_pq4_kernel<M>)
+    PqIl2,   // IVF-PQ, M = 32 interleaved: table build and block scan in one kernel (dfx_scan_il2.cu)
+    PqWide,  // IVF-PQ, 64 < M <= 128: the scan builds the table in its own shared memory
+    Pq,      // IVF-PQ, 8-bit row-major codes, M <= 64 (scan_pq_kernel)
+    Rows,    // IVF-Flat, IVF-SQ fp16, IVF-SQ8 (scan_rows_kernel)
+};
+
+// what an IVF search decides once, before it launches anything
+struct IvfPlan {
+    int kind;            // the first stage's kind (IVF_PQR: IVF_PQ)
+    bool refine, rflat;  // IVF-PQR or the flat refinement: k candidates re-ranked down to kout
+    int k, kout;         // k = k' = k * k_factor when refining, else kout
+    int nprobe;
+    bool mat;            // k > 1024: candidate rows of ld slots instead of per-warp queues
+    int64_t ld;
+    int64_t QC;          // queries per chunk
+    int cap;             // composites per warp queue: 2 KP, KP = next_pow2(max(k, 32))
+    int wide_threads;    // PqWide: the CTA shape
+    int smetric;         // the list scan's metric (the coarse quantizer's is cfg.metric)
+    bool use_tc;         // coarse quantizer on tensor cores
+    ScanFamily family;
+};
+
+// Every refusal of the IVF path is here, in this order, so a refused search launches nothing (the M
+// checks of launch_list_scan only guard shapes dfx_create refuses).  Runs after the pending rows are
+// finalized, which can change the layout (idx->il).
+static IvfPlan plan_ivf(dfx_index* idx, int64_t nq, int64_t k64) {
+    IvfPlan p{};
     // IVF-PQR and the flat refinement: the base kind's search for k' = (int64)(k * k_factor)
     // candidates (faiss's float product) into workspace rows, re-ranked per query chunk down to
     // kout = k; every sizing rule below sees k'
-    const bool rflat = idx->rflat();
-    const bool refine = idx->cfg.kind == DFX_IVF_PQR || rflat;
-    const int64_t kfirst = refine ? (int64_t)((float)k64 * idx->k_factor) : k64;
-    const int kout = (int)k64;
-    const int k = (int)std::min<int64_t>(kfirst, 1 << 30);
-    const int kind = idx->cfg.kind == DFX_IVF_PQR ? DFX_IVF_PQ : idx->cfg.kind;
-    idx->last_keys_valid = false;
+    p.rflat = idx->rflat();
+    p.refine = idx->cfg.kind == DFX_IVF_PQR || p.rflat;
+    const int64_t kfirst = p.refine ? (int64_t)((float)k64 * idx->k_factor) : k64;
+    p.kout = (int)k64;
+    const int k = p.k = (int)std::min<int64_t>(kfirst, 1 << 30);
+    p.kind = idx->cfg.kind == DFX_IVF_PQR ? DFX_IVF_PQ : idx->cfg.kind;
+    if (p.kind == DFX_IVF_PQ_FS) p.family = ScanFamily::Fs;
+    else if (p.kind != DFX_IVF_PQ) p.family = ScanFamily::Rows;
+    else if (idx->ksub == 16) p.family = ScanFamily::Pq4;
+    else if (idx->il) p.family = ScanFamily::PqIl2;
+    else if (idx->M > 64) p.family = ScanFamily::PqWide;
+    else p.family = ScanFamily::Pq;
 
-    if (kind == DFX_FLAT) {
-        DFX_REQUIRE(k64 <= 4096, "flat search supports k <= 4096");
-        const int64_t N = idx->n_sorted;
-        const int metric = idx->cfg.metric;
-        if (N == 0) {
-            ResultWriter wr{d_D, d_I, k, metric, nullptr};
-            CompLoader ldr{nullptr, 0};
-            dfx_launch_select<128>(ldr, wr, nq, 0, k, st);
-            return;
-        }
-        float* qnorm_tc = nullptr;
-        if (idx->flat_tc && idx->tc_enabled) {  // screening on tensor cores + exact re-rank
-            const int64_t ng = dfx_ceil_div(N, 128) * 4;
-            const int64_t QT = std::max<int64_t>(128, ((64ll << 20) / (ng * 4)) / 128 * 128);
-            bool handled = true;
-            for (int64_t q0 = 0; q0 < nq && handled; q0 += QT) {
-                const int64_t qc = std::min(QT, nq - q0);
-                const int ncand = dfx_tc_flat_candidates(idx, d_x + q0 * d, qc, k, st);
-                if (ncand == 0) {
-                    handled = false;  // shape not covered (only possible on the first chunk)
-                    break;
-                }
-                if (metric == DFX_METRIC_L2 && !qnorm_tc) {
-                    idx->w_dis0.reserve((size_t)nq * 4);
-                    qnorm_tc = idx->w_dis0.as<float>();
-                    dfx_launch_row_norms(d_x, nq, d, qnorm_tc, st);
-                }
-                CompLoader ldr{idx->tc_cand.as<uint64_t>(), ncand};
-                ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, metric, qnorm_tc ? qnorm_tc + q0 : nullptr};
-                dfx_launch_select<128>(ldr, wr, qc, ncand, k, st);
-            }
-            if (handled) return;
-        }
-        const int64_t NT = 32768;
-        const int64_t ntiles = dfx_ceil_div(N, NT);
-        int64_t QC = (32ll << 20) / NT;  // 1024 queries per chunk (128 MB of values)
-        if (QC > nq) QC = nq;
-        idx->w_vals.reserve((size_t)QC * NT * 4);
-        idx->w_part.reserve((size_t)QC * ntiles * k * 8);
-        float* qnorm = nullptr;
-        if (metric == DFX_METRIC_L2) {
-            idx->w_dis0.reserve((size_t)nq * 4);
-            qnorm = idx->w_dis0.as<float>();
-            dfx_launch_row_norms(d_x, nq, d, qnorm, st);
-        }
-        for (int64_t q0 = 0; q0 < nq; q0 += QC) {
-            const int64_t qc = (nq - q0 < QC) ? (nq - q0) : QC;
-            for (int64_t t = 0; t < ntiles; t++) {
-                const int64_t c0 = t * NT;
-                const int64_t nc = (N - c0 < NT) ? (N - c0) : NT;
-                dfx_launch_gemm_values(d_x + q0 * d, qc, idx->payload.as<float>() + c0 * d,
-                                       idx->xnorm.as<float>() ? idx->xnorm.as<float>() + c0 : nullptr,
-                                       nc, d, metric, idx->w_vals.as<float>(), NT, st);
-                dfx_launch_select_cols(idx->w_vals.as<float>(), qc, (int)nc, NT, k, (uint32_t)c0,
-                                       nullptr, nullptr, idx->w_part.as<uint64_t>() + t * k,
-                                       ntiles * k, st);
-            }
-            CompLoader ldr{idx->w_part.as<uint64_t>(), ntiles * k};
-            ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, metric, qnorm ? qnorm + q0 : nullptr};
-            dfx_launch_select<128>(ldr, wr, qc, (int)(ntiles * k), k, st);
-        }
-        return;
-    }
-
-    // ---------------- IVF kinds
     DFX_REQUIRE(k64 <= 4096, "IVF search supports k <= 4096");
     const int pqr_kmax = 16384;  // candidate rows selected by select_cand_kernel: P * 8 = 128 KiB of shared memory
-    DFX_REQUIRE(!refine || kfirst <= pqr_kmax,
-                std::string(rflat ? "RFlat" : "IVF-PQR") + " search at k=" + std::to_string(k64) +
+    DFX_REQUIRE(!p.refine || kfirst <= pqr_kmax,
+                std::string(p.rflat ? "RFlat" : "IVF-PQR") + " search at k=" + std::to_string(k64) +
                     " with k_factor=" + std::to_string(idx->k_factor) + ": k' = " + std::to_string(kfirst) + " candidates to re-rank, more than " +
                     std::to_string(pqr_kmax));
     const int64_t nlist = idx->cfg.nlist;
-    int nprobe = (int)std::min<int64_t>(std::max<int64_t>(idx->nprobe, 1), nlist);
+    const int nprobe = p.nprobe = (int)std::min<int64_t>(std::max<int64_t>(idx->nprobe, 1), nlist);
     DFX_REQUIRE(nprobe <= 4096, "nprobe <= 4096");
-    // k > 1024: candidate rows instead of per-warp queues; ld = slots per row
-    const bool mat = k > 1024;
+    p.mat = k > 1024;
     const int64_t part_max = (int64_t)1 << 24;  // composites of a chunk's partial results / candidates (128 MiB)
-    int64_t ld = 0;
-    if (mat) {
+    if (p.mat) {
         DFX_REQUIRE(idx->h_len_top.size() == (size_t)nlist + 1, "IVF search: list lengths are not known");
-        ld = std::max<int64_t>(idx->h_len_top[(size_t)nprobe], 1);
-        DFX_REQUIRE(ld <= part_max,
+        p.ld = std::max<int64_t>(idx->h_len_top[(size_t)nprobe], 1);
+        DFX_REQUIRE(p.ld <= part_max,
                     "IVF search at k=" + std::to_string(k) + " with nprobe=" + std::to_string(nprobe) +
-                        ": one query's candidates can reach " + std::to_string(ld) +
+                        ": one query's candidates can reach " + std::to_string(p.ld) +
                         " vectors (the nprobe longest lists), more than the 16777216 (128 MiB) of a query chunk");
     }
-    const int cmetric = idx->cfg.metric;  // coarse quantizer metric
-    const int smetric = (kind == DFX_IVF_FLAT) ? idx->cfg.metric : DFX_METRIC_L2;
+    p.smetric = (p.kind == DFX_IVF_FLAT) ? idx->cfg.metric : DFX_METRIC_L2;
 
     // query chunk: bounds the workspace (values matrix on the FFMA coarse path, tables and
     // partial results otherwise)
-    const bool use_tc = idx->tc_enabled && idx->tc_ready && nlist >= 1024 && nprobe <= 512;
-    int64_t QC = use_tc ? 8192 : (32ll << 20) / nlist;
+    p.use_tc = idx->tc_enabled && idx->tc_ready && nlist >= 1024 && nprobe <= 512;
+    int64_t QC = p.use_tc ? 8192 : (32ll << 20) / nlist;
     if (QC < 1) QC = 1;
     if (QC > 8192) QC = 8192;
     // the chunk's partial results (qc x ngroups x k composites) stay within the values matrix's
@@ -923,8 +901,8 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
     // gives at that cap (choose_group never gives a larger chunk more groups per query).
     // k > 1024: the chunk's candidate rows (qc x ld composites) stay within the same 128 MiB.
     const int64_t q1 = std::max<int64_t>(1, part_max / ((int64_t)nprobe * k));
-    if (mat) {
-        QC = std::min(QC, part_max / ld);
+    if (p.mat) {
+        QC = std::min(QC, part_max / p.ld);
     } else if (QC > q1) {
         const int G1 = choose_group(q1, nprobe);
         const int64_t ng1 = (nprobe + G1 - 1) / G1;
@@ -932,41 +910,167 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
     }
     // refinements: the chunk's first-stage rows and refined composites (qc x k' of each) stay within 2^22
     const int64_t pqr_cand_max = (int64_t)1 << 22;
-    if (refine) QC = std::min(QC, std::max<int64_t>(1, pqr_cand_max / k));
+    if (p.refine) QC = std::min(QC, std::max<int64_t>(1, pqr_cand_max / k));
     if (QC > nq) QC = nq;
-    const int KP = dfx_next_pow2(k < 32 ? 32 : k);
-    const int cap = 2 * KP;
+    p.QC = QC;
+    p.cap = 2 * dfx_next_pow2(k < 32 ? 32 : k);
 
-    // IVF-PQ with 64 < M <= 128 (scan_pq_wide_kernel): the widest CTA whose table and per-warp
-    // queues fit in the device's shared memory, decided before anything is launched
+    // 64 < M <= 128: the widest CTA whose table and per-warp queues fit in the device's shared memory
     // (k > 1024: no queues, the table alone; the 512-thread shape, the only one instantiated)
-    int wide_threads = 0;
-    if (kind == DFX_IVF_PQ && idx->M > 64) {
+    if (p.family == ScanFamily::PqWide) {
         const size_t optin = (size_t)dfx_smem_optin();
         for (int t : {512, 256, 128}) {
-            if (dfx_pq_wide_smem(idx->M, t, mat ? 0 : cap) <= optin) {
-                wide_threads = t;
+            if (dfx_pq_wide_smem(idx->M, t, p.mat ? 0 : p.cap) <= optin) {
+                p.wide_threads = t;
                 break;
             }
         }
-        DFX_REQUIRE(!mat || wide_threads == 512, "IVF-PQ with " + std::to_string(idx->M) +
-                                                     " sub-quantizers: the table does not fit in shared memory");
-        DFX_REQUIRE(wide_threads > 0,
+        DFX_REQUIRE(!p.mat || p.wide_threads == 512, "IVF-PQ with " + std::to_string(idx->M) +
+                                                         " sub-quantizers: the table does not fit in shared memory");
+        DFX_REQUIRE(p.wide_threads > 0,
                     "IVF-PQ with " + std::to_string(idx->M) + " sub-quantizers at k=" + std::to_string(k) +
                         ": the distance table and the candidate queues need " +
-                        std::to_string(dfx_pq_wide_smem(idx->M, 128, cap)) +
+                        std::to_string(dfx_pq_wide_smem(idx->M, 128, p.cap)) +
                         " bytes of shared memory per thread block, the device allows " + std::to_string(optin));
     }
+    DFX_REQUIRE(!p.refine || p.rflat || idx->inv_valid, "IVF-PQR search: the id -> position map is not built");
+    return p;
+}
 
+// A runtime value as a template argument: calls f(std::integral_constant<int, V>{}) for the V of
+// the list that equals v, and returns false when none does.  Every V of the list is instantiated.
+template <int... Vs> using IntList = std::integer_sequence<int, Vs...>;
+template <int... Vs, class F>
+static bool dispatch_int(IntList<Vs...>, int v, F&& f) {
+    return ((v == Vs && (f(std::integral_constant<int, Vs>{}), true)) || ...);
+}
+// M of the 4-bit and FastScan scans: a multiple of 8 in [8, 128] (checked by dfx_create)
+using PqMByEight = IntList<8, 16, 24, 32, 40, 48, 56, 64, 72, 80, 88, 96, 104, 112, 120, 128>;
+
+// a list-scan launch, opted in to its dynamic shared memory
+template <class K, class... A>
+static void launch_scan(K kern, unsigned grid, int threads, size_t smem, cudaStream_t st, A... args) {
+    DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    DFX_LAUNCH(kern, grid, threads, smem, st, args...);
+}
+
+// K3 + K4: the list scan of one query chunk, with the table its family needs.  It writes per-group
+// partial results or, k > 1024, the candidate rows into `part`; returns true when it wrote the
+// chunk's final rows (outD, outI) itself.
+static bool launch_list_scan(dfx_index* idx, const IvfPlan& p, const float* xq, int64_t qc, const int32_t* keys,
+                             int G, int ngroups, uint64_t* part, const int64_t* coff, float* outD, int64_t* outI,
+                             cudaStream_t st) {
+    const int d = idx->cfg.d, M = idx->M, ksub = idx->ksub, k = p.k, cap = p.cap, nprobe = p.nprobe;
+    const unsigned grid = (unsigned)(qc * ngroups);
+    if (p.family == ScanFamily::Pq || p.family == ScanFamily::PqWide || p.family == ScanFamily::Pq4) {
+        // K3: each query's [M][ksub] table (w_lut; the wide scan builds its own) and the exact
+        // |q - c|^2 of its probed lists (w_dis0)
+        const bool lut = p.family != ScanFamily::PqWide;
+        if (lut) idx->w_lut.reserve((size_t)qc * M * ksub * 4);
+        idx->w_dis0.reserve((size_t)qc * nprobe * 4);
+        DFX_LAUNCH(pq_prep_kernel, (unsigned)qc, 256, (size_t)((d + 3) / 4) * 16, st, xq, d, M, ksub, idx->dsub,
+                   idx->codebooks.as<float>(), idx->centroids.as<float>(), keys, nprobe,
+                   lut ? idx->w_lut.as<float>() : nullptr, idx->w_dis0.as<float>());
+    }
+    switch (p.family) {
+        case ScanFamily::Fs: {
+            // each query's table quantized to u8 (w_lut) with its (1 / a, b) (w_dis0), then the
+            // integer scan; fs_dequant_kernel maps the selected distances after the selection
+            idx->w_lut.reserve((size_t)qc * M * 16);
+            idx->w_dis0.reserve((size_t)qc * 8);
+            DFX_LAUNCH(pq_fs_lut_kernel, (unsigned)qc, 256, dfx_pq_fs_lut_smem(d, M), st, xq, d, M, idx->dsub,
+                       idx->codebooks.as<float>(), idx->w_lut.as<uint8_t>(), idx->w_dis0.as<float2>());
+            const bool found = dispatch_int(PqMByEight{}, M, [&](auto MT) {
+                launch_scan(p.mat ? scan_pq_fs_kernel<MT, true> : scan_pq_fs_kernel<MT>, grid, 128,
+                            p.mat ? 0 : dfx_pq_fs_smem(cap), st, idx->w_lut.as<uint8_t>(), keys, nprobe, G, ngroups,
+                            idx->list_off.as<int64_t>(), idx->payload.as<uint8_t>(), idx->ids.as<int32_t>(), k, cap,
+                            part, coff);
+            });
+            DFX_REQUIRE(found, "IVF-PQ FastScan: no list scan for M=" + std::to_string(M));
+            return false;
+        }
+        case ScanFamily::Pq4: {
+            const bool found = dispatch_int(PqMByEight{}, M, [&](auto MT) {
+                launch_scan(p.mat ? scan_pq4_kernel<MT, true> : scan_pq4_kernel<MT>, grid, 128,
+                            p.mat ? 0 : dfx_pq4_smem(cap), st, idx->w_lut.as<float>(), idx->w_dis0.as<float>(), keys,
+                            nprobe, G, ngroups, idx->list_off.as<int64_t>(), idx->payload.as<uint8_t>(),
+                            idx->tvals.as<float>(), idx->ids.as<int32_t>(), k, cap, part, coff);
+            });
+            DFX_REQUIRE(found, "IVF-PQ with 4-bit codes: no list scan for M=" + std::to_string(M));
+            return false;
+        }
+        case ScanFamily::PqIl2:
+            // with a single probe group per query the scan also writes the final rows
+            if (!p.mat) return dfx_launch_scan_pq_il2(idx, xq, qc, keys, nprobe, G, ngroups, k, cap, part, outD, outI, st);
+            dfx_launch_scan_pq_il2_mat(idx, xq, qc, keys, nprobe, G, ngroups, part, coff, st);
+            return false;
+        case ScanFamily::PqWide: {
+            const size_t smem = dfx_pq_wide_smem(M, p.wide_threads, p.mat ? 0 : cap);
+            const int mt = (M == 128 || M == 96) ? M : 0;  // any other M % 4 == 0: 32-bit code loads
+            dispatch_int(IntList<128, 96, 0>{}, mt, [&](auto MT) {
+                dispatch_int(IntList<512, 256, 128>{}, p.wide_threads, [&](auto THREADS) {
+                    launch_scan(p.mat ? scan_pq_wide_kernel<MT, 512, true> : scan_pq_wide_kernel<MT, THREADS>, grid,
+                                p.wide_threads, smem, st, xq, d, M, idx->dsub, idx->codebooks.as<float>(),
+                                idx->w_dis0.as<float>(), keys, nprobe, G, ngroups, idx->list_off.as<int64_t>(),
+                                idx->payload.as<uint8_t>(), idx->tvals.as<float>(), idx->ids.as<int32_t>(), k, cap,
+                                part, coff);
+                });
+            });
+            return false;
+        }
+        case ScanFamily::Pq: {
+            const size_t smem = (size_t)M * ksub * 4 + (p.mat ? 0 : (size_t)4 * cap * 8);
+            const int mt = (M == 8 || M == 16 || M == 32 || M == 64) ? M : 0;  // other M: padded to 64 with +0
+            dispatch_int(IntList<8, 16, 32, 64, 0>{}, mt, [&](auto MT) {
+                launch_scan(p.mat ? scan_pq_kernel<MT, true> : scan_pq_kernel<MT>, grid, 128, smem, st,
+                            idx->w_lut.as<float>(), idx->w_dis0.as<float>(), keys, nprobe, G, ngroups,
+                            idx->list_off.as<int64_t>(), idx->payload.as<uint8_t>(), idx->tvals.as<float>(),
+                            idx->ids.as<int32_t>(), M, ksub, k, cap, part, coff);
+            });
+            return false;
+        }
+        case ScanFamily::Rows: {
+            // shared memory: the query; + the raw query (SQ16); + vmin and vdiff (SQ8)
+            const int dq = (p.kind == DFX_IVF_SQ8) ? 4 * d : (p.kind == DFX_IVF_SQ16) ? 2 * d : d;
+            const size_t smem = (((size_t)dq * 4 + 15) / 16) * 16 + (p.mat ? 0 : (size_t)4 * cap * 8);
+            // vectors in flight per warp: rows of up to 1 KB need 8 to cover the DRAM latency,
+            // longer rows keep 4 (rows_inflight overrides)
+            const int inflight = idx->rows_inflight ? idx->rows_inflight : (idx->row_bytes() <= 1024 ? 8 : 4);
+            const int mode = p.kind == DFX_IVF_SQ8 ? 3 : p.kind == DFX_IVF_SQ16 ? 2 : p.smetric == DFX_METRIC_IP ? 0 : 1;
+            dispatch_int(IntList<0, 1, 2, 3>{}, mode, [&](auto MODE) {
+                dispatch_int(IntList<4, 8>{}, inflight, [&](auto U) {
+                    launch_scan(p.mat ? scan_rows_kernel<MODE, U, true> : scan_rows_kernel<MODE, U>, grid, 128, smem,
+                                st, xq, d, idx->centroids.as<float>(), keys, nprobe, G, ngroups,
+                                idx->list_off.as<int64_t>(), idx->payload.p, idx->ids.as<int32_t>(), k, cap, part,
+                                idx->sq_trained.as<float>(), coff);
+                });
+            });
+            return false;
+        }
+    }
+    return false;
+}
+
+void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, float* d_D,
+                     int64_t* d_I, cudaStream_t st) {
+    DFX_REQUIRE(idx->trained || idx->cfg.kind == DFX_FLAT, "index is not trained");
+    DFX_REQUIRE(k64 >= 1, "k must be >= 1");
+    if (nq <= 0) return;
+    if (idx->n_pending > 0) dfx_finalize_impl(idx, st);
+    idx->last_keys_valid = false;
+    if (idx->cfg.kind == DFX_FLAT) return search_flat(idx, nq, d_x, k64, d_D, d_I, st);
+
+    const IvfPlan p = plan_ivf(idx, nq, k64);
+    const int d = idx->cfg.d, k = p.k, kout = p.kout, nprobe = p.nprobe;
+    const int64_t nlist = idx->cfg.nlist, QC = p.QC;
     idx->w_keys.reserve((size_t)nq * nprobe * 4);
     int32_t* keys_all = idx->w_keys.as<int32_t>();
     int64_t* coff = nullptr;  // k > 1024: [qc][nprobe + 1] slot offsets of the candidate rows
-    if (mat) {
+    if (p.mat) {
         idx->w_coff.reserve((size_t)QC * (nprobe + 1) * 8);
         coff = idx->w_coff.as<int64_t>();
     }
-    if (refine) {
-        DFX_REQUIRE(rflat || idx->inv_valid, "IVF-PQR search: the id -> position map is not built");
+    if (p.refine) {
         idx->w_rD.reserve((size_t)QC * k * 4);
         idx->w_rI.reserve((size_t)QC * k * 8);
         idx->w_rcomp.reserve((size_t)QC * k * 8);
@@ -977,166 +1081,45 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
         const float* xq = d_x + q0 * d;
         int32_t* keys = keys_all + q0 * nprobe;
         // where the scan's selection writes: the result rows, or (refinements) the first-stage rows
-        float* outD = refine ? idx->w_rD.as<float>() : d_D + q0 * k;
-        int64_t* outI = refine ? idx->w_rI.as<int64_t>() : d_I + q0 * k;
+        float* outD = p.refine ? idx->w_rD.as<float>() : d_D + q0 * k;
+        int64_t* outI = p.refine ? idx->w_rI.as<int64_t>() : d_I + q0 * k;
         // K1: coarse quantizer -- tensor cores (screen) + canonical fp32 (decide), or plain FFMA
-        if (use_tc) {
+        if (p.use_tc) {
             dfx_tc_coarse_search(idx, xq, qc, nprobe, keys, st);
         } else {
             idx->w_vals.reserve((size_t)QC * nlist * 4);
             dfx_launch_gemm_values(xq, qc, idx->centroids.as<float>(), idx->cnorm.as<float>(), nlist, d,
-                                   cmetric, idx->w_vals.as<float>(), nlist, st);
+                                   idx->cfg.metric, idx->w_vals.as<float>(), nlist, st);
             dfx_launch_select_cols(idx->w_vals.as<float>(), qc, (int)nlist, nlist, nprobe, 0, keys,
                                    nullptr, nullptr, 0, st);
         }
         const int G = choose_group(qc, nprobe);
         const int ngroups = (nprobe + G - 1) / G;
         // k > 1024: `part` holds the candidate rows
-        idx->w_part.reserve(mat ? (size_t)qc * ld * 8 : (size_t)qc * ngroups * k * 8);
+        idx->w_part.reserve(p.mat ? (size_t)qc * p.ld * 8 : (size_t)qc * ngroups * k * 8);
         uint64_t* part = idx->w_part.as<uint64_t>();
-        if (mat)
+        if (p.mat)
             DFX_LAUNCH(cand_offsets_kernel, (unsigned)dfx_ceil_div(qc, 4), 128, 0, st, keys, qc, nprobe,
-                       idx->list_off.as<int64_t>(), ld, coff);
-        std::pair<cudaEvent_t, cudaEvent_t>* pev = nullptr;
-        if (idx->prof_on) {
-            if (idx->prof_used == idx->prof_events.size()) {
-                cudaEvent_t a, b;
-                DFX_CUDA(cudaEventCreate(&a));
-                DFX_CUDA(cudaEventCreate(&b));
-                idx->prof_events.emplace_back(a, b);
-            }
-            pev = &idx->prof_events[idx->prof_used++];
-            DFX_CUDA(cudaEventRecord(pev->first, st));
-        }
-
-        bool final_written = false;
-        if (kind == DFX_IVF_PQ_FS) {
-            // FastScan: each query's table quantized to u8 (w_lut) with its (1 / a, b) (w_dis0), then
-            // the integer scan; fs_dequant_kernel maps the selected distances below
-            const int M = idx->M;
-            idx->w_lut.reserve((size_t)qc * M * 16);
-            idx->w_dis0.reserve((size_t)qc * 8);
-            DFX_LAUNCH(pq_fs_lut_kernel, (unsigned)qc, 256, dfx_pq_fs_lut_smem(d, M), st, xq, d, M, idx->dsub,
-                       idx->codebooks.as<float>(), idx->w_lut.as<uint8_t>(), idx->w_dis0.as<float2>());
-            auto launch = mat ? dfx_launch_scan_pq_fs<true> : dfx_launch_scan_pq_fs<false>;
-            launch(M, (unsigned)(qc * ngroups), mat ? 0 : dfx_pq_fs_smem(cap), st, idx->w_lut.as<uint8_t>(), keys,
-                   nprobe, G, ngroups, idx->list_off.as<int64_t>(), idx->payload.as<uint8_t>(),
-                   idx->ids.as<int32_t>(), k, cap, part, coff);
-        } else if (kind == DFX_IVF_PQ && idx->ksub == 16) {
-            // 4-bit codes: the [M][16] table of each query goes to registers (dfx_scan_pq4_dev.cuh)
-            const int M = idx->M;
-            idx->w_lut.reserve((size_t)qc * M * PQ4_KSUB * 4);
-            idx->w_dis0.reserve((size_t)qc * nprobe * 4);
-            const size_t prep_smem = (size_t)((d + 3) / 4) * 16;
-            DFX_LAUNCH(pq_prep_kernel, (unsigned)qc, 256, prep_smem, st, xq, d, M, PQ4_KSUB, idx->dsub,
-                       idx->codebooks.as<float>(), idx->centroids.as<float>(), keys, nprobe,
-                       idx->w_lut.as<float>(), idx->w_dis0.as<float>());
-            auto launch = mat ? dfx_launch_scan_pq4<true> : dfx_launch_scan_pq4<false>;
-            launch(M, (unsigned)(qc * ngroups), mat ? 0 : dfx_pq4_smem(cap), st, idx->w_lut.as<float>(),
-                   idx->w_dis0.as<float>(), keys, nprobe, G, ngroups, idx->list_off.as<int64_t>(),
-                   idx->payload.as<uint8_t>(), idx->tvals.as<float>(), idx->ids.as<int32_t>(), k, cap, part, coff);
-        } else if (kind == DFX_IVF_PQ && idx->il) {
-            // M == 32: table build + exact |q-c|^2 + block scan in ONE kernel; with a single probe
-            // group per query it also writes the final rows (dfx_scan_il2.cu)
-            if (mat) dfx_launch_scan_pq_il2_mat(idx, xq, qc, keys, nprobe, G, ngroups, part, coff, st);
-            else final_written = dfx_launch_scan_pq_il2(idx, xq, qc, keys, nprobe, G, ngroups, k, cap, part,
-                                                        outD, outI, st);
-        } else if (kind == DFX_IVF_PQ && idx->M > 64) {
-            // 64 < M <= 128: the scan kernel builds the query's table in its own shared memory, so
-            // only |q - c|^2 of the probed lists is prepared here (no w_lut)
-            const int M = idx->M;
-            idx->w_dis0.reserve((size_t)qc * nprobe * 4);
-            const size_t prep_smem = (size_t)((d + 3) / 4) * 16;
-            DFX_LAUNCH(pq_prep_kernel, (unsigned)qc, 256, prep_smem, st, xq, d, M, idx->ksub, idx->dsub,
-                       idx->codebooks.as<float>(), idx->centroids.as<float>(), keys, nprobe, (float*)nullptr,
-                       idx->w_dis0.as<float>());
-            const size_t smem = dfx_pq_wide_smem(M, wide_threads, mat ? 0 : cap);
-#define DFX_SCAN_PQ_WIDE(MT)                                                                     \
-    do {                                                                                         \
-        auto kern = mat                     ? scan_pq_wide_kernel<MT, 512, true>                 \
-                    : (wide_threads == 512) ? scan_pq_wide_kernel<MT, 512>                       \
-                    : (wide_threads == 256) ? scan_pq_wide_kernel<MT, 256>                       \
-                                            : scan_pq_wide_kernel<MT, 128>;                      \
-        DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,         \
-                                      (int)smem));                                               \
-        DFX_LAUNCH(kern, (unsigned)(qc * ngroups), wide_threads, smem, st, xq, d, M, idx->dsub,  \
-                   idx->codebooks.as<float>(), idx->w_dis0.as<float>(), keys, nprobe, G, ngroups, \
-                   idx->list_off.as<int64_t>(), idx->payload.as<uint8_t>(), idx->tvals.as<float>(), \
-                   idx->ids.as<int32_t>(), k, cap, part, coff);                                  \
-    } while (0)
-            if (M == 128) DFX_SCAN_PQ_WIDE(128);
-            else if (M == 96) DFX_SCAN_PQ_WIDE(96);
-            else DFX_SCAN_PQ_WIDE(0);  // any other M % 4 == 0: 32-bit code loads
-#undef DFX_SCAN_PQ_WIDE
-        } else if (kind == DFX_IVF_PQ) {
-            const int M = idx->M, ksub = idx->ksub;
-            idx->w_lut.reserve((size_t)qc * M * ksub * 4);
-            idx->w_dis0.reserve((size_t)qc * nprobe * 4);
-            const size_t prep_smem = (size_t)((d + 3) / 4) * 16;
-            DFX_LAUNCH(pq_prep_kernel, (unsigned)qc, 256, prep_smem, st, xq, d, M, ksub, idx->dsub,
-                       idx->codebooks.as<float>(), idx->centroids.as<float>(), keys, nprobe,
-                       idx->w_lut.as<float>(), idx->w_dis0.as<float>());
-            {
-            const size_t smem = (size_t)M * ksub * 4 + (mat ? 0 : (size_t)4 * cap * 8);
-#define DFX_SCAN_PQ(MT)                                                                          \
-    do {                                                                                         \
-        auto kern = mat ? scan_pq_kernel<MT, true> : scan_pq_kernel<MT>;                         \
-        DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,         \
-                                      (int)smem));                                               \
-        DFX_LAUNCH(kern, (unsigned)(qc * ngroups), 128, smem, st, idx->w_lut.as<float>(),        \
-                   idx->w_dis0.as<float>(), keys, nprobe, G, ngroups, idx->list_off.as<int64_t>(), \
-                   idx->payload.as<uint8_t>(), idx->tvals.as<float>(), idx->ids.as<int32_t>(), M, \
-                   ksub, k, cap, part, coff);                                                    \
-    } while (0)
-            if (M == 32) DFX_SCAN_PQ(32);
-            else if (M == 64) DFX_SCAN_PQ(64);
-            else if (M == 16) DFX_SCAN_PQ(16);
-            else if (M == 8) DFX_SCAN_PQ(8);
-            else DFX_SCAN_PQ(0);  // any other M <= 64: values padded to 64 with +0
-#undef DFX_SCAN_PQ
-            }
-        } else {
-            // shared memory: the query; + the raw query (SQ16); + vmin and vdiff (SQ8)
-            const int dq = (kind == DFX_IVF_SQ8) ? 4 * d : (kind == DFX_IVF_SQ16) ? 2 * d : d;
-            const size_t smem = (((size_t)dq * 4 + 15) / 16) * 16 + (mat ? 0 : (size_t)4 * cap * 8);
-            // vectors in flight per warp: rows of up to 1 KB need 8 to cover the DRAM latency,
-            // longer rows keep 4 (rows_inflight overrides)
-            const int inflight = idx->rows_inflight ? idx->rows_inflight : (idx->row_bytes() <= 1024 ? 8 : 4);
-#define DFX_SCAN_ROWS(MODE)                                                                      \
-    do {                                                                                         \
-        auto kern = (inflight == 8) ? (mat ? scan_rows_kernel<MODE, 8, true> : scan_rows_kernel<MODE, 8>) \
-                                    : (mat ? scan_rows_kernel<MODE, 4, true> : scan_rows_kernel<MODE, 4>); \
-        DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize,         \
-                                      (int)smem));                                               \
-        DFX_LAUNCH(kern, (unsigned)(qc * ngroups), 128, smem, st, xq, d, idx->centroids.as<float>(), \
-                   keys, nprobe, G, ngroups, idx->list_off.as<int64_t>(), idx->payload.p,        \
-                   idx->ids.as<int32_t>(), k, cap, part, idx->sq_trained.as<float>(), coff);     \
-    } while (0)
-            if (kind == DFX_IVF_SQ8) DFX_SCAN_ROWS(3);
-            else if (kind == DFX_IVF_SQ16) DFX_SCAN_ROWS(2);
-            else if (smetric == DFX_METRIC_IP) DFX_SCAN_ROWS(0);
-            else DFX_SCAN_ROWS(1);
-#undef DFX_SCAN_ROWS
-        }
-        if (pev) DFX_CUDA(cudaEventRecord(pev->second, st));
-        if (mat) {
+                       idx->list_off.as<int64_t>(), p.ld, coff);
+        if (idx->prof_on) idx->prof_scan.begin(st);
+        const bool final_written = launch_list_scan(idx, p, xq, qc, keys, G, ngroups, part, coff, outD, outI, st);
+        if (idx->prof_on) idx->prof_scan.end(st);
+        ResultWriter wr{outD, outI, k, p.smetric, nullptr};
+        if (p.mat) {
             // P >= 2048 = sort_cap: a row of up to sort_cap candidates is sorted whole
             const int P = dfx_next_pow2(k);
-            ResultWriter wr{outD, outI, k, smetric, nullptr};
             if ((size_t)P * 8 > 48 * 1024)  // a refinement's k' > 4096: opt in to more shared memory
                 DFX_CUDA(cudaFuncSetAttribute(select_cand_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                               P * 8));
             DFX_LAUNCH(select_cand_kernel<256>, (unsigned)qc, 256, (size_t)P * 8, st, part, coff, nprobe, wr, k, P,
                        2048);
         } else if (!final_written) {
-            CompLoader ldr{part, (int64_t)ngroups * k};
-            ResultWriter wr{outD, outI, k, smetric, nullptr};
-            dfx_launch_select<128>(ldr, wr, qc, ngroups * k, k, st);
+            dfx_launch_select<128>(CompLoader{part, (int64_t)ngroups * k}, wr, qc, ngroups * k, k, st);
         }
-        if (kind == DFX_IVF_PQ_FS && !rflat)  // the flat refinement reads the first stage's ids only
+        if (p.family == ScanFamily::Fs && !p.rflat)  // the flat refinement reads the first stage's ids only
             DFX_LAUNCH(fs_dequant_kernel, (unsigned)dfx_ceil_div(qc * k, 256), 256, 0, st, outD, outI,
                        qc * k, k, idx->w_dis0.as<float2>());
-        if (refine) refine_candidates(idx, xq, qc, k, kout, outI, d_D + q0 * kout, d_I + q0 * kout, st);
+        if (p.refine) refine_candidates(idx, xq, qc, k, kout, outI, d_D + q0 * kout, d_I + q0 * kout, st);
     }
     idx->last_nq = nq;
     idx->last_nprobe = nprobe;
