@@ -160,16 +160,8 @@ __global__ void pq_tvals_kernel(const uint8_t* __restrict__ codes, const int32_t
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     int64_t l;
-    if (list_of) {
-        l = list_of[i];
-    } else {  // list-sorted storage: binary search the list owning row i
-        int64_t lo = 0, hi = nlist;
-        while (hi - lo > 1) {
-            int64_t mid = (lo + hi) >> 1;
-            if (list_off[mid] <= i) lo = mid; else hi = mid;
-        }
-        l = lo;
-    }
+    if (list_of) l = list_of[i];
+    else l = dfx_list_of(list_off, nlist, i);  // list-sorted storage: the list owning row i
     const float* c = cent + (size_t)l * d;
     float t = 0.f;
     for (int m = 0; m < M; m++) {
@@ -250,12 +242,7 @@ __global__ void expand_lists_kernel(const int64_t* __restrict__ list_off, int64_
                                     int32_t* __restrict__ out) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    int64_t lo = 0, hi = nlist;
-    while (hi - lo > 1) {
-        int64_t mid = (lo + hi) >> 1;
-        if (list_off[mid] <= i) lo = mid; else hi = mid;
-    }
-    out[i] = (int32_t)lo;
+    out[i] = (int32_t)dfx_list_of(list_off, nlist, i);
 }
 
 // new[i] = (src < n_sorted ? old_sorted[src] : pending[src - n_sorted]) in 4-byte words
@@ -284,24 +271,79 @@ __global__ void widen_kernel(const int32_t* __restrict__ in, int64_t n, int64_t*
 
 static inline unsigned blocks_for(int64_t n, int t) { return (unsigned)dfx_ceil_div(n, t); }
 
-// codes u8[n][M] of the rows x themselves (pq_encode_kernel<DS, false>: no centroid subtracted)
-static void launch_pq_encode_raw(const float* x, int64_t n, int d, int M, int ksub, int dsub, const float* codebooks,
-                                 uint8_t* codes, cudaStream_t st) {
+// codes u8[n][M], one per byte: the nearest codeword of each sub-vector of the residual x - c
+// (res; c = cent[assign[i]]) or of the row x itself (!res: cent and assign are not read).  The
+// kernel keeps the sub-vector in registers for the common dsub (6: d = 768 with M = 128, residual
+// codes only); any other dsub runs the generic DS = 0.
+static void launch_pq_encode(bool res, const float* x, const float* cent, const int32_t* assign, int64_t n, int d,
+                             int M, int ksub, int dsub, const float* codebooks, uint8_t* codes, cudaStream_t st) {
     if (n <= 0) return;
-    dim3 grid(blocks_for(n, 256), (unsigned)M);
-#define DFX_PQ_ENCODE_RAW(DS)                                                                          \
-    do {                                                                                               \
-        auto kern = pq_encode_kernel<DS, false>;                                                       \
-        DFX_LAUNCH(kern, grid, 256, (size_t)ksub * dsub * 4, st, x, (const float*)nullptr,             \
-                   (const int32_t*)nullptr, n, d, M, ksub, dsub, codebooks, codes);                    \
-    } while (0)
-    if (dsub == 2) DFX_PQ_ENCODE_RAW(2);
-    else if (dsub == 4) DFX_PQ_ENCODE_RAW(4);
-    else if (dsub == 8) DFX_PQ_ENCODE_RAW(8);
-    else if (dsub == 16) DFX_PQ_ENCODE_RAW(16);
-    else DFX_PQ_ENCODE_RAW(0);
-#undef DFX_PQ_ENCODE_RAW
+    const dim3 grid(blocks_for(n, 256), (unsigned)M);
+    auto launch = [&](auto DS, auto RES) {
+        auto kern = pq_encode_kernel<decltype(DS)::value, decltype(RES)::value>;
+        DFX_LAUNCH(kern, grid, 256, (size_t)ksub * dsub * 4, st, x, cent, assign, n, d, M, ksub, dsub, codebooks,
+                   codes);
+    };
+    if (res) {
+        if (!dispatch_int(IntList<2, 4, 6, 8, 16>{}, dsub, [&](auto DS) { launch(DS, std::true_type{}); }))
+            launch(std::integral_constant<int, 0>{}, std::true_type{});
+    } else if (!dispatch_int(IntList<2, 4, 8, 16>{}, dsub, [&](auto DS) { launch(DS, std::false_type{}); })) {
+        launch(std::integral_constant<int, 0>{}, std::false_type{});
+    }
 }
+
+// k distinct rows of x f32[n][d] chosen at random (a partial Fisher-Yates shuffle of 0..n-1 driven by
+// mt19937_64(seed)) -> out f32[k][d]
+static void gather_random_rows(const float* x, int64_t n, int d, int64_t k, uint64_t seed, float* out,
+                               cudaStream_t st) {
+    std::vector<int32_t> perm((size_t)n);
+    std::iota(perm.begin(), perm.end(), 0);
+    std::mt19937_64 rng(seed);
+    for (int64_t i = 0; i < k; i++) {
+        int64_t j = i + (int64_t)(rng() % (uint64_t)(n - i));
+        std::swap(perm[(size_t)i], perm[(size_t)j]);
+    }
+    DevBuf d_sel;
+    d_sel.reserve((size_t)k * 4);
+    DFX_CUDA(cudaMemcpyAsync(d_sel.p, perm.data(), (size_t)k * 4, cudaMemcpyHostToDevice, st));
+    DFX_LAUNCH(gather_rows_kernel, blocks_for(k * d, 256), 256, 0, st, x, d_sel.as<int32_t>(), k, d, 0, d, out);
+    DFX_CUDA(cudaStreamSynchronize(st));  // perm is on the stack of this call
+}
+
+// Rows grouped by an int32 key in [0, nkeys): run(keys) leaves cnt[key] = rows per key, off = the
+// exclusive prefix sum of cnt (nkeys + 1 entries) and order = the row indices sorted by key (a
+// stable radix sort, so rows keep ascending order inside a key).  The buffers and cub's temporary
+// storage are sized once for n rows; run() may be repeated on new keys.
+struct KeyBuckets {
+    int64_t n, nkeys;
+    int bits = 1;
+    DevBuf keys_out, order_in, order, cnt, off, tmp;
+    KeyBuckets(int64_t n_, int64_t nkeys_, cudaStream_t st) : n(n_), nkeys(nkeys_) {
+        keys_out.reserve((size_t)n * 4);
+        order_in.reserve((size_t)n * 4);
+        order.reserve((size_t)n * 4);
+        cnt.reserve((size_t)(nkeys + 1) * 4);
+        off.reserve((size_t)(nkeys + 1) * 4);
+        DFX_LAUNCH(iota_kernel, blocks_for(n, 256), 256, 0, st, order_in.as<int32_t>(), n);
+        while ((1ll << bits) < nkeys) bits++;
+        size_t tmp_sort = 0, tmp_scan = 0;
+        cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, (const int32_t*)nullptr, keys_out.as<int32_t>(),
+                                        order_in.as<int32_t>(), order.as<int32_t>(), (int)n, 0, bits, st);
+        cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, cnt.as<int32_t>(), off.as<int32_t>(), (int)(nkeys + 1), st);
+        tmp.reserve(std::max(tmp_sort, tmp_scan));
+    }
+    void run(const int32_t* keys, cudaStream_t st) {
+        DFX_CUDA(cudaMemsetAsync(cnt.p, 0, (size_t)(nkeys + 1) * 4, st));
+        DFX_LAUNCH(count_kernel, blocks_for(n, 256), 256, 0, st, keys, n, cnt.as<int32_t>());
+        size_t tb = tmp.cap;
+        DFX_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, cnt.as<int32_t>(), off.as<int32_t>(), (int)(nkeys + 1),
+                                               st));
+        tb = tmp.cap;
+        DFX_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, keys, keys_out.as<int32_t>(), order_in.as<int32_t>(),
+                                                 order.as<int32_t>(), (int)n, 0, bits, st));
+        g_dfx_launches.fetch_add(2, std::memory_order_relaxed);
+    }
+};
 
 // ------------------------------------------------------------------ assign
 void dfx_assign_impl(dfx_index* idx, const float* d_cent, const float* d_cnorm, int64_t nlist,
@@ -323,59 +365,24 @@ static void kmeans_device(dfx_index* idx, int d, int64_t n, const float* d_x, in
     DFX_REQUIRE(n >= k, "k-means: need at least as many training points as centroids (" +
                             std::to_string(n) + " < " + std::to_string(k) + ")");
     DFX_REQUIRE(n < (1ll << 31), "k-means: too many training points");
-    // init = random subset without replacement
-    std::vector<int32_t> perm((size_t)n);
-    std::iota(perm.begin(), perm.end(), 0);
-    std::mt19937_64 rng(seed);
-    for (int64_t i = 0; i < k; i++) {
-        int64_t j = i + (int64_t)(rng() % (uint64_t)(n - i));
-        std::swap(perm[(size_t)i], perm[(size_t)j]);
-    }
-    DevBuf d_sel, d_assign, d_order_in, d_order, d_keys_out, d_cnt, d_off, d_cnorm, d_tmp;
-    d_sel.reserve((size_t)k * 4);
-    DFX_CUDA(cudaMemcpyAsync(d_sel.p, perm.data(), (size_t)k * 4, cudaMemcpyHostToDevice, st));
-    DFX_LAUNCH(gather_rows_kernel, blocks_for(k * d, 256), 256, 0, st, d_x, d_sel.as<int32_t>(), k, d,
-               0, d, d_cent);
-    DFX_CUDA(cudaStreamSynchronize(st));
+    gather_random_rows(d_x, n, d, k, seed, d_cent, st);  // init = random subset without replacement
 
+    DevBuf d_assign, d_cnorm;
     d_assign.reserve((size_t)n * 4);
-    d_order_in.reserve((size_t)n * 4);
-    d_order.reserve((size_t)n * 4);
-    d_keys_out.reserve((size_t)n * 4);
-    d_cnt.reserve((size_t)(k + 1) * 4);
-    d_off.reserve((size_t)(k + 1) * 4);
     d_cnorm.reserve((size_t)k * 4);
-    DFX_LAUNCH(iota_kernel, blocks_for(n, 256), 256, 0, st, d_order_in.as<int32_t>(), n);
-    int bits = 1;
-    while ((1ll << bits) < k) bits++;
-    size_t tmp_sort = 0, tmp_scan = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, d_assign.as<int32_t>(), d_keys_out.as<int32_t>(),
-                                    d_order_in.as<int32_t>(), d_order.as<int32_t>(), (int)n, 0, bits, st);
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, d_cnt.as<int32_t>(), d_off.as<int32_t>(),
-                                  (int)(k + 1), st);
-    d_tmp.reserve(std::max(tmp_sort, tmp_scan));
+    KeyBuckets b(n, k, st);
     std::vector<int32_t> h_cnt((size_t)k + 1);
 
     for (int it = 0; it < niter; it++) {
         dfx_launch_row_norms(d_cent, k, d, d_cnorm.as<float>(), st);
         dfx_assign_impl(idx, d_cent, d_cnorm.as<float>(), k, DFX_METRIC_L2, d, n, d_x,
                         d_assign.as<int32_t>(), st);
-        DFX_CUDA(cudaMemsetAsync(d_cnt.p, 0, (size_t)(k + 1) * 4, st));
-        DFX_LAUNCH(count_kernel, blocks_for(n, 256), 256, 0, st, d_assign.as<int32_t>(), n,
-                   d_cnt.as<int32_t>());
-        size_t tb = d_tmp.cap;
-        DFX_CUDA(cub::DeviceScan::ExclusiveSum(d_tmp.p, tb, d_cnt.as<int32_t>(), d_off.as<int32_t>(),
-                                               (int)(k + 1), st));
-        tb = d_tmp.cap;
-        DFX_CUDA(cub::DeviceRadixSort::SortPairs(d_tmp.p, tb, d_assign.as<int32_t>(),
-                                                 d_keys_out.as<int32_t>(), d_order_in.as<int32_t>(),
-                                                 d_order.as<int32_t>(), (int)n, 0, bits, st));
-        g_dfx_launches.fetch_add(2, std::memory_order_relaxed);
+        b.run(d_assign.as<int32_t>(), st);
         int threads = d >= 128 ? 128 : (d >= 64 ? 64 : 32);
-        DFX_LAUNCH(centroid_update_kernel, (unsigned)k, threads, 0, st, d_x, d, d_order.as<int32_t>(),
-                   d_off.as<int32_t>(), d_cent);
+        DFX_LAUNCH(centroid_update_kernel, (unsigned)k, threads, 0, st, d_x, d, b.order.as<int32_t>(),
+                   b.off.as<int32_t>(), d_cent);
         // empty clusters: split the currently largest (host decides, like the oracle)
-        DFX_CUDA(cudaMemcpyAsync(h_cnt.data(), d_cnt.p, (size_t)k * 4, cudaMemcpyDeviceToHost, st));
+        DFX_CUDA(cudaMemcpyAsync(h_cnt.data(), b.cnt.p, (size_t)k * 4, cudaMemcpyDeviceToHost, st));
         DFX_CUDA(cudaStreamSynchronize(st));
         for (int64_t c = 0; c < k; c++) {
             if (h_cnt[(size_t)c] != 0) continue;
@@ -390,130 +397,99 @@ static void kmeans_device(dfx_index* idx, int d, int64_t n, const float* d_x, in
 }
 
 // ------------------------------------------------------------------ train
-void dfx_train_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) {
-    const int kind = idx->cfg.kind;
-    if (kind == DFX_FLAT) {
-        idx->trained = true;
-        return;
-    }
+// the coarse quantizer from the k-means sample xt f32[nt][d]: centroids, their norms and the
+// tensor-core screening table
+static void train_coarse(dfx_index* idx, int64_t nt, const float* xt, int niter, cudaStream_t st) {
     const int d = idx->cfg.d;
     const int64_t nlist = idx->cfg.nlist;
-    DFX_REQUIRE(n >= nlist, "train: need at least nlist=" + std::to_string(nlist) +
-                                " training vectors, got " + std::to_string(n));
-    const int niter = idx->kmeans_niter > 0 ? idx->kmeans_niter : 25;
-    const uint64_t seed = idx->train_seed;
-
-    // faiss Clustering: at most 256 points per centroid (random subset)
-    const float* xt = d_x;
-    int64_t nt = n;
-    DevBuf sub;
-    const int64_t maxpts = (int64_t)idx->max_points_per_centroid * nlist;
-    if (n > maxpts) {
-        std::vector<int32_t> perm((size_t)n);
-        std::iota(perm.begin(), perm.end(), 0);
-        std::mt19937_64 rng(seed ^ 0x5bd1e995u);
-        for (int64_t i = 0; i < maxpts; i++) {
-            int64_t j = i + (int64_t)(rng() % (uint64_t)(n - i));
-            std::swap(perm[(size_t)i], perm[(size_t)j]);
-        }
-        DevBuf d_sel;
-        d_sel.reserve((size_t)maxpts * 4);
-        DFX_CUDA(cudaMemcpyAsync(d_sel.p, perm.data(), (size_t)maxpts * 4, cudaMemcpyHostToDevice, st));
-        sub.reserve((size_t)maxpts * d * 4);
-        DFX_LAUNCH(gather_rows_kernel, blocks_for(maxpts * d, 256), 256, 0, st, d_x,
-                   d_sel.as<int32_t>(), maxpts, d, 0, d, sub.as<float>());
-        DFX_CUDA(cudaStreamSynchronize(st));
-        xt = sub.as<float>();
-        nt = maxpts;
-    }
     idx->centroids.reserve((size_t)nlist * d * 4);
     idx->cnorm.reserve((size_t)nlist * 4);
-    kmeans_device(idx, d, nt, xt, nlist, niter, seed, idx->centroids.as<float>(), st);
+    kmeans_device(idx, d, nt, xt, nlist, niter, idx->train_seed, idx->centroids.as<float>(), st);
     dfx_launch_row_norms(idx->centroids.as<float>(), nlist, d, idx->cnorm.as<float>(), st);
     dfx_tc_prepare_centroids(idx, st);
+}
 
-    if (idx->pq_res()) {
+// residuals r = x - c of the rows x f32[ns][d], c the nearest coarse centroid under the index's
+// metric -> res f32[ns][d]
+static void sample_residuals(dfx_index* idx, const float* x, int64_t ns, DevBuf& res, cudaStream_t st) {
+    const int d = idx->cfg.d;
+    DevBuf assign;
+    assign.reserve((size_t)ns * 4);
+    res.reserve((size_t)ns * d * 4);
+    dfx_assign_impl(idx, idx->centroids.as<float>(), idx->cnorm.as<float>(), idx->cfg.nlist, idx->cfg.metric, d, ns,
+                    x, assign.as<int32_t>(), st);
+    DFX_LAUNCH(residual_kernel, blocks_for(ns * d, 256), 256, 0, st, x, idx->centroids.as<float>(),
+               assign.as<int32_t>(), ns, d, res.as<float>());
+}
+
+// the M sub-quantizers of a PQ: sub-quantizer m is k-means (ksub centroids, seed seed0 + m) on
+// column slice m of rows f32[ns][ld], into out[m] f32[ksub][dsub]
+static void train_subquantizers(dfx_index* idx, const float* rows, int64_t ns, int ld, int M, int ksub, int dsub,
+                                int niter, uint64_t seed0, float* out, cudaStream_t st) {
+    DevBuf subv;
+    subv.reserve((size_t)ns * dsub * 4);
+    for (int m = 0; m < M; m++) {
+        DFX_LAUNCH(gather_rows_kernel, blocks_for(ns * dsub, 256), 256, 0, st, rows, (const int32_t*)nullptr, ns, dsub,
+                   m * dsub, ld, subv.as<float>());
+        kmeans_device(idx, dsub, ns, subv.as<float>(), ksub, niter, seed0 + m, out + (size_t)m * ksub * dsub, st);
+    }
+}
+
+// the codec of the kind, trained on the first rows of the k-means sample xt f32[nt][d]
+static void train_codec(dfx_index* idx, int64_t nt, const float* xt, int niter, cudaStream_t st) {
+    const int kind = idx->cfg.kind, d = idx->cfg.d;
+    const uint64_t seed = idx->train_seed;
+    if (idx->has_pq()) {
+        // faiss ProductQuantizer on the first min(nt, 256 * ksub) rows: their residuals (IVF_PQ,
+        // IVF_PQR), or the raw sub-vectors (FastScan is not by_residual)
         const int M = idx->M, ksub = idx->ksub, dsub = idx->dsub;
-        int64_t ns = std::min<int64_t>(nt, 256ll * ksub);
+        const int64_t ns = std::min<int64_t>(nt, 256ll * ksub);
         DFX_REQUIRE(ns >= ksub, "train: need at least " + std::to_string(ksub) + " vectors for PQ");
-        DevBuf d_assign, d_res, d_subv, d_cb;
-        d_assign.reserve((size_t)ns * 4);
-        d_res.reserve((size_t)ns * d * 4);
-        d_subv.reserve((size_t)ns * dsub * 4);
-        dfx_assign_impl(idx, idx->centroids.as<float>(), idx->cnorm.as<float>(), nlist, idx->cfg.metric,
-                        d, ns, xt, d_assign.as<int32_t>(), st);
-        DFX_LAUNCH(residual_kernel, blocks_for(ns * d, 256), 256, 0, st, xt, idx->centroids.as<float>(),
-                   d_assign.as<int32_t>(), ns, d, d_res.as<float>());
+        DevBuf res;
+        if (idx->pq_res()) sample_residuals(idx, xt, ns, res, st);
+        const float* rows = idx->pq_res() ? res.as<float>() : xt;
         idx->codebooks.reserve((size_t)M * ksub * dsub * 4);
         idx->cbT_valid = false;
-        for (int m = 0; m < M; m++) {
-            DFX_LAUNCH(gather_rows_kernel, blocks_for(ns * dsub, 256), 256, 0, st, d_res.as<float>(),
-                       (const int32_t*)nullptr, ns, dsub, m * dsub, d, d_subv.as<float>());
-            kmeans_device(idx, dsub, ns, d_subv.as<float>(), ksub, niter, seed + 1 + m,
-                          idx->codebooks.as<float>() + (size_t)m * ksub * dsub, st);
-        }
+        train_subquantizers(idx, rows, ns, d, M, ksub, dsub, niter, seed + 1, idx->codebooks.as<float>(), st);
         if (kind == DFX_IVF_PQR) {
             // faiss IndexIVFPQR::train_encoder: the refinement PQ is trained on what PQ1 leaves of the
             // same residuals, r2 = r - decode(encode(r)); seeds seed + 1 + M + m2 (PQ1 has seed + 1 + m)
             const int M2 = idx->M2, dsub2 = idx->dsub2;
-            DevBuf d_codes, d_r2;
-            d_codes.reserve((size_t)ns * M);
-            d_r2.reserve((size_t)ns * d * 4);
-            launch_pq_encode_raw(d_res.as<float>(), ns, d, M, ksub, dsub, idx->codebooks.as<float>(),
-                                 d_codes.as<uint8_t>(), st);
-            DFX_LAUNCH(pq_residual2_kernel, blocks_for(ns * d, 256), 256, 0, st, d_res.as<float>(), (const float*)nullptr,
-                       (const int32_t*)nullptr, d_codes.as<uint8_t>(), ns, d, M, dsub, idx->codebooks.as<float>(),
-                       d_r2.as<float>());
-            d_subv.reserve((size_t)ns * dsub2 * 4);
+            DevBuf codes, r2;
+            codes.reserve((size_t)ns * M);
+            r2.reserve((size_t)ns * d * 4);
+            launch_pq_encode(false, rows, nullptr, nullptr, ns, d, M, ksub, dsub, idx->codebooks.as<float>(),
+                             codes.as<uint8_t>(), st);
+            DFX_LAUNCH(pq_residual2_kernel, blocks_for(ns * d, 256), 256, 0, st, rows, (const float*)nullptr,
+                       (const int32_t*)nullptr, codes.as<uint8_t>(), ns, d, M, dsub, idx->codebooks.as<float>(),
+                       r2.as<float>());
             idx->refine_cb.reserve((size_t)M2 * 256 * dsub2 * 4);
-            for (int m2 = 0; m2 < M2; m2++) {
-                DFX_LAUNCH(gather_rows_kernel, blocks_for(ns * dsub2, 256), 256, 0, st, d_r2.as<float>(),
-                           (const int32_t*)nullptr, ns, dsub2, m2 * dsub2, d, d_subv.as<float>());
-                kmeans_device(idx, dsub2, ns, d_subv.as<float>(), 256, niter, seed + 1 + M + m2,
-                              idx->refine_cb.as<float>() + (size_t)m2 * 256 * dsub2, st);
-            }
+            train_subquantizers(idx, r2.as<float>(), ns, d, M2, 256, dsub2, niter, seed + 1 + M,
+                                idx->refine_cb.as<float>(), st);
         }
-    }
-    if (kind == DFX_IVF_PQ_FS) {
-        // FastScan is not by_residual: the 16-centroid sub-quantizers are trained on the raw
-        // sub-vectors of the first min(nt, 256 * ksub) rows of the k-means sample
-        const int M = idx->M, ksub = idx->ksub, dsub = idx->dsub;
-        const int64_t ns = std::min<int64_t>(nt, 256ll * ksub);
-        DFX_REQUIRE(ns >= ksub, "train: need at least " + std::to_string(ksub) + " vectors for PQ");
-        DevBuf d_subv;
-        d_subv.reserve((size_t)ns * dsub * 4);
-        idx->codebooks.reserve((size_t)M * ksub * dsub * 4);
-        for (int m = 0; m < M; m++) {
-            DFX_LAUNCH(gather_rows_kernel, blocks_for(ns * dsub, 256), 256, 0, st, xt, (const int32_t*)nullptr, ns,
-                       dsub, m * dsub, d, d_subv.as<float>());
-            kmeans_device(idx, dsub, ns, d_subv.as<float>(), ksub, niter, seed + 1 + m,
-                          idx->codebooks.as<float>() + (size_t)m * ksub * dsub, st);
-        }
-    }
-    if (kind == DFX_IVF_SQ8) {
+    } else if (kind == DFX_IVF_SQ8) {
         // faiss ScalarQuantizer (QT_8bit, RS_minmax) on the residuals of the first min(nt, 100000)
         // rows of the k-means sample, the way the PQ above takes a prefix of it
         const int64_t ns = std::min<int64_t>(nt, 100000);
         const int64_t rows_per = 256;
         const int64_t nch = dfx_ceil_div(ns, rows_per);
-        DevBuf d_assign, d_res, d_part;
-        d_assign.reserve((size_t)ns * 4);
-        d_res.reserve((size_t)ns * d * 4);
-        d_part.reserve((size_t)nch * d * 8);
-        dfx_assign_impl(idx, idx->centroids.as<float>(), idx->cnorm.as<float>(), nlist, idx->cfg.metric,
-                        d, ns, xt, d_assign.as<int32_t>(), st);
-        DFX_LAUNCH(residual_kernel, blocks_for(ns * d, 256), 256, 0, st, xt, idx->centroids.as<float>(),
-                   d_assign.as<int32_t>(), ns, d, d_res.as<float>());
-        float* pmin = d_part.as<float>();
+        DevBuf res, part;
+        sample_residuals(idx, xt, ns, res, st);
+        part.reserve((size_t)nch * d * 8);
+        float* pmin = part.as<float>();
         float* pmax = pmin + (size_t)nch * d;
         DFX_LAUNCH(sq8_minmax_partial_kernel, dim3(blocks_for(d, 128), (unsigned)nch), 128, 0, st,
-                   d_res.as<float>(), ns, d, rows_per, pmin, pmax);
+                   res.as<float>(), ns, d, rows_per, pmin, pmax);
         idx->sq_trained.reserve((size_t)2 * d * 4);
         DFX_LAUNCH(sq8_minmax_final_kernel, blocks_for(d, 128), 128, 0, st, pmin, pmax, nch, d,
                    idx->sq_trained.as<float>());
         DFX_CUDA(cudaStreamSynchronize(st));
     }
-    // an empty, trained index
+}
+
+// an empty, trained index
+static void start_empty_lists(dfx_index* idx, cudaStream_t st) {
+    const int64_t nlist = idx->cfg.nlist;
     idx->h_list_off.assign((size_t)nlist + 1, 0);
     idx->update_list_lengths();
     idx->list_off.reserve((size_t)(nlist + 1) * 8);
@@ -522,10 +498,32 @@ void dfx_train_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st
     idx->n_sorted = 0;
     idx->n_pending = 0;
     idx->trained = true;
-    if (kind == DFX_IVF_PQR) {
-        idx->inv_valid = false;
-        dfx_refresh_inv(idx, st);
+    dfx_layout_changed(idx, st);
+}
+
+void dfx_train_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) {
+    if (idx->cfg.kind == DFX_FLAT) {
+        idx->trained = true;
+        return;
     }
+    const int d = idx->cfg.d;
+    const int64_t nlist = idx->cfg.nlist;
+    DFX_REQUIRE(n >= nlist, "train: need at least nlist=" + std::to_string(nlist) +
+                                " training vectors, got " + std::to_string(n));
+    const int niter = idx->kmeans_niter > 0 ? idx->kmeans_niter : 25;
+
+    // faiss Clustering: at most 256 points per centroid (random subset)
+    const int64_t nt = std::min<int64_t>(n, (int64_t)idx->max_points_per_centroid * nlist);
+    const float* xt = d_x;
+    DevBuf sub;
+    if (nt < n) {
+        sub.reserve((size_t)nt * d * 4);
+        gather_random_rows(d_x, n, d, nt, idx->train_seed ^ 0x5bd1e995u, sub.as<float>(), st);
+        xt = sub.as<float>();
+    }
+    train_coarse(idx, nt, xt, niter, st);
+    train_codec(idx, nt, xt, niter, st);
+    start_empty_lists(idx, st);
 }
 
 // ------------------------------------------------------------------ add
@@ -542,104 +540,49 @@ static void ensure_pending(dfx_index* idx, int64_t need, cudaStream_t st) {
     idx->p_cap = cap;
 }
 
-void dfx_add_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) {
-    if (n <= 0) return;
-    const int kind = idx->cfg.kind;
+// FLAT: the rows in arrival order, and their norms under L2
+static void add_flat(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) {
     const int d = idx->cfg.d;
-    DFX_REQUIRE(idx->ntotal() + n < (1ll << 31), "a shard holds at most 2^31-1 vectors");
-    if (kind == DFX_FLAT) {
-        const int64_t N = idx->n_sorted;
-        if ((size_t)(N + n) * d * 4 > idx->payload.cap) {
-            int64_t cap = std::max<int64_t>({N + n, 2 * N, idx->reserve_hint});
-            idx->payload.reserve((size_t)cap * d * 4, (size_t)N * d * 4, st);
-            if (idx->cfg.metric == DFX_METRIC_L2) idx->xnorm.reserve((size_t)cap * 4, (size_t)N * 4, st);
-        }
-        DFX_CUDA(cudaMemcpyAsync(idx->payload.as<float>() + N * d, d_x, (size_t)n * d * 4,
-                                 cudaMemcpyDeviceToDevice, st));
-        if (idx->cfg.metric == DFX_METRIC_L2)
-            dfx_launch_row_norms(d_x, n, d, idx->xnorm.as<float>() + N, st);
-        idx->n_sorted += n;
-        return;
+    const int64_t N = idx->n_sorted;
+    if ((size_t)(N + n) * d * 4 > idx->payload.cap) {
+        int64_t cap = std::max<int64_t>({N + n, 2 * N, idx->reserve_hint});
+        idx->payload.reserve((size_t)cap * d * 4, (size_t)N * d * 4, st);
+        if (idx->cfg.metric == DFX_METRIC_L2) idx->xnorm.reserve((size_t)cap * 4, (size_t)N * 4, st);
     }
-    DFX_REQUIRE(idx->trained, "add: index is not trained");
-    const int64_t nlist = idx->cfg.nlist;
-    ensure_pending(idx, idx->n_pending + n, st);
-    int32_t* plist = idx->p_list.as<int32_t>() + idx->n_pending;
-    dfx_assign_impl(idx, idx->centroids.as<float>(), idx->cnorm.as<float>(), nlist, idx->cfg.metric, d, n,
-                    d_x, plist, st);
-    const size_t rb = idx->row_bytes();
-    unsigned char* prow = idx->p_payload.as<unsigned char>() + (size_t)idx->n_pending * rb;
+    DFX_CUDA(cudaMemcpyAsync(idx->payload.as<float>() + N * d, d_x, (size_t)n * d * 4,
+                             cudaMemcpyDeviceToDevice, st));
+    if (idx->cfg.metric == DFX_METRIC_L2)
+        dfx_launch_row_norms(d_x, n, d, idx->xnorm.as<float>() + N, st);
+    idx->n_sorted += n;
+}
+
+// the pending list rows (prow, row_bytes() each) of n new vectors x whose lists are plist
+static void encode_rows(dfx_index* idx, int64_t n, const float* d_x, const int32_t* plist, unsigned char* prow,
+                        cudaStream_t st) {
+    const int kind = idx->cfg.kind, d = idx->cfg.d;
     if (kind == DFX_IVF_FLAT) {
-        DFX_CUDA(cudaMemcpyAsync(prow, d_x, (size_t)n * rb, cudaMemcpyDeviceToDevice, st));
-    } else if (idx->pq_res()) {
-        const int M = idx->M, ksub = idx->ksub, dsub = idx->dsub;
+        DFX_CUDA(cudaMemcpyAsync(prow, d_x, (size_t)n * d * 4, cudaMemcpyDeviceToDevice, st));
+    } else if (idx->has_pq()) {
         // one code per byte first; 4-bit codes are packed afterwards (two sub-quantizers share a
-        // byte, so the per-sub-quantizer encode launch cannot write nibbles in place)
+        // byte, so the per-sub-quantizer encode launch cannot write nibbles in place).  FastScan codes
+        // the raw vector and keeps no t-value.
+        const int M = idx->M, ksub = idx->ksub, dsub = idx->dsub;
         DevBuf unpacked;
         uint8_t* enc = (uint8_t*)prow;
         if (ksub == 16) {
             unpacked.reserve((size_t)n * M);
             enc = unpacked.as<uint8_t>();
         }
-        dim3 grid(blocks_for(n, 256), (unsigned)M);
-#define DFX_PQ_ENCODE(DS)                                                                       \
-    do {                                                                                        \
-        auto kern = pq_encode_kernel<DS>;                                                       \
-        DFX_LAUNCH(kern, grid, 256, (size_t)ksub * dsub * 4, st, d_x, idx->centroids.as<float>(), \
-                   plist, n, d, M, ksub, dsub, idx->codebooks.as<float>(), enc);                \
-    } while (0)
-        if (dsub == 2) DFX_PQ_ENCODE(2);
-        else if (dsub == 4) DFX_PQ_ENCODE(4);
-        else if (dsub == 6) DFX_PQ_ENCODE(6);  // d = 768 with M = 128
-        else if (dsub == 8) DFX_PQ_ENCODE(8);
-        else if (dsub == 16) DFX_PQ_ENCODE(16);
-        else DFX_PQ_ENCODE(0);
-#undef DFX_PQ_ENCODE
-        DFX_LAUNCH(pq_tvals_kernel<8>, blocks_for(n, 128), 128, 0, st, (const uint8_t*)enc, plist,
-                   (const int64_t*)nullptr, nlist, n, d, M, ksub, dsub, idx->codebooks.as<float>(),
-                   idx->centroids.as<float>(), idx->p_tvals.as<float>() + idx->n_pending);
+        launch_pq_encode(idx->pq_res(), d_x, idx->centroids.as<float>(), plist, n, d, M, ksub, dsub,
+                         idx->codebooks.as<float>(), enc, st);
+        if (idx->pq_res())
+            DFX_LAUNCH(pq_tvals_kernel<8>, blocks_for(n, 128), 128, 0, st, (const uint8_t*)enc, plist,
+                       (const int64_t*)nullptr, idx->cfg.nlist, n, d, M, ksub, dsub, idx->codebooks.as<float>(),
+                       idx->centroids.as<float>(), idx->p_tvals.as<float>() + idx->n_pending);
         if (ksub == 16)
             DFX_LAUNCH(pq_pack4_kernel, blocks_for(n * M / 2, 256), 256, 0, st, (const uint8_t*)enc,
                        n * M / 2, (uint8_t*)prow);
-        if (kind == DFX_IVF_PQR) {
-            // refine_codes[id] = refine_pq.encode((x - c) - PQ1(code)); the new rows get the ids
-            // ntotal .. ntotal + n - 1, their arrival order, so they append
-            const int64_t id0 = idx->ntotal();
-            if (id0 + n > idx->refine_cap) {
-                const int64_t cap = std::max<int64_t>({id0 + n, 2 * idx->refine_cap, idx->reserve_hint});
-                idx->refine_codes.reserve((size_t)cap * idx->M2, (size_t)id0 * idx->M2, st);
-                idx->refine_cap = cap;
-            }
-            DevBuf r2;
-            r2.reserve((size_t)n * d * 4);
-            DFX_LAUNCH(pq_residual2_kernel, blocks_for(n * d, 256), 256, 0, st, d_x, idx->centroids.as<float>(),
-                       (const int32_t*)plist, (const uint8_t*)enc, n, d, M, dsub, idx->codebooks.as<float>(),
-                       r2.as<float>());
-            launch_pq_encode_raw(r2.as<float>(), n, d, idx->M2, 256, idx->dsub2, idx->refine_cb.as<float>(),
-                                 idx->refine_codes.as<uint8_t>() + (size_t)id0 * idx->M2, st);
-        }
-        // (`unpacked` and `r2` are freed on return: cudaFree waits for the kernels above)
-    } else if (kind == DFX_IVF_PQ_FS) {
-        // the codes of the raw vector (no residual, no t-value), one per byte, then packed
-        const int M = idx->M, ksub = idx->ksub, dsub = idx->dsub;
-        DevBuf unpacked;
-        unpacked.reserve((size_t)n * M);
-        dim3 grid(blocks_for(n, 256), (unsigned)M);
-#define DFX_PQ_ENCODE_RAW(DS)                                                                   \
-    do {                                                                                        \
-        auto kern = pq_encode_kernel<DS, false>;                                                \
-        DFX_LAUNCH(kern, grid, 256, (size_t)ksub * dsub * 4, st, d_x, (const float*)nullptr,    \
-                   (const int32_t*)nullptr, n, d, M, ksub, dsub, idx->codebooks.as<float>(),    \
-                   unpacked.as<uint8_t>());                                                     \
-    } while (0)
-        if (dsub == 2) DFX_PQ_ENCODE_RAW(2);
-        else if (dsub == 4) DFX_PQ_ENCODE_RAW(4);
-        else if (dsub == 8) DFX_PQ_ENCODE_RAW(8);
-        else if (dsub == 16) DFX_PQ_ENCODE_RAW(16);
-        else DFX_PQ_ENCODE_RAW(0);
-#undef DFX_PQ_ENCODE_RAW
-        DFX_LAUNCH(pq_pack4_kernel, blocks_for(n * M / 2, 256), 256, 0, st, (const uint8_t*)unpacked.as<uint8_t>(),
-                   n * M / 2, (uint8_t*)prow);
+        // (`unpacked` is freed on return: cudaFree waits for the kernels above)
     } else if (kind == DFX_IVF_SQ16) {
         DFX_LAUNCH(sq_encode_kernel, blocks_for(n * d, 256), 256, 0, st, d_x, idx->centroids.as<float>(),
                    plist, n, d, (__half*)prow);
@@ -647,18 +590,59 @@ void dfx_add_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) 
         DFX_LAUNCH(sq8_encode_kernel, blocks_for(n * d, 256), 256, 0, st, d_x, idx->centroids.as<float>(),
                    plist, n, d, idx->sq_trained.as<float>(), (uint8_t*)prow);
     }
+}
+
+// rows id0 .. id0 + n - 1 of a store kept in id order next to the lists (refine_codes of IVF_PQR,
+// refine_vecs of the flat refinement), grown to refine_cap rows; returns the first of them
+static unsigned char* append_by_id(dfx_index* idx, DevBuf& store, size_t row_bytes, int64_t id0, int64_t n,
+                                   cudaStream_t st) {
+    if (id0 + n > idx->refine_cap) {
+        const int64_t cap = std::max<int64_t>({id0 + n, 2 * idx->refine_cap, idx->reserve_hint});
+        store.reserve((size_t)cap * row_bytes, (size_t)id0 * row_bytes, st);
+        idx->refine_cap = cap;
+    }
+    return store.as<unsigned char>() + (size_t)id0 * row_bytes;
+}
+
+// the stores by id: the new rows get the ids ntotal .. ntotal + n - 1, their arrival order, so they
+// append.  IVF_PQR: refine_codes[id] = refine_pq.encode((x - c) - PQ1(code)), codes1 the PQ1 codes
+// just encoded; flat refinement: the raw rows.
+static void add_by_id(dfx_index* idx, int64_t n, const float* d_x, const int32_t* plist, const uint8_t* codes1,
+                      cudaStream_t st) {
+    const int d = idx->cfg.d;
+    const int64_t id0 = idx->ntotal();
+    if (idx->cfg.kind == DFX_IVF_PQR) {
+        uint8_t* rcodes = append_by_id(idx, idx->refine_codes, (size_t)idx->M2, id0, n, st);
+        DevBuf r2;
+        r2.reserve((size_t)n * d * 4);
+        DFX_LAUNCH(pq_residual2_kernel, blocks_for(n * d, 256), 256, 0, st, d_x, idx->centroids.as<float>(), plist,
+                   codes1, n, d, idx->M, idx->dsub, idx->codebooks.as<float>(), r2.as<float>());
+        launch_pq_encode(false, r2.as<float>(), nullptr, nullptr, n, d, idx->M2, 256, idx->dsub2,
+                         idx->refine_cb.as<float>(), rcodes, st);
+        // (`r2` is freed on return: cudaFree waits for the kernels above)
+    }
     if (idx->rflat()) {
-        // the raw rows by id: the new rows get the ids ntotal .. ntotal + n - 1, so they append
-        const int64_t id0 = idx->ntotal();
         const size_t rowb = (size_t)d * 4;
-        if (id0 + n > idx->refine_cap) {
-            const int64_t cap = std::max<int64_t>({id0 + n, 2 * idx->refine_cap, idx->reserve_hint});
-            idx->refine_vecs.reserve((size_t)cap * rowb, (size_t)id0 * rowb, st);
-            idx->refine_cap = cap;
-        }
-        DFX_CUDA(cudaMemcpyAsync(idx->refine_vecs.as<unsigned char>() + (size_t)id0 * rowb, d_x, (size_t)n * rowb,
+        DFX_CUDA(cudaMemcpyAsync(append_by_id(idx, idx->refine_vecs, rowb, id0, n, st), d_x, (size_t)n * rowb,
                                  cudaMemcpyDeviceToDevice, st));
     }
+}
+
+void dfx_add_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) {
+    if (n <= 0) return;
+    DFX_REQUIRE(idx->ntotal() + n < (1ll << 31), "a shard holds at most 2^31-1 vectors");
+    if (idx->cfg.kind == DFX_FLAT) {
+        add_flat(idx, n, d_x, st);
+        return;
+    }
+    DFX_REQUIRE(idx->trained, "add: index is not trained");
+    ensure_pending(idx, idx->n_pending + n, st);
+    int32_t* plist = idx->p_list.as<int32_t>() + idx->n_pending;
+    dfx_assign_impl(idx, idx->centroids.as<float>(), idx->cnorm.as<float>(), idx->cfg.nlist, idx->cfg.metric,
+                    idx->cfg.d, n, d_x, plist, st);
+    unsigned char* prow = idx->p_payload.as<unsigned char>() + (size_t)idx->n_pending * idx->row_bytes();
+    encode_rows(idx, n, d_x, plist, prow, st);
+    add_by_id(idx, n, d_x, plist, prow, st);
     idx->n_pending += n;
 }
 
@@ -681,40 +665,18 @@ void dfx_finalize_impl(dfx_index* idx, cudaStream_t st) {
     const int64_t nlist = idx->cfg.nlist;
     const size_t rb = idx->row_bytes();
     DFX_REQUIRE(rb % 4 == 0, "row size must be a multiple of 4 bytes");
-    DevBuf keys_in, keys_out, order_in, order, cnt, off32, tmp;
-    keys_in.reserve((size_t)n * 4);
-    keys_out.reserve((size_t)n * 4);
-    order_in.reserve((size_t)n * 4);
-    order.reserve((size_t)n * 4);
-    cnt.reserve((size_t)(nlist + 1) * 4);
-    off32.reserve((size_t)(nlist + 1) * 4);
+    DevBuf keys;
+    keys.reserve((size_t)n * 4);
     if (na > 0)
         DFX_LAUNCH(expand_lists_kernel, blocks_for(na, 256), 256, 0, st, idx->list_off.as<int64_t>(),
-                   nlist, na, keys_in.as<int32_t>());
-    DFX_CUDA(cudaMemcpyAsync(keys_in.as<int32_t>() + na, idx->p_list.p, (size_t)nb * 4,
+                   nlist, na, keys.as<int32_t>());
+    DFX_CUDA(cudaMemcpyAsync(keys.as<int32_t>() + na, idx->p_list.p, (size_t)nb * 4,
                              cudaMemcpyDeviceToDevice, st));
-    DFX_LAUNCH(iota_kernel, blocks_for(n, 256), 256, 0, st, order_in.as<int32_t>(), n);
-    int bits = 1;
-    while ((1ll << bits) < nlist) bits++;
-    size_t tmp_sort = 0, tmp_scan = 0;
-    cub::DeviceRadixSort::SortPairs(nullptr, tmp_sort, keys_in.as<int32_t>(), keys_out.as<int32_t>(),
-                                    order_in.as<int32_t>(), order.as<int32_t>(), (int)n, 0, bits, st);
-    cub::DeviceScan::ExclusiveSum(nullptr, tmp_scan, cnt.as<int32_t>(), off32.as<int32_t>(),
-                                  (int)(nlist + 1), st);
-    tmp.reserve(std::max(tmp_sort, tmp_scan));
-    size_t tb = tmp.cap;
-    DFX_CUDA(cub::DeviceRadixSort::SortPairs(tmp.p, tb, keys_in.as<int32_t>(), keys_out.as<int32_t>(),
-                                             order_in.as<int32_t>(), order.as<int32_t>(), (int)n, 0,
-                                             bits, st));
-    DFX_CUDA(cudaMemsetAsync(cnt.p, 0, (size_t)(nlist + 1) * 4, st));
-    DFX_LAUNCH(count_kernel, blocks_for(n, 256), 256, 0, st, keys_in.as<int32_t>(), n, cnt.as<int32_t>());
-    tb = tmp.cap;
-    DFX_CUDA(cub::DeviceScan::ExclusiveSum(tmp.p, tb, cnt.as<int32_t>(), off32.as<int32_t>(),
-                                           (int)(nlist + 1), st));
-    g_dfx_launches.fetch_add(2, std::memory_order_relaxed);
-    keys_in.release();
-    keys_out.release();
-    order_in.release();
+    KeyBuckets b(n, nlist, st);
+    b.run(keys.as<int32_t>(), st);
+    keys.release();
+    b.keys_out.release();
+    b.order_in.release();
 
     // gather into fresh list-sorted storage
     DevBuf new_payload, new_ids, new_tvals;
@@ -722,17 +684,17 @@ void dfx_finalize_impl(dfx_index* idx, cudaStream_t st) {
     new_ids.reserve((size_t)n * 4);
     const int words = (int)(rb / 4);
     DFX_LAUNCH(gather_words_kernel, blocks_for(n * words, 256), 256, 0, st, idx->payload.as<uint32_t>(),
-               idx->p_payload.as<uint32_t>(), na, order.as<int32_t>(), n, words,
+               idx->p_payload.as<uint32_t>(), na, b.order.as<int32_t>(), n, words,
                new_payload.as<uint32_t>());
     DFX_LAUNCH(gather_ids_kernel, blocks_for(n, 256), 256, 0, st, idx->ids.as<int32_t>(), na,
-               order.as<int32_t>(), n, new_ids.as<int32_t>());
+               b.order.as<int32_t>(), n, new_ids.as<int32_t>());
     if (idx->pq_res()) {
         new_tvals.reserve((size_t)n * 4);
         DFX_LAUNCH(gather_words_kernel, blocks_for(n, 256), 256, 0, st, idx->tvals.as<uint32_t>(),
-                   idx->p_tvals.as<uint32_t>(), na, order.as<int32_t>(), n, 1, new_tvals.as<uint32_t>());
+                   idx->p_tvals.as<uint32_t>(), na, b.order.as<int32_t>(), n, 1, new_tvals.as<uint32_t>());
     }
     idx->list_off.reserve((size_t)(nlist + 1) * 8);
-    DFX_LAUNCH(widen_kernel, blocks_for(nlist + 1, 256), 256, 0, st, off32.as<int32_t>(), nlist + 1,
+    DFX_LAUNCH(widen_kernel, blocks_for(nlist + 1, 256), 256, 0, st, b.off.as<int32_t>(), nlist + 1,
                idx->list_off.as<int64_t>());
     idx->h_list_off.resize((size_t)nlist + 1);
     DFX_CUDA(cudaMemcpyAsync(idx->h_list_off.data(), idx->list_off.p, (size_t)(nlist + 1) * 8,
@@ -748,9 +710,9 @@ void dfx_finalize_impl(dfx_index* idx, cudaStream_t st) {
     idx->p_cap = 0;
     idx->n_sorted = n;
     idx->n_pending = 0;
-    idx->inv_valid = false;
-    dfx_pq_rm_to_il(idx, st);  // IVF-PQ, M == 32: interleaved blocks for the scan (no-op otherwise)
-    if (idx->cfg.kind == DFX_IVF_PQR) dfx_refresh_inv(idx, st);
+    // IVF-PQ, M == 32: interleaved blocks for the scan, a layout change of its own
+    if (dfx_il_wanted(idx)) dfx_pq_rm_to_il(idx, st);
+    else dfx_layout_changed(idx, st);
 }
 
 // ------------------------------------------------------------------ reconstruct
@@ -759,117 +721,92 @@ __global__ void invert_ids_kernel(const int32_t* __restrict__ ids, int64_t n, in
     if (i < n && ids[i] >= 0) inv[ids[i]] = (int32_t)i;
 }
 
-// il != 0 (IVF-PQ interleaved, il = block layout 1 or 2): `inv` holds padded block positions and
-// codes are read from the interleaved blocks (dfx_il_byte_of(il, pos%32, m) of block pos/32).
-// NB = bits per stored IVF-PQ code of the row-major form (dfx_pq_code).
-template <int NB>
-__global__ void reconstruct_kernel(int kind, int d, int M, int ksub, int dsub, int64_t ntotal,
-                                   int64_t nlist, const int64_t* __restrict__ want,
-                                   const int32_t* __restrict__ inv, const void* __restrict__ rows,
-                                   const int64_t* __restrict__ list_off, const float* __restrict__ cent,
-                                   const float* __restrict__ codebooks, int il,
-                                   const int64_t* __restrict__ blk_off, float* __restrict__ out,
-                                   int64_t tag) {
-    const int64_t r = blockIdx.x;
-    int64_t id = want[r];
-    if (tag >= 0) {
-        // exchange ids ((shard tag << 40) | local id, see encode_ids_kernel): decode only the rows
-        // this shard owns and leave every other row of `out` untouched
-        if (id < 0 || ((id >> 40) & 0xfffff) != tag) return;
-        id &= (1ll << 40) - 1;
-    }
-    if (id < 0 || id >= ntotal) {
-        for (int k = threadIdx.x; k < d; k += blockDim.x) out[r * d + k] = __int_as_float(0x7fc00000);
-        return;
-    }
-    const int64_t pos = (kind == DFX_FLAT) ? id : inv[id];
-    int64_t l = 0;
-    if (kind == DFX_IVF_PQ || kind == DFX_IVF_SQ16) {
-        const int64_t* off = il ? blk_off : list_off;
-        const int64_t key = il ? (pos >> 5) : pos;
-        int64_t lo = 0, hi = nlist;
-        while (hi - lo > 1) {
-            int64_t mid = (lo + hi) >> 1;
-            if (off[mid] <= key) lo = mid; else hi = mid;
-        }
-        l = lo;
-    }
-    for (int k = threadIdx.x; k < d; k += blockDim.x) {
-        float v;
-        if (kind == DFX_FLAT || kind == DFX_IVF_FLAT) {
-            v = reinterpret_cast<const float*>(rows)[pos * d + k];
-        } else if (kind == DFX_IVF_SQ16) {
-            v = cent[(size_t)l * d + k] + __half2float(reinterpret_cast<const __half*>(rows)[pos * d + k]);
-        } else {
-            int m = k / dsub;
-            int code;
-            if (il) code = reinterpret_cast<const uint8_t*>(rows)[(pos >> 5) * 1024 + dfx_il_byte_of(il, (int)(pos & 31), m)];
-            else code = dfx_pq_code<NB>(reinterpret_cast<const uint8_t*>(rows), pos, M, m);
-            v = cent[(size_t)l * d + k] + codebooks[((size_t)m * ksub + code) * dsub + (k - m * dsub)];
-        }
-        out[r * d + k] = v;
-    }
-}
+// Row decoders of reconstruct_kernel: dec(k, id, pos, l) is component k of the vector with local id
+// `id`, stored at position pos of list l.  kFrom is what the kernel looks up first: Id, rows
+// addressed by id (pos = id); Pos, the storage position pos = inv[id]; List, also the list l that
+// holds it (the decoders that add the list's centroid).
+enum class RowFrom { Id, Pos, List };
 
-// IVF-SQ8: centroid + decoded residual (the decode of the list scan, DESIGN.md section 2).  Ids as
-// reconstruct_kernel: tag < 0 local ids (unknown / -1 -> NaN row), tag >= 0 exchange ids.
-__global__ void sq8_reconstruct_kernel(int d, int64_t ntotal, int64_t nlist, const int64_t* __restrict__ want,
-                                       const int32_t* __restrict__ inv, const uint8_t* __restrict__ codes,
-                                       const int64_t* __restrict__ list_off, const float* __restrict__ cent,
-                                       const float* __restrict__ trained, float* __restrict__ out, int64_t tag) {
-    const int64_t r = blockIdx.x;
-    int64_t id = want[r];
-    if (tag >= 0) {
-        if (id < 0 || ((id >> 40) & 0xfffff) != tag) return;
-        id &= (1ll << 40) - 1;
+template <RowFrom FROM>
+struct RowsDec {  // FLAT and the flat refinement (by id), IVF_FLAT (by position): the stored row
+    static constexpr RowFrom kFrom = FROM;
+    const float* rows;
+    int d;
+    __device__ float operator()(int k, int64_t, int64_t pos, int64_t) const { return rows[pos * d + k]; }
+};
+
+struct Sq16Dec {  // IVF_SQ16: c + r in fp16
+    static constexpr RowFrom kFrom = RowFrom::List;
+    const __half* codes;
+    const float* cent;
+    int d;
+    __device__ float operator()(int k, int64_t, int64_t pos, int64_t l) const {
+        return cent[(size_t)l * d + k] + __half2float(codes[pos * d + k]);
     }
-    if (id < 0 || id >= ntotal) {
-        for (int k = threadIdx.x; k < d; k += blockDim.x) out[r * d + k] = __int_as_float(0x7fc00000);
-        return;
-    }
-    const int64_t pos = inv[id];
-    int64_t lo = 0, hi = nlist;
-    while (hi - lo > 1) {
-        int64_t mid = (lo + hi) >> 1;
-        if (list_off[mid] <= pos) lo = mid; else hi = mid;
-    }
-    for (int k = threadIdx.x; k < d; k += blockDim.x) {
+};
+
+struct Sq8Dec {  // IVF_SQ8: c + the decode of the list scan (DESIGN.md section 2)
+    static constexpr RowFrom kFrom = RowFrom::List;
+    const uint8_t* codes;
+    const float* cent;
+    const float* trained;
+    int d;
+    __device__ float operator()(int k, int64_t, int64_t pos, int64_t l) const {
         const float t = __fmaf_rn((float)codes[pos * d + k], DFX_SQ8_SCALE, DFX_SQ8_BIAS);
-        out[r * d + k] = cent[(size_t)lo * d + k] + __fmaf_rn(t, trained[d + k], trained[k]);
+        return cent[(size_t)l * d + k] + __fmaf_rn(t, trained[d + k], trained[k]);
     }
-}
+};
 
-// IVF-PQ FastScan: x_m = P[m][code_m], no centroid (the codes are of the raw vector).  Ids as
-// reconstruct_kernel.
-__global__ void pq_fs_reconstruct_kernel(int d, int M, int dsub, int64_t ntotal, const int64_t* __restrict__ want,
-                                         const int32_t* __restrict__ inv, const uint8_t* __restrict__ codes,
-                                         const float* __restrict__ codebooks, float* __restrict__ out, int64_t tag) {
-    const int64_t r = blockIdx.x;
-    int64_t id = want[r];
-    if (tag >= 0) {
-        if (id < 0 || ((id >> 40) & 0xfffff) != tag) return;
-        id &= (1ll << 40) - 1;
-    }
-    if (id < 0 || id >= ntotal) {
-        for (int k = threadIdx.x; k < d; k += blockDim.x) out[r * d + k] = __int_as_float(0x7fc00000);
-        return;
-    }
-    const int64_t pos = inv[id];
-    for (int k = threadIdx.x; k < d; k += blockDim.x) {
+// IVF_PQ: c + P[m][code_m].  NB = bits per code of the row-major form (dfx_pq_code); il != 0: the
+// codes are the interleaved blocks (dfx_il2_byte of block pos / 32) and pos a padded block position.
+template <int NB>
+struct PqDec {
+    static constexpr RowFrom kFrom = RowFrom::List;
+    const uint8_t* codes;
+    const float* cent;
+    const float* codebooks;
+    int d, M, ksub, dsub, il;
+    __device__ float operator()(int k, int64_t, int64_t pos, int64_t l) const {
         const int m = k / dsub;
-        out[r * d + k] = codebooks[((size_t)m * 16 + dfx_pq_code<4>(codes, pos, M, m)) * dsub + (k - m * dsub)];
+        const int code = il ? codes[(pos >> 5) * 1024 + dfx_il2_byte((int)(pos & 31), m)]
+                            : dfx_pq_code<NB>(codes, pos, M, m);
+        return cent[(size_t)l * d + k] + codebooks[((size_t)m * ksub + code) * dsub + (k - m * dsub)];
     }
-}
+};
 
-// IVF-PQR: (c + P1[m][code_m]) + P2[m2][refine_code_m2], the reconstruction of faiss's
-// IndexIVFPQR.  Ids as reconstruct_kernel; il != 0: `inv` holds padded block positions, `off` is
-// blk_off and the codes are the interleaved blocks, else `off` is list_off.
-__global__ void pqr_reconstruct_kernel(int d, int M, int dsub, int M2, int dsub2, int64_t ntotal, int64_t nlist,
-                                       const int64_t* __restrict__ want, const int32_t* __restrict__ inv,
-                                       const uint8_t* __restrict__ codes, int il, const int64_t* __restrict__ off,
-                                       const float* __restrict__ cent, const float* __restrict__ codebooks,
-                                       const uint8_t* __restrict__ rcodes, const float* __restrict__ rcb,
-                                       float* __restrict__ out, int64_t tag) {
+struct PqFsDec {  // IVF_PQ_FS: P[m][code_m], no centroid (the codes are of the raw vector)
+    static constexpr RowFrom kFrom = RowFrom::Pos;
+    const uint8_t* codes;
+    const float* codebooks;
+    int M, dsub;
+    __device__ float operator()(int k, int64_t, int64_t pos, int64_t) const {
+        const int m = k / dsub;
+        return codebooks[((size_t)m * 16 + dfx_pq_code<4>(codes, pos, M, m)) * dsub + (k - m * dsub)];
+    }
+};
+
+// IVF_PQR: (c + P1[m][code_m]) + P2[m2][refine_code_m2], the reconstruction of faiss's IndexIVFPQR;
+// the refinement codes are stored by id
+struct PqrDec {
+    static constexpr RowFrom kFrom = RowFrom::List;
+    PqDec<8> pq1;
+    const uint8_t* rcodes;
+    const float* rcb;
+    int M2, dsub2;
+    __device__ float operator()(int k, int64_t id, int64_t pos, int64_t l) const {
+        const int m2 = k / dsub2;
+        return pq1(k, id, pos, l) + rcb[((size_t)m2 * 256 + rcodes[id * M2 + m2]) * dsub2 + (k - m2 * dsub2)];
+    }
+};
+
+// One CTA per wanted id.  tag < 0: local ids, an unknown one (-1, >= ntotal) gives a NaN row.
+// tag >= 0: exchange ids ((shard tag << 40) | local id, see encode_ids_kernel), only the rows this
+// shard owns are decoded and every other row of `out` is left untouched.  `off` holds the list
+// offsets, or with il != 0 the block offsets (then inv holds padded block positions).
+template <class Dec>
+__global__ void reconstruct_kernel(Dec dec, int d, int64_t ntotal, int64_t nlist, const int64_t* __restrict__ want,
+                                   const int32_t* __restrict__ inv, const int64_t* __restrict__ off, int il,
+                                   float* __restrict__ out, int64_t tag) {
     const int64_t r = blockIdx.x;
     int64_t id = want[r];
     if (tag >= 0) {
@@ -880,20 +817,9 @@ __global__ void pqr_reconstruct_kernel(int d, int M, int dsub, int M2, int dsub2
         for (int k = threadIdx.x; k < d; k += blockDim.x) out[r * d + k] = __int_as_float(0x7fc00000);
         return;
     }
-    const int64_t pos = inv[id];
-    const int64_t key = il ? (pos >> 5) : pos;
-    int64_t lo = 0, hi = nlist;
-    while (hi - lo > 1) {
-        int64_t mid = (lo + hi) >> 1;
-        if (off[mid] <= key) lo = mid; else hi = mid;
-    }
-    for (int k = threadIdx.x; k < d; k += blockDim.x) {
-        const int m = k / dsub, m2 = k / dsub2;
-        const int code = il ? codes[(pos >> 5) * 1024 + dfx_il2_byte((int)(pos & 31), m)] : codes[pos * M + m];
-        const float p1 = codebooks[((size_t)m * 256 + code) * dsub + (k - m * dsub)];
-        const float p2 = rcb[((size_t)m2 * 256 + rcodes[id * M2 + m2]) * dsub2 + (k - m2 * dsub2)];
-        out[r * d + k] = (cent[(size_t)lo * d + k] + p1) + p2;
-    }
+    const int64_t pos = Dec::kFrom == RowFrom::Id ? id : inv[id];
+    const int64_t l = Dec::kFrom == RowFrom::List ? dfx_list_of(off, nlist, il ? pos >> 5 : pos) : 0;
+    for (int k = threadIdx.x; k < d; k += blockDim.x) out[r * d + k] = dec(k, id, pos, l);
 }
 
 void dfx_refresh_inv(dfx_index* idx, cudaStream_t st) {
@@ -908,43 +834,39 @@ void dfx_refresh_inv(dfx_index* idx, cudaStream_t st) {
     idx->inv_valid = true;
 }
 
+void dfx_layout_changed(dfx_index* idx, cudaStream_t st) {
+    idx->inv_valid = false;
+    if (idx->cfg.kind == DFX_IVF_PQR) dfx_refresh_inv(idx, st);
+}
+
 void dfx_reconstruct_impl(dfx_index* idx, int64_t n, const int64_t* d_ids, float* d_out,
                           cudaStream_t st, int64_t tag) {
     if (n <= 0) return;
     if (idx->n_pending > 0) dfx_finalize_impl(idx, st);
-    const int64_t nt = idx->n_sorted;
+    const int d = idx->cfg.d, M = idx->M, ksub = idx->ksub, dsub = idx->dsub;
     const int il = idx->il ? 2 : 0;  // 0 = row-major, else the block layout
-    if (idx->rflat()) {
-        // the stored row, addressed by id as a FLAT index addresses its rows
-        DFX_LAUNCH(reconstruct_kernel<8>, (unsigned)n, 128, 0, st, (int)DFX_FLAT, idx->cfg.d, 0, 0, 0, nt,
-                   (int64_t)0, d_ids, (const int32_t*)nullptr, (const void*)idx->refine_vecs.p,
-                   (const int64_t*)nullptr, (const float*)nullptr, (const float*)nullptr, 0,
-                   (const int64_t*)nullptr, d_out, tag);
-        return;
-    }
+    const uint8_t* codes = il ? idx->il_codes.as<uint8_t>() : idx->payload.as<uint8_t>();
+    const float* cent = idx->centroids.as<float>();
+    const float* cb = idx->codebooks.as<float>();
+    auto run = [&](auto dec) {
+        DFX_LAUNCH(reconstruct_kernel<decltype(dec)>, (unsigned)n, 128, 0, st, dec, d, idx->n_sorted, idx->cfg.nlist,
+                   d_ids, idx->inv.as<int32_t>(), il ? idx->blk_off.as<int64_t>() : idx->list_off.as<int64_t>(), il,
+                   d_out, tag);
+    };
+    // flat refinement: the stored row, addressed by id as a FLAT index addresses its rows
+    if (idx->rflat()) return run(RowsDec<RowFrom::Id>{idx->refine_vecs.as<float>(), d});
     dfx_refresh_inv(idx, st);
-    if (idx->cfg.kind == DFX_IVF_PQR) {
-        DFX_LAUNCH(pqr_reconstruct_kernel, (unsigned)n, 128, 0, st, idx->cfg.d, idx->M, idx->dsub, idx->M2, idx->dsub2,
-                   nt, idx->cfg.nlist, d_ids, idx->inv.as<int32_t>(),
-                   il ? (const uint8_t*)idx->il_codes.p : (const uint8_t*)idx->payload.p, il,
-                   il ? idx->blk_off.as<int64_t>() : idx->list_off.as<int64_t>(), idx->centroids.as<float>(),
-                   idx->codebooks.as<float>(), idx->refine_codes.as<uint8_t>(), idx->refine_cb.as<float>(), d_out, tag);
-        return;
+    switch (idx->cfg.kind) {
+        case DFX_FLAT: return run(RowsDec<RowFrom::Id>{idx->payload.as<float>(), d});
+        case DFX_IVF_FLAT: return run(RowsDec<RowFrom::Pos>{idx->payload.as<float>(), d});
+        case DFX_IVF_SQ16: return run(Sq16Dec{idx->payload.as<__half>(), cent, d});
+        case DFX_IVF_SQ8: return run(Sq8Dec{idx->payload.as<uint8_t>(), cent, idx->sq_trained.as<float>(), d});
+        case DFX_IVF_PQ:
+            if (ksub == 16) return run(PqDec<4>{codes, cent, cb, d, M, ksub, dsub, il});
+            return run(PqDec<8>{codes, cent, cb, d, M, ksub, dsub, il});
+        case DFX_IVF_PQ_FS: return run(PqFsDec{idx->payload.as<uint8_t>(), cb, M, dsub});
+        case DFX_IVF_PQR:
+            return run(PqrDec{PqDec<8>{codes, cent, cb, d, M, ksub, dsub, il}, idx->refine_codes.as<uint8_t>(),
+                              idx->refine_cb.as<float>(), idx->M2, idx->dsub2});
     }
-    if (idx->cfg.kind == DFX_IVF_SQ8) {
-        DFX_LAUNCH(sq8_reconstruct_kernel, (unsigned)n, 128, 0, st, idx->cfg.d, nt, idx->cfg.nlist, d_ids,
-                   idx->inv.as<int32_t>(), idx->payload.as<uint8_t>(), idx->list_off.as<int64_t>(),
-                   idx->centroids.as<float>(), idx->sq_trained.as<float>(), d_out, tag);
-        return;
-    }
-    if (idx->cfg.kind == DFX_IVF_PQ_FS) {
-        DFX_LAUNCH(pq_fs_reconstruct_kernel, (unsigned)n, 128, 0, st, idx->cfg.d, idx->M, idx->dsub, nt, d_ids,
-                   idx->inv.as<int32_t>(), idx->payload.as<uint8_t>(), idx->codebooks.as<float>(), d_out, tag);
-        return;
-    }
-    auto kern = (idx->cfg.kind == DFX_IVF_PQ && idx->ksub == 16) ? reconstruct_kernel<4> : reconstruct_kernel<8>;
-    DFX_LAUNCH(kern, (unsigned)n, 128, 0, st, idx->cfg.kind, idx->cfg.d, idx->M, idx->ksub,
-               idx->dsub, nt, idx->cfg.nlist, d_ids, idx->inv.as<int32_t>(),
-               il ? (const void*)idx->il_codes.p : (const void*)idx->payload.p, idx->list_off.as<int64_t>(),
-               idx->centroids.as<float>(), idx->codebooks.as<float>(), il, idx->blk_off.as<int64_t>(), d_out, tag);
 }

@@ -191,6 +191,18 @@ __device__ __forceinline__ int dfx_pq_code(const uint8_t* codes, int64_t i, int 
     else return codes[i * M + m];
 }
 
+// the list l with off[l] <= key < off[l + 1] (binary search over off[0..nlist]): the list that holds
+// position key of list-sorted storage (off = list_off), or block key of the interleaved storage
+// (off = blk_off)
+__device__ __forceinline__ int64_t dfx_list_of(const int64_t* __restrict__ off, int64_t nlist, int64_t key) {
+    int64_t lo = 0, hi = nlist;
+    while (hi - lo > 1) {
+        int64_t mid = (lo + hi) >> 1;
+        if (off[mid] <= key) lo = mid; else hi = mid;
+    }
+    return lo;
+}
+
 static inline int64_t dfx_ceil_div(int64_t a, int64_t b) { return (a + b - 1) / b; }
 static inline int dfx_next_pow2(int x) {
     int p = 1;

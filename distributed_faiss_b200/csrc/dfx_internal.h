@@ -6,6 +6,8 @@
 #include <mutex>
 #include <memory>
 #include <algorithm>
+#include <utility>
+#include <type_traits>
 
 // streaming multiprocessors of the current device (launch shapes are sized in waves over them)
 int dfx_num_sms();
@@ -57,6 +59,14 @@ struct dfx_event_ranges {
         }
     }
 };
+
+// A runtime value as a template argument: calls f(std::integral_constant<int, V>{}) for the V of
+// the list that equals v, and returns false when none does.  Every V of the list is instantiated.
+template <int... Vs> using IntList = std::integer_sequence<int, Vs...>;
+template <int... Vs, class F>
+static bool dispatch_int(IntList<Vs...>, int v, F&& f) {
+    return ((v == Vs && (f(std::integral_constant<int, Vs>{}), true)) || ...);
+}
 
 struct dfx_index {
     dfx_cfg cfg{};
@@ -302,5 +312,9 @@ void dfx_assign_impl(dfx_index* idx, const float* d_cent, const float* d_cnorm, 
 void dfx_compute_tvals_sorted(dfx_index* idx, cudaStream_t st);
 // `inv` (shard-local id -> storage position, padded block position when interleaved) for the
 // current layout; a no-op while it is valid.  IVF_PQR searches read it, so every change of the
-// layout rebuilds it right away (finalize, import, the interleaved conversions).
+// layout rebuilds it right away (dfx_layout_changed; import).
 void dfx_refresh_inv(dfx_index* idx, cudaStream_t st);
+// after every change of the storage layout (train, finalize, the interleaved conversions): `inv` is
+// stale, and an IVF_PQR shard rebuilds it at once, so a search captured into a CUDA graph depends on
+// no host flag
+void dfx_layout_changed(dfx_index* idx, cudaStream_t st);

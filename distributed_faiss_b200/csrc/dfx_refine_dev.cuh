@@ -32,14 +32,9 @@ pqr_refine_kernel(const float* __restrict__ xq, int d, int64_t ncand, int k1, co
         return;
     }
     const int64_t pos = inv[id];
-    const int64_t key = il ? (pos >> 5) : pos;
-    int64_t lo = 0, hi = nlist;
-    while (hi - lo > 1) {
-        const int64_t mid = (lo + hi) >> 1;
-        if (off[mid] <= key) lo = mid; else hi = mid;
-    }
+    const int64_t l = dfx_list_of(off, nlist, il ? (pos >> 5) : pos);
     const float* q = xq + (c / k1) * d;
-    const float* cl = cent + lo * d;
+    const float* cl = cent + l * d;
     const uint8_t* rc = rcodes + id * M2;
     float acc = 0.f;
     for (int base = 4 * lane; base < d; base += 128) {

@@ -33,8 +33,7 @@ void dfx_pq_rm_to_il(dfx_index* idx, cudaStream_t st) {
     idx->ids.release();
     idx->nblk = nblk;
     idx->il = true;
-    idx->inv_valid = false;
-    if (idx->cfg.kind == DFX_IVF_PQR) dfx_refresh_inv(idx, st);
+    dfx_layout_changed(idx, st);
 }
 
 // il_* -> payload/tvals/ids (row-major); frees the interleaved arrays
@@ -55,7 +54,6 @@ void dfx_pq_il_to_rm(dfx_index* idx, cudaStream_t st) {
     idx->il_ids.release();
     idx->nblk = 0;
     idx->il = false;
-    idx->inv_valid = false;
-    if (idx->cfg.kind == DFX_IVF_PQR) dfx_refresh_inv(idx, st);
+    dfx_layout_changed(idx, st);
 }
 

@@ -9,15 +9,6 @@
 #include "dfx_ptx.cuh"
 
 // ------------------------------------------------------------------ layout conversion
-__device__ __forceinline__ int64_t il_list_of_block(const int64_t* __restrict__ blk_off, int64_t nlist, int64_t blk) {
-    int64_t lo = 0, hi = nlist;
-    while (hi - lo > 1) {
-        int64_t mid = (lo + hi) >> 1;
-        if (blk_off[mid] <= blk) lo = mid; else hi = mid;
-    }
-    return lo;
-}
-
 // row-major (list-sorted) -> interleaved blocks.  one CTA per block.
 __global__ void __launch_bounds__(256)
 pq_rm_to_il_kernel(const int64_t* __restrict__ list_off, const int64_t* __restrict__ blk_off, int64_t nlist,
@@ -25,7 +16,7 @@ pq_rm_to_il_kernel(const int64_t* __restrict__ list_off, const int64_t* __restri
                    const int32_t* __restrict__ ids, uint8_t* __restrict__ il_codes, float* __restrict__ il_tvals,
                    int32_t* __restrict__ il_ids) {
     const int64_t blk = blockIdx.x;
-    const int64_t l = il_list_of_block(blk_off, nlist, blk);
+    const int64_t l = dfx_list_of(blk_off, nlist, blk);
     const int64_t base = list_off[l] + (blk - blk_off[l]) * 32, end = list_off[l + 1];
     for (int e = threadIdx.x; e < 1024; e += 256) {
         const int v = e >> 5, m = e & 31;
@@ -45,7 +36,7 @@ pq_il_to_rm_kernel(const int64_t* __restrict__ list_off, const int64_t* __restri
                    const int32_t* __restrict__ il_ids, uint8_t* __restrict__ codes, float* __restrict__ tvals,
                    int32_t* __restrict__ ids) {
     const int64_t blk = blockIdx.x;
-    const int64_t l = il_list_of_block(blk_off, nlist, blk);
+    const int64_t l = dfx_list_of(blk_off, nlist, blk);
     const int64_t base = list_off[l] + (blk - blk_off[l]) * 32, end = list_off[l + 1];
     for (int e = threadIdx.x; e < 1024; e += 256) {
         const int v = e >> 5, m = e & 31;

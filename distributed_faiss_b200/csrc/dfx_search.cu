@@ -937,13 +937,6 @@ static IvfPlan plan_ivf(dfx_index* idx, int64_t nq, int64_t k64) {
     return p;
 }
 
-// A runtime value as a template argument: calls f(std::integral_constant<int, V>{}) for the V of
-// the list that equals v, and returns false when none does.  Every V of the list is instantiated.
-template <int... Vs> using IntList = std::integer_sequence<int, Vs...>;
-template <int... Vs, class F>
-static bool dispatch_int(IntList<Vs...>, int v, F&& f) {
-    return ((v == Vs && (f(std::integral_constant<int, Vs>{}), true)) || ...);
-}
 // M of the 4-bit and FastScan scans: a multiple of 8 in [8, 128] (checked by dfx_create)
 using PqMByEight = IntList<8, 16, 24, 32, 40, 48, 56, 64, 72, 80, 88, 96, 104, 112, 120, 128>;
 
