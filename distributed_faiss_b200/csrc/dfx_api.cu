@@ -523,17 +523,59 @@ int dfx_profile_read(dfx_index* idx, double* scan_ms, int64_t* scan_launches, in
 }
 
 // ------------------------------------------------------------------ state exchange
-static const char* payload_name(int kind) {
-    switch (kind) {
-        case DFX_FLAT: return "xb";
-        case DFX_IVF_FLAT: return "vecs";
-        case DFX_IVF_PQ: return "codes";
-        case DFX_IVF_SQ16: return "codes16";
-        case DFX_IVF_SQ8: return "codes8";
-        case DFX_IVF_PQ_FS: return "codes";
-        case DFX_IVF_PQR: return "codes";
-    }
-    return "";
+// How an array travels between the host and its device buffer: as it is, or converted on the host
+// (ids: int64 exchanged, int32 stored; 4-bit codes: one per byte exchanged, two per byte stored)
+enum class ExchangeConv { none, ids32, codes4 };
+
+struct ExchangeArray {
+    const char* name;
+    DevBuf* buf;
+    ExchangeConv conv;
+    int64_t bytes;        // exchange size; a converted array is stored in bytes / 2
+    bool needs_trained;   // dfx_get_array has it only once the index is trained
+    bool importable;      // dfx_set_array accepts it
+    const char* size_error;
+};
+
+// The arrays of the exchange format (include/dfx.h) that this index has, in import order, sized for
+// the n_sorted vectors of the list-sorted storage
+static std::vector<ExchangeArray> exchange_arrays(dfx_index* idx) {
+    using C = ExchangeConv;
+    const int kind = idx->cfg.kind;
+    const int64_t n = idx->n_sorted, nlist = idx->cfg.nlist, d = idx->cfg.d, M = idx->M, M2 = idx->M2;
+    if (kind == DFX_FLAT) return {{"xb", &idx->payload, C::none, n * d * 4, false, true, "xb: wrong size"}};
+    std::vector<ExchangeArray> a{{"centroids", &idx->centroids, C::none, nlist * d * 4, true, true, "centroids: wrong size"}};
+    if (idx->has_pq())
+        a.push_back({"codebooks", &idx->codebooks, C::none, M * idx->ksub * idx->dsub * 4, true, true, "codebooks: wrong size"});
+    if (kind == DFX_IVF_SQ8)
+        a.push_back({"sq_trained", &idx->sq_trained, C::none, 2 * d * 4, true, true,
+                     "sq_trained: wrong size (2 * d floats: vmin, then vdiff)"});
+    if (kind == DFX_IVF_PQR)
+        a.push_back({"refine_codebooks", &idx->refine_cb, C::none, M2 * 256 * idx->dsub2 * 4, true, true,
+                     "refine_codebooks: wrong size"});
+    a.push_back({"list_off", &idx->list_off, C::none, (nlist + 1) * 8, true, true, "list_off: wrong size"});
+    a.push_back({"ids", &idx->ids, C::ids32, n * 8, false, true, "ids: wrong size (set list_off first)"});
+    if (idx->has_pq() && idx->ksub == 16)
+        a.push_back({"codes", &idx->payload, C::codes4, n * M, false, true,
+                     "codes: wrong size (one byte per code, u8[ntotal, M]; set list_off first)"});
+    else
+        a.push_back({kind == DFX_IVF_FLAT ? "vecs" : kind == DFX_IVF_SQ16 ? "codes16" : kind == DFX_IVF_SQ8 ? "codes8" : "codes",
+                     &idx->payload, C::none, n * (int64_t)idx->row_bytes(), false, true,
+                     "payload: wrong size (set list_off first)"});
+    if (idx->pq_res()) a.push_back({"tvals", &idx->tvals, C::none, n * 4, false, false, nullptr});  // recomputed on import
+    if (kind == DFX_IVF_PQR)
+        a.push_back({"refine_codes", &idx->refine_codes, C::none, n * M2, false, true,
+                     "refine_codes: wrong size (u8[ntotal, M2] in id order; set list_off first)"});
+    if (idx->rflat())
+        a.push_back({"refine_vecs", &idx->refine_vecs, C::none, n * d * 4, false, true,
+                     "refine_vecs: wrong size (f32[ntotal, d] in id order; set list_off first)"});
+    return a;
+}
+
+static const ExchangeArray* find_exchange_array(const std::vector<ExchangeArray>& arrays, const std::string& n) {
+    for (const ExchangeArray& a : arrays)
+        if (n == a.name) return &a;
+    return nullptr;
 }
 
 int dfx_get_array(dfx_index* idx, const char* name, void* out, int64_t max_bytes, int64_t* nbytes) {
@@ -559,43 +601,28 @@ int dfx_get_array(dfx_index* idx, const char* name, void* out, int64_t max_bytes
         dfx_pq_il_to_rm(idx, idx->stream);
         restore.on = true;
     }
-    const int64_t nt = idx->n_sorted, nlist = idx->cfg.nlist, d = idx->cfg.d;
-    const void* src = nullptr;
-    int64_t bytes = 0;
-    bool widen_ids = false;
-    // 4-bit IVF-PQ codes are stored packed (two per byte) and exchanged one code per byte
-    const bool unpack4 = n == "codes" && idx->has_pq() && idx->ksub == 16;
-    if (n == "centroids" && idx->is_ivf() && idx->trained) { src = idx->centroids.p; bytes = nlist * d * 4; }
-    else if (n == "codebooks" && idx->has_pq() && idx->trained) { src = idx->codebooks.p; bytes = (int64_t)idx->M * idx->ksub * idx->dsub * 4; }
-    else if (n == "sq_trained" && idx->cfg.kind == DFX_IVF_SQ8 && idx->trained) { src = idx->sq_trained.p; bytes = 2 * d * 4; }
-    else if (n == "list_off" && idx->is_ivf() && idx->trained) { src = idx->list_off.p; bytes = (nlist + 1) * 8; }
-    else if (n == "ids" && idx->is_ivf()) { widen_ids = true; bytes = nt * 8; }
-    else if (n == "tvals" && idx->pq_res()) { src = idx->tvals.p; bytes = nt * 4; }
-    else if (n == "refine_codebooks" && idx->cfg.kind == DFX_IVF_PQR && idx->trained) { src = idx->refine_cb.p; bytes = (int64_t)idx->M2 * 256 * idx->dsub2 * 4; }
-    else if (n == "refine_codes" && idx->cfg.kind == DFX_IVF_PQR) { src = idx->refine_codes.p; bytes = nt * idx->M2; }
-    else if (n == "refine_vecs" && idx->rflat()) { src = idx->refine_vecs.p; bytes = nt * d * 4; }
-    else if (unpack4) { bytes = nt * idx->M; }
-    else if (n == payload_name(idx->cfg.kind)) { src = idx->payload.p; bytes = nt * (int64_t)idx->row_bytes(); }
-    else throw DfxError{"no array named '" + n + "' in this index"};
+    const std::vector<ExchangeArray> arrays = exchange_arrays(idx);
+    const ExchangeArray* a = find_exchange_array(arrays, n);
+    if (!a || (a->needs_trained && !idx->trained)) throw DfxError{"no array named '" + n + "' in this index"};
+    const int64_t bytes = a->bytes;
     if (nbytes) *nbytes = bytes;
     if (!out) return 0;
     DFX_REQUIRE(max_bytes >= bytes, "output buffer too small for '" + n + "'");
     if (bytes == 0) return 0;
-    if (unpack4) {
+    if (a->conv == ExchangeConv::ids32) {
+        std::vector<int32_t> tmp((size_t)bytes / 8);
+        DFX_CUDA(cudaMemcpy(tmp.data(), a->buf->p, (size_t)bytes / 2, cudaMemcpyDeviceToHost));
+        std::copy(tmp.begin(), tmp.end(), (int64_t*)out);
+    } else if (a->conv == ExchangeConv::codes4) {
         std::vector<uint8_t> packed((size_t)bytes / 2);
-        DFX_CUDA(cudaMemcpy(packed.data(), idx->payload.p, packed.size(), cudaMemcpyDeviceToHost));
+        DFX_CUDA(cudaMemcpy(packed.data(), a->buf->p, packed.size(), cudaMemcpyDeviceToHost));
         uint8_t* o = (uint8_t*)out;
         for (size_t b = 0; b < packed.size(); b++) {  // M is even: byte b holds codes 2b and 2b + 1
             o[2 * b] = packed[b] & 15;
             o[2 * b + 1] = packed[b] >> 4;
         }
-    } else if (widen_ids) {
-        std::vector<int32_t> tmp((size_t)nt);
-        DFX_CUDA(cudaMemcpy(tmp.data(), idx->ids.p, (size_t)nt * 4, cudaMemcpyDeviceToHost));
-        int64_t* o = (int64_t*)out;
-        for (int64_t i = 0; i < nt; i++) o[i] = tmp[(size_t)i];
     } else {
-        DFX_CUDA(cudaMemcpy(out, src, (size_t)bytes, cudaMemcpyDeviceToHost));
+        DFX_CUDA(cudaMemcpy(out, a->buf->p, (size_t)bytes, cudaMemcpyDeviceToHost));
     }
     DFX_API_END
 }
@@ -609,51 +636,27 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
     std::string n(name);
     if (idx->il) dfx_pq_il_to_rm(idx, idx->stream);  // imports arrive row-major
     const int64_t nlist = idx->cfg.nlist, d = idx->cfg.d;
-    auto upload = [&](DevBuf& b, int64_t bytes) {
-        b.reserve((size_t)std::max<int64_t>(bytes, 4));
-        if (bytes) DFX_CUDA(cudaMemcpy(b.p, in, (size_t)bytes, cudaMemcpyHostToDevice));
-    };
-    if (n == "centroids" && idx->is_ivf()) {
-        DFX_REQUIRE(nbytes == nlist * d * 4, "centroids: wrong size");
-        upload(idx->centroids, nbytes);
-        idx->cnorm.reserve((size_t)nlist * 4);
-        dfx_launch_row_norms(idx->centroids.as<float>(), nlist, (int)d, idx->cnorm.as<float>(), idx->stream);
-        DFX_CUDA(cudaStreamSynchronize(idx->stream));
-    } else if (n == "codebooks" && idx->has_pq()) {
-        DFX_REQUIRE(nbytes == (int64_t)idx->M * idx->ksub * idx->dsub * 4, "codebooks: wrong size");
-        upload(idx->codebooks, nbytes);
-        idx->cbT_valid = false;
-    } else if (n == "sq_trained" && idx->cfg.kind == DFX_IVF_SQ8) {
-        DFX_REQUIRE(nbytes == 2 * d * 4, "sq_trained: wrong size (2 * d floats: vmin, then vdiff)");
-        upload(idx->sq_trained, nbytes);
-    } else if (n == "refine_codebooks" && idx->cfg.kind == DFX_IVF_PQR) {
-        DFX_REQUIRE(nbytes == (int64_t)idx->M2 * 256 * idx->dsub2 * 4, "refine_codebooks: wrong size");
-        upload(idx->refine_cb, nbytes);
-    } else if (n == "refine_codes" && idx->cfg.kind == DFX_IVF_PQR) {
-        DFX_REQUIRE(nbytes == idx->n_sorted * (int64_t)idx->M2,
-                    "refine_codes: wrong size (u8[ntotal, M2] in id order; set list_off first)");
-        upload(idx->refine_codes, nbytes);
-        idx->refine_cap = idx->refine_rows = idx->n_sorted;
-    } else if (n == "refine_vecs" && idx->rflat()) {
-        DFX_REQUIRE(nbytes == idx->n_sorted * d * 4,
-                    "refine_vecs: wrong size (f32[ntotal, d] in id order; set list_off first)");
-        upload(idx->refine_vecs, nbytes);
-        idx->refine_cap = idx->refine_rows = idx->n_sorted;
-    } else if (n == "list_off" && idx->is_ivf()) {
-        DFX_REQUIRE(nbytes == (nlist + 1) * 8, "list_off: wrong size");
-        upload(idx->list_off, nbytes);
-        idx->h_list_off.assign((const int64_t*)in, (const int64_t*)in + nlist + 1);
-        DFX_REQUIRE(idx->h_list_off[0] == 0, "list_off[0] must be 0");
-        idx->update_list_lengths();
-        idx->n_sorted = idx->h_list_off[(size_t)nlist];
-        idx->n_pending = 0;
-    } else if (n == "ids" && idx->is_ivf()) {
-        DFX_REQUIRE(nbytes == idx->n_sorted * 8, "ids: wrong size (set list_off first)");
-        std::vector<int32_t> tmp((size_t)idx->n_sorted);
+    const std::vector<ExchangeArray> arrays = exchange_arrays(idx);
+    const ExchangeArray* a = find_exchange_array(arrays, n);
+    if (!a || !a->importable) throw DfxError{"cannot import array '" + n + "'"};
+    if (idx->cfg.kind == DFX_FLAT) {  // the import sets the number of rows
+        DFX_REQUIRE(nbytes % (d * 4) == 0, a->size_error);
+        idx->n_sorted = nbytes / (d * 4);
+        idx->tc_flat_rows = -1;  // imported rows: any fp16 planes are stale
+    } else {
+        DFX_REQUIRE(nbytes == a->bytes, a->size_error);
+    }
+    // the host conversions, which check the values they convert before anything is uploaded
+    const void* src = in;
+    int64_t dev_bytes = nbytes;
+    std::vector<int32_t> ids32;
+    std::vector<uint8_t> packed;
+    if (a->conv == ExchangeConv::ids32) {
         const int64_t* s = (const int64_t*)in;
+        ids32.resize((size_t)idx->n_sorted);
         for (int64_t i = 0; i < idx->n_sorted; i++) {
             DFX_REQUIRE(s[i] >= 0 && s[i] < (1ll << 31), "ids must be in [0, 2^31)");
-            tmp[(size_t)i] = (int32_t)s[i];
+            ids32[(size_t)i] = (int32_t)s[i];
         }
         if (idx->cfg.kind == DFX_IVF_PQR || idx->rflat()) {
             // the refine codes / rows are addressed by id (faiss asserts the same of IndexIVFPQR)
@@ -665,38 +668,39 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
                 seen[(size_t)s[i]] = 1;
             }
         }
-        idx->ids.reserve((size_t)std::max<int64_t>(idx->n_sorted, 1) * 4);
-        if (idx->n_sorted)
-            DFX_CUDA(cudaMemcpy(idx->ids.p, tmp.data(), (size_t)idx->n_sorted * 4, cudaMemcpyHostToDevice));
-    } else if (n == payload_name(idx->cfg.kind)) {
-        if (idx->cfg.kind == DFX_FLAT) {
-            DFX_REQUIRE(nbytes % (d * 4) == 0, "xb: wrong size");
-            idx->n_sorted = nbytes / (d * 4);
-            idx->tc_flat_rows = -1;  // imported rows: any fp16 planes are stale
-            upload(idx->payload, nbytes);
-            if (idx->cfg.metric == DFX_METRIC_L2) {
-                idx->xnorm.reserve((size_t)std::max<int64_t>(idx->n_sorted, 1) * 4);
-                dfx_launch_row_norms(idx->payload.as<float>(), idx->n_sorted, (int)d, idx->xnorm.as<float>(), idx->stream);
-                DFX_CUDA(cudaStreamSynchronize(idx->stream));
-            }
-        } else if (idx->has_pq() && idx->ksub == 16) {
-            DFX_REQUIRE(nbytes == idx->n_sorted * (int64_t)idx->M,
-                        "codes: wrong size (one byte per code, u8[ntotal, M]; set list_off first)");
-            const uint8_t* s = (const uint8_t*)in;
-            std::vector<uint8_t> packed((size_t)nbytes / 2);
-            for (size_t b = 0; b < packed.size(); b++) {
-                DFX_REQUIRE(s[2 * b] < 16 && s[2 * b + 1] < 16, "codes: a 4-bit code must be in [0, 16)");
-                packed[b] = (uint8_t)(s[2 * b] | (s[2 * b + 1] << 4));
-            }
-            idx->payload.reserve(std::max<size_t>(packed.size(), 4));
-            if (!packed.empty())
-                DFX_CUDA(cudaMemcpy(idx->payload.p, packed.data(), packed.size(), cudaMemcpyHostToDevice));
-        } else {
-            DFX_REQUIRE(nbytes == idx->n_sorted * (int64_t)idx->row_bytes(), "payload: wrong size (set list_off first)");
-            upload(idx->payload, nbytes);
+        src = ids32.data();
+        dev_bytes = nbytes / 2;
+    } else if (a->conv == ExchangeConv::codes4) {
+        const uint8_t* s = (const uint8_t*)in;
+        packed.resize((size_t)nbytes / 2);
+        for (size_t b = 0; b < packed.size(); b++) {
+            DFX_REQUIRE(s[2 * b] < 16 && s[2 * b + 1] < 16, "codes: a 4-bit code must be in [0, 16)");
+            packed[b] = (uint8_t)(s[2 * b] | (s[2 * b + 1] << 4));
         }
-    } else {
-        throw DfxError{"cannot import array '" + n + "'"};
+        src = packed.data();
+        dev_bytes = nbytes / 2;
+    }
+    a->buf->reserve((size_t)std::max<int64_t>(dev_bytes, 4));
+    if (dev_bytes) DFX_CUDA(cudaMemcpy(a->buf->p, src, (size_t)dev_bytes, cudaMemcpyHostToDevice));
+    // what the uploaded array determines
+    if (n == "centroids") {
+        idx->cnorm.reserve((size_t)nlist * 4);
+        dfx_launch_row_norms(idx->centroids.as<float>(), nlist, (int)d, idx->cnorm.as<float>(), idx->stream);
+        DFX_CUDA(cudaStreamSynchronize(idx->stream));
+    } else if (n == "codebooks") {
+        idx->cbT_valid = false;
+    } else if (n == "list_off") {
+        idx->h_list_off.assign((const int64_t*)in, (const int64_t*)in + nlist + 1);
+        DFX_REQUIRE(idx->h_list_off[0] == 0, "list_off[0] must be 0");
+        idx->update_list_lengths();
+        idx->n_sorted = idx->h_list_off[(size_t)nlist];
+        idx->n_pending = 0;
+    } else if (n == "xb" && idx->cfg.metric == DFX_METRIC_L2) {
+        idx->xnorm.reserve((size_t)std::max<int64_t>(idx->n_sorted, 1) * 4);
+        dfx_launch_row_norms(idx->payload.as<float>(), idx->n_sorted, (int)d, idx->xnorm.as<float>(), idx->stream);
+        DFX_CUDA(cudaStreamSynchronize(idx->stream));
+    } else if (n == "refine_codes" || n == "refine_vecs") {
+        idx->refine_cap = idx->refine_rows = idx->n_sorted;
     }
     idx->inv_valid = false;
     DFX_API_END

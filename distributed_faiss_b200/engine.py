@@ -41,6 +41,60 @@ EXPORTED_SYMBOLS = [
 ]
 
 
+# ---- the state exchange format (include/dfx.h), shared by GpuIndex, the stored-shard loader and the
+# CPU oracles.  Every array's dtype and shape given (d, M, ksub, M2); -1 counts the stored vectors
+# (nlist for "centroids", nlist + 1 for "list_off").
+STATE_ARRAYS = {
+    "xb": (np.float32, lambda d, M, ksub, M2: (-1, d)),
+    "centroids": (np.float32, lambda d, M, ksub, M2: (-1, d)),
+    "codebooks": (np.float32, lambda d, M, ksub, M2: (M, ksub, d // M)),
+    "sq_trained": (np.float32, lambda d, M, ksub, M2: (2, d)),  # vmin, then vdiff
+    "refine_codebooks": (np.float32, lambda d, M, ksub, M2: (M2, 256, d // M2)),
+    "list_off": (np.int64, lambda d, M, ksub, M2: (-1,)),
+    "ids": (np.int64, lambda d, M, ksub, M2: (-1,)),
+    "vecs": (np.float32, lambda d, M, ksub, M2: (-1, d)),
+    "codes": (np.uint8, lambda d, M, ksub, M2: (-1, M)),  # one code per byte, also of 4-bit codes
+    "codes16": (np.uint16, lambda d, M, ksub, M2: (-1, d)),
+    "codes8": (np.uint8, lambda d, M, ksub, M2: (-1, d)),
+    "tvals": (np.float32, lambda d, M, ksub, M2: (-1,)),
+    "refine_codes": (np.uint8, lambda d, M, ksub, M2: (-1, M2)),  # by id
+    "refine_vecs": (np.float32, lambda d, M, ksub, M2: (-1, d)),  # by id
+}
+# every kind's scalar keys (besides "kind" and "d") and arrays, the arrays in the import order of dfx.h;
+# a flat refinement (",RFlat") adds STATE_RFLAT's
+STATE_KINDS = {
+    "flat": (("metric",), ("xb",)),
+    "ivf_flat": (("nlist", "metric"), ("centroids", "list_off", "ids", "vecs")),
+    "ivf_pq": (("nlist", "coarse_metric", "M", "ksub"), ("centroids", "codebooks", "list_off", "ids", "codes", "tvals")),
+    "ivf_sq": (("nlist", "coarse_metric"), ("centroids", "list_off", "ids", "codes16")),
+    "ivf_sq8": (("nlist", "coarse_metric"), ("centroids", "sq_trained", "list_off", "ids", "codes8")),
+    "ivf_pq_fs": (("nlist", "coarse_metric", "M", "ksub"), ("centroids", "codebooks", "list_off", "ids", "codes")),
+    "ivf_pqr": (("nlist", "coarse_metric", "M", "ksub", "M2", "k_factor"),
+                ("centroids", "codebooks", "refine_codebooks", "list_off", "ids", "codes", "tvals", "refine_codes")),
+}
+STATE_RFLAT = (("refine_flat", "k_factor"), ("refine_vecs",))
+
+
+class StateLayout:
+    """What the state dict of one engine object, a GpuIndex or a CPU oracle, holds."""
+
+    def __init__(self, ix):
+        self.kind = ix.kind if isinstance(ix.kind, str) else KIND_NAMES[ix.kind]
+        self.refine_flat = bool(getattr(ix, "refine_flat", False))
+        self.scalars, self.arrays = STATE_KINDS[self.kind]
+        if self.refine_flat:
+            self.scalars, self.arrays = self.scalars + STATE_RFLAT[0], self.arrays + STATE_RFLAT[1]
+        self.d = int(ix.d)
+        if isinstance(ix.kind, str):  # a CPU oracle names M and M2 as the state does; kinds without them have none
+            M, M2 = getattr(ix, "M", 0), getattr(ix, "M2", 0)
+        else:  # GpuIndex names them as dfx_cfg does
+            M, M2 = ix.pq_m, ix.refine_m
+        self.dims = {"M": int(M), "ksub": int(getattr(ix, "ksub", 0)), "M2": int(M2)}
+
+    def shape(self, name):
+        return STATE_ARRAYS[name][1](self.d, **self.dims)
+
+
 class DfxCfg(C.Structure):
     _fields_ = [("kind", C.c_int32), ("metric", C.c_int32), ("d", C.c_int32), ("pq_m", C.c_int32),
                 ("pq_nbits", C.c_int32), ("device", C.c_int32), ("nlist", C.c_int64), ("refine_m", C.c_int32),
@@ -276,86 +330,35 @@ class GpuIndex:
         return ms.value, n.value
 
     # ---- state exchange (tests / persistence)
-    _DTYPES = {"centroids": np.float32, "codebooks": np.float32, "list_off": np.int64, "ids": np.int64,
-               "codes": np.uint8, "tvals": np.float32, "vecs": np.float32, "codes16": np.uint16,
-               "xb": np.float32, "sq_trained": np.float32, "codes8": np.uint8, "refine_codebooks": np.float32,
-               "refine_codes": np.uint8, "refine_vecs": np.float32}
-
     def get_array(self, name):
         nb = C.c_int64(0)
         _check(lib().dfx_get_array(self._h, name.encode(), None, C.c_int64(0), C.byref(nb)))
-        dt = np.dtype(self._DTYPES[name])
+        dt = np.dtype(STATE_ARRAYS[name][0])
         out = np.empty((nb.value // dt.itemsize,), dtype=dt)
         _check(lib().dfx_get_array(self._h, name.encode(), _np_ptr(out), C.c_int64(nb.value), C.byref(nb)))
         return out
 
     def set_array(self, name, arr):
-        arr = np.ascontiguousarray(arr, dtype=self._DTYPES[name])
+        arr = np.ascontiguousarray(arr, dtype=STATE_ARRAYS[name][0])
         _check(lib().dfx_set_array(self._h, name.encode(), _np_ptr(arr), C.c_int64(arr.nbytes)))
-
-    def payload_name(self):
-        return {KIND_FLAT: "xb", KIND_IVF_FLAT: "vecs", KIND_IVF_PQ: "codes", KIND_IVF_SQ16: "codes16",
-                KIND_IVF_SQ8: "codes8", KIND_IVF_PQ_FS: "codes", KIND_IVF_PQR: "codes"}[self.kind]
 
     def get_state(self):
         """Same dict layout as oracle.get_state() (list-sorted storage order)."""
-        d = self.d
-        if self.kind == KIND_FLAT:
-            return {"kind": "flat", "d": d, "metric": self.metric, "xb": self.get_array("xb").reshape(-1, d)}
-        st = {"kind": KIND_NAMES[self.kind], "d": d, "nlist": self.nlist,
-              "centroids": self.get_array("centroids").reshape(-1, d),
-              "list_off": self.get_array("list_off"), "ids": self.get_array("ids")}
-        if self.kind == KIND_IVF_FLAT:
-            st["metric"] = self.metric
-            st["vecs"] = self.get_array("vecs").reshape(-1, d)
-        else:
-            st["coarse_metric"] = self.metric
-        if self.kind in (KIND_IVF_PQ, KIND_IVF_PQR):
-            st["M"], st["ksub"] = self.pq_m, self.ksub
-            st["codebooks"] = self.get_array("codebooks").reshape(self.pq_m, self.ksub, d // self.pq_m)
-            st["codes"] = self.get_array("codes").reshape(-1, self.pq_m)
-            st["tvals"] = self.get_array("tvals")
-        if self.kind == KIND_IVF_PQR:  # the refinement PQ; its codes are in id order
-            M2 = self.refine_m
-            st["M2"] = M2
-            st["refine_codebooks"] = self.get_array("refine_codebooks").reshape(M2, 256, d // M2)
-            st["refine_codes"] = self.get_array("refine_codes").reshape(-1, M2)
-            st["k_factor"] = self.get_param("k_factor")
-        if self.kind == KIND_IVF_PQ_FS:  # codes of the raw vectors: no t-values
-            st["M"], st["ksub"] = self.pq_m, self.ksub
-            st["codebooks"] = self.get_array("codebooks").reshape(self.pq_m, self.ksub, d // self.pq_m)
-            st["codes"] = self.get_array("codes").reshape(-1, self.pq_m)
-        if self.kind == KIND_IVF_SQ16:
-            st["codes16"] = self.get_array("codes16").reshape(-1, d)
-        if self.kind == KIND_IVF_SQ8:
-            st["sq_trained"] = self.get_array("sq_trained").reshape(2, d)
-            st["codes8"] = self.get_array("codes8").reshape(-1, d)
-        if self.refine_flat:  # the raw rows, in id order
-            st["refine_flat"] = 1
-            st["refine_vecs"] = self.get_array("refine_vecs").reshape(-1, d)
-            st["k_factor"] = self.get_param("k_factor")
+        lay = StateLayout(self)
+        scalars = {"nlist": self.nlist, "metric": self.metric, "coarse_metric": self.metric, "refine_flat": 1,
+                   **lay.dims}
+        st = {"kind": lay.kind, "d": self.d}
+        st.update((key, self.get_param(key) if key == "k_factor" else scalars[key]) for key in lay.scalars)
+        st.update((name, self.get_array(name).reshape(lay.shape(name))) for name in lay.arrays)
         return st
 
     def set_state(self, st):
-        if self.kind == KIND_FLAT:
-            self.set_array("xb", st["xb"])
-        else:
-            self.set_array("centroids", st["centroids"])
-            if self.kind in (KIND_IVF_PQ, KIND_IVF_PQ_FS, KIND_IVF_PQR):
-                self.set_array("codebooks", st["codebooks"])
-            if self.kind == KIND_IVF_SQ8:
-                self.set_array("sq_trained", st["sq_trained"])
-            if self.kind == KIND_IVF_PQR:
-                self.set_array("refine_codebooks", st["refine_codebooks"])
-            self.set_array("list_off", st["list_off"])
-            self.set_array("ids", st["ids"])
-            self.set_array(self.payload_name(), st[self.payload_name()])
-            if self.kind == KIND_IVF_PQR:
-                self.set_array("refine_codes", st["refine_codes"])
-            if self.refine_flat:
-                self.set_array("refine_vecs", st["refine_vecs"])
-            if (self.kind == KIND_IVF_PQR or self.refine_flat) and "k_factor" in st:
-                self.set_param("k_factor", float(st["k_factor"]))
+        lay = StateLayout(self)
+        for name in lay.arrays:
+            if name != "tvals":  # the library recomputes them
+                self.set_array(name, st[name])
+        if "k_factor" in lay.scalars and "k_factor" in st:
+            self.set_param("k_factor", float(st["k_factor"]))
         _check(lib().dfx_import_done(self._h))
 
 

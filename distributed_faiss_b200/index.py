@@ -121,16 +121,6 @@ def default_engine_factory(cfg: IndexCfg, device: Optional[int] = None):
     raise RuntimeError("Either faiss_factory or valid index_builder_type should be specified to initialize index")
 
 
-def _kind_name(engine_obj) -> str:
-    """state-dict kind name ("flat", "ivf_sq8", ...) of an engine object (GPU or oracle)"""
-    kind = getattr(engine_obj, "kind", None)
-    if isinstance(kind, str):
-        return kind
-    from . import engine
-
-    return engine.KIND_NAMES.get(kind, str(kind))
-
-
 class IntMetadata:
     """`id_to_metadata` of a shard adopted from the device: local id -> integer, kept as an int64
     tensor (1 B vectors worth of Python ints would not fit a host).  Read-only sequence."""
@@ -567,31 +557,25 @@ class Index:
         saved_nprobe = cfg.nprobe
         engine = result._engine_factory(build_cfg)
         cfg.nprobe = saved_nprobe
-        want = _kind_name(engine)
-        stored_rf, built_rf = bool(state.get("refine_flat", 0)), bool(getattr(engine, "refine_flat", False))
-        if state.get("kind") != want or stored_rf != built_rf:
+        from .engine import StateLayout
+
+        built = StateLayout(engine)
+        stored_rf = bool(state.get("refine_flat", 0))
+        if state.get("kind") != built.kind or stored_rf != built.refine_flat:
             # e.g. an SQfp16 file under a cfg that builds IVF-SQ8: never reinterpret the codes; and a
             # shard with a flat refinement is not one without (its answers and its stored rows differ)
             rf = {True: " with a flat refinement (RFlat)", False: ""}
             raise RuntimeError(f"the stored index is of kind {state.get('kind')!r}{rf[stored_rf]} but the cfg builds "
-                               f"{want!r}{rf[built_rf]}; refusing to load it")
-        if want in ("ivf_pq", "ivf_pq_fs"):
-            # e.g. 4-bit codes under a cfg that builds 8-bit ones: the codebooks would not fit either
-            stored = (int(state["M"]), int(state["ksub"]))
-            built = (int(getattr(engine, "pq_m", getattr(engine, "M", 0))), int(engine.ksub))
-            if stored != built:
-                raise RuntimeError(f"the stored IVF-PQ index has (M, ksub) = {stored} but the cfg builds {built}; "
-                                   "refusing to load it")
-        if want == "ivf_pqr":
-            # the refinement codes are M2 bytes per vector: another M2 would misread every one of them
-            stored = (int(state["M"]), int(state["ksub"]), int(state["M2"]))
-            built = (int(getattr(engine, "pq_m", getattr(engine, "M", 0))), int(engine.ksub),
-                     int(getattr(engine, "refine_m", getattr(engine, "M2", 0))))
-            if stored != built:
-                raise RuntimeError(f"the stored IVF-PQR index has (M, ksub, M2) = {stored} but the cfg builds "
-                                   f"{built}; refusing to load it")
+                               f"{built.kind!r}{rf[built.refine_flat]}; refusing to load it")
+        # e.g. 4-bit codes under a cfg that builds 8-bit ones, or another M2 for IVF-PQR: every code would
+        # be misread
+        keys = [key for key in built.dims if key in built.scalars]
+        stored, want = tuple(int(state[key]) for key in keys), tuple(built.dims[key] for key in keys)
+        if stored != want:
+            raise RuntimeError(f"the stored {'IVF-PQR' if 'M2' in keys else 'IVF-PQ'} index has ({', '.join(keys)}) = "
+                               f"{stored} but the cfg builds {want}; refusing to load it")
         engine.set_state(state)
-        if built_rf and "k_factor" in cfg.extra:  # the caller's cfg wins over the stored value
+        if built.refine_flat and "k_factor" in cfg.extra:  # the caller's cfg wins over the stored value
             engine.set_param("k_factor", float(cfg.extra["k_factor"]))
         assert len(meta) >= engine.ntotal, "Deserialized meta list should be at least of index size"
         result.faiss_index = engine

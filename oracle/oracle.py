@@ -20,6 +20,8 @@ import subprocess
 
 import numpy as np
 
+from distributed_faiss_b200.engine import STATE_ARRAYS, StateLayout
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _LIB_PATH = os.path.join(_HERE, "libdfx_oracle.so")
 
@@ -135,6 +137,26 @@ def merge(Dall, Iall):
 
 
 # ---------------------------------------------------------------- index objects
+class _OracleState:
+    """get_state / set_state over the scalars and arrays engine.StateLayout lists for the oracle's kind;
+    the arrays are attributes of the same names"""
+
+    def get_state(self):
+        lay = StateLayout(self)
+        st = {"kind": self.kind, "d": self.d}
+        st.update((key, getattr(self, key)) for key in lay.scalars)
+        st.update((name, getattr(self, name)) for name in lay.arrays)
+        return st
+
+    def set_state(self, st):
+        lay = StateLayout(self)
+        for name in lay.arrays:
+            if name != "tvals":  # recomputed (or taken) by OracleIVFPQ.set_state
+                setattr(self, name, np.ascontiguousarray(st[name], dtype=STATE_ARRAYS[name][0]).reshape(lay.shape(name)))
+        if "k_factor" in lay.scalars and "k_factor" in st:
+            self.k_factor = float(st["k_factor"])
+
+
 class _Quantizer:
     def __init__(self, owner):
         self._o = owner
@@ -143,7 +165,7 @@ class _Quantizer:
         return self._o.centroids[i0:i0 + n].copy()
 
 
-class OracleFlat:
+class OracleFlat(_OracleState):
     """faiss.IndexFlatIP / IndexFlatL2 restated (reference index.py:94, 25-33)."""
 
     kind = "flat"
@@ -177,14 +199,8 @@ class OracleFlat:
         R = self.reconstruct_rows(I.reshape(-1)).reshape(I.shape[0], I.shape[1], self.d)
         return D, I, R
 
-    def get_state(self):
-        return {"kind": "flat", "d": self.d, "metric": self.metric, "xb": self.xb.copy()}
 
-    def set_state(self, st):
-        self.xb = _f32(st["xb"])
-
-
-class _OracleIVF:
+class _OracleIVF(_OracleState):
     def __init__(self, d, nlist, coarse_metric):
         self.d, self.nlist, self.coarse_metric = int(d), int(nlist), int(coarse_metric)
         self.nprobe = 1  # faiss default
@@ -236,6 +252,11 @@ class _OracleIVF:
         R = self.reconstruct_rows(I.reshape(-1)).reshape(I.shape[0], I.shape[1], self.d)
         return D, I, R
 
+    def set_state(self, st):
+        super().set_state(st)
+        self.ntotal = int(self.ids.shape[0])
+        self.is_trained = True
+
 
 class OracleIVFFlat(_OracleIVF):
     """faiss.IndexIVFFlat restated (reference index.py:36-40 'ivf_simple')."""
@@ -274,19 +295,6 @@ class OracleIVFFlat(_OracleIVF):
         ok = ids >= 0
         out[ok] = self.vecs[inv[ids[ok]]]
         return out
-
-    def get_state(self):
-        return {"kind": self.kind, "d": self.d, "metric": self.metric, "nlist": self.nlist,
-                "centroids": self.centroids, "list_off": self.list_off, "ids": self.ids,
-                "vecs": self.vecs}
-
-    def set_state(self, st):
-        self.centroids = _f32(st["centroids"])
-        self.list_off = _i64(st["list_off"])
-        self.ids = _i64(st["ids"])
-        self.vecs = _f32(st["vecs"])
-        self.ntotal = int(self.ids.shape[0])
-        self.is_trained = True
 
 
 class OracleIVFPQ(_OracleIVF):
@@ -370,24 +378,12 @@ class OracleIVFPQ(_OracleIVF):
             out[r] = v
         return out
 
-    def get_state(self):
-        return {"kind": self.kind, "d": self.d, "coarse_metric": self.coarse_metric,
-                "nlist": self.nlist, "M": self.M, "ksub": self.ksub, "centroids": self.centroids,
-                "codebooks": self.codebooks, "list_off": self.list_off, "ids": self.ids,
-                "codes": self.codes, "tvals": self.tvals}
-
     def set_state(self, st, recompute_tvals=True):
-        self.centroids = _f32(st["centroids"])
-        self.codebooks = _f32(st["codebooks"]).reshape(self.M, self.ksub, self.dsub)
-        self.list_off = _i64(st["list_off"])
-        self.ids = _i64(st["ids"])
-        self.codes = np.ascontiguousarray(st["codes"], dtype=np.uint8)
-        self.ntotal = int(self.ids.shape[0])
+        super().set_state(st)
         if recompute_tvals or "tvals" not in st:
             self.tvals = self.compute_tvals(self.codes, self.list_of_rows())
         else:
             self.tvals = _f32(st["tvals"])
-        self.is_trained = True
 
 
 class OracleIVFSQ(_OracleIVF):
@@ -433,19 +429,6 @@ class OracleIVFSQ(_OracleIVF):
         pos = inv[ids[ok]]
         out[ok] = self.centroids[lo[pos]] + half_to_float(self.codes16[pos])
         return out
-
-    def get_state(self):
-        return {"kind": self.kind, "d": self.d, "coarse_metric": self.coarse_metric,
-                "nlist": self.nlist, "centroids": self.centroids, "list_off": self.list_off,
-                "ids": self.ids, "codes16": self.codes16}
-
-    def set_state(self, st):
-        self.centroids = _f32(st["centroids"])
-        self.list_off = _i64(st["list_off"])
-        self.ids = _i64(st["ids"])
-        self.codes16 = np.ascontiguousarray(st["codes16"], dtype=np.uint16)
-        self.ntotal = int(self.ids.shape[0])
-        self.is_trained = True
 
 
 def make_index(kind, d, metric=METRIC_IP, nlist=0, M=0, nbits=8):

@@ -137,20 +137,6 @@ class OracleIVFPQFastScan(O._OracleIVF):
         out[ok] = self.codebooks[np.arange(self.M)[None, :], codes].reshape(-1, self.d)
         return out
 
-    def get_state(self):
-        return {"kind": self.kind, "d": self.d, "coarse_metric": self.coarse_metric, "nlist": self.nlist,
-                "M": self.M, "ksub": self.ksub, "centroids": self.centroids, "codebooks": self.codebooks,
-                "list_off": self.list_off, "ids": self.ids, "codes": self.codes}
-
-    def set_state(self, st):
-        self.centroids = np.ascontiguousarray(st["centroids"], dtype=F32)
-        self.codebooks = np.ascontiguousarray(st["codebooks"], dtype=F32).reshape(self.M, KSUB, self.dsub)
-        self.list_off = np.ascontiguousarray(st["list_off"], dtype=np.int64)
-        self.ids = np.ascontiguousarray(st["ids"], dtype=np.int64)
-        self.codes = np.ascontiguousarray(st["codes"], dtype=np.uint8).reshape(-1, self.M)
-        self.ntotal = int(self.ids.shape[0])
-        self.is_trained = True
-
 
 def make_index(kind, d, metric=O.METRIC_IP, nlist=0, M=0, nbits=8):
     """tests/oracle_sq8.make_index plus "ivf_pq_fs" (metric: the coarse quantizer's, L2)"""

@@ -153,19 +153,6 @@ class OracleIVFPQR(O.OracleIVFPQ):
         out[ok] = (out[ok] + decode(self.refine_codebooks, self.refine_codes[ids[ok]])).astype(F32)
         return out
 
-    def get_state(self):
-        st = super().get_state()
-        st.update(kind=self.kind, M2=self.M2, refine_codebooks=self.refine_codebooks,
-                  refine_codes=self.refine_codes, k_factor=self.k_factor)
-        return st
-
-    def set_state(self, st, recompute_tvals=True):
-        super().set_state(st, recompute_tvals)
-        self.refine_codebooks = np.ascontiguousarray(st["refine_codebooks"], dtype=F32).reshape(self.M2, KSUB, self.dsub2)
-        self.refine_codes = np.ascontiguousarray(st["refine_codes"], dtype=np.uint8).reshape(-1, self.M2)
-        if "k_factor" in st:
-            self.k_factor = float(st["k_factor"])
-
 
 # ---------------------------------------------------------------- float64 restatement
 def reconstruct_f64(state, rows):

@@ -46,7 +46,7 @@ def refine_exact(x, I1, vecs, k):
 class _RFlat:
     """mixed in before a base oracle class: the refinement store and the re-ranked search"""
 
-    refine_flat = True
+    refine_flat = 1   # as the state dict holds it
 
     def __init__(self, *a, **kw):
         super().__init__(*a, **kw)
@@ -76,17 +76,9 @@ class _RFlat:
         assert name == "k_factor" and 1 <= value <= 16384
         self.k_factor = float(value)
 
-    def get_state(self):
-        st = super().get_state()
-        st.update(refine_flat=1, refine_vecs=self.refine_vecs, k_factor=self.k_factor)
-        return st
-
     def set_state(self, st):
         super().set_state(st)
-        self.refine_vecs = np.ascontiguousarray(st["refine_vecs"], dtype=F32).reshape(-1, self.d)
         assert len(self.refine_vecs) == self.ntotal
-        if "k_factor" in st:
-            self.k_factor = float(st["k_factor"])
 
 
 _CLASSES = {kind: type("RFlat" + base.__name__, (_RFlat, base), {}) for kind, base in BASES.items()}

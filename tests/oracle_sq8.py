@@ -161,20 +161,6 @@ class OracleIVFSQ8(O._OracleIVF):
         out[ok] = self.centroids[lo[pos]] + sq8_decode(self.sq_trained, self.codes8[pos])
         return out
 
-    def get_state(self):
-        return {"kind": self.kind, "d": self.d, "coarse_metric": self.coarse_metric,
-                "nlist": self.nlist, "centroids": self.centroids, "sq_trained": self.sq_trained,
-                "list_off": self.list_off, "ids": self.ids, "codes8": self.codes8}
-
-    def set_state(self, st):
-        self.centroids = np.ascontiguousarray(st["centroids"], dtype=np.float32)
-        self.sq_trained = np.ascontiguousarray(st["sq_trained"], dtype=np.float32).reshape(2, self.d)
-        self.list_off = np.ascontiguousarray(st["list_off"], dtype=np.int64)
-        self.ids = np.ascontiguousarray(st["ids"], dtype=np.int64)
-        self.codes8 = np.ascontiguousarray(st["codes8"], dtype=np.uint8).reshape(-1, self.d)
-        self.ntotal = int(self.ids.shape[0])
-        self.is_trained = True
-
 
 def make_index(kind, d, metric=O.METRIC_IP, nlist=0, M=0, nbits=8):
     """oracle.make_index plus "ivf_sq8" (same (kind, metric) meaning as the engine factory)"""

@@ -93,6 +93,8 @@ def test_flat_edge_cases():
     xb[2] = xb[0]  # exact duplicate -> tie broken by id
     g.add(xb); o.add(xb)
     _assert_same(*g.search(xq, 5), *o.search(xq, 5), "flat k > ntotal with ties")
+    with pytest.raises(RuntimeError, match="xb: wrong size"):
+        g.set_array("xb", xb.reshape(-1)[:-1])
 
 
 # ------------------------------------------------------------------ IVF kinds
@@ -186,6 +188,58 @@ def test_ivf_edge_cases():
             _assert_same(Dg, Ig, Do, Io, f"edge {kind} nprobe={nprobe}")
             assert (Ig == -1).any()
             assert (Dg[Ig == -1] == np.finfo(np.float32).max).all()
+        _assert_exchange_refusals(g, o.get_state(), {"ivf_flat": "vecs", "ivf_pq": "codes", "ivf_sq": "codes16"}[kind])
+
+
+def _import_without(g, st, skip):
+    """import every array of the state `st` into `g` but `skip`, then finish the import"""
+    E = _engine()
+    for name in E.StateLayout(g).arrays:
+        if name not in (skip, "tvals"):
+            g.set_array(name, st[name])
+    E._check(E.lib().dfx_import_done(g._h))
+
+
+def _assert_exchange_refusals(g, st, payload):
+    """what the state exchange of an IVF index `g` holding the state `st` (payload array `payload`,
+    8-bit codes) refuses"""
+    import ctypes as C
+
+    E = _engine()
+    small = np.zeros(2, dtype=np.int64)
+    with pytest.raises(RuntimeError, match="output buffer too small for 'ids'"):
+        E._check(E.lib().dfx_get_array(g._h, b"ids", E._np_ptr(small), C.c_int64(small.nbytes), None))
+    with pytest.raises(RuntimeError, match="no array named 'nope' in this index"):
+        E._check(E.lib().dfx_get_array(g._h, b"nope", None, C.c_int64(0), None))
+
+    def fresh():
+        return E.GpuIndex(g.kind, g.d, g.metric, nlist=g.nlist, pq_m=g.pq_m, pq_nbits=g.pq_nbits)
+
+    g2 = fresh()
+    with pytest.raises(RuntimeError, match="no array named 'centroids' in this index"):
+        g2.get_array("centroids")  # not trained yet
+    for name in ("nope", "tvals", "xb"):
+        with pytest.raises(RuntimeError, match=f"cannot import array '{name}'"):
+            E._check(E.lib().dfx_set_array(g2._h, name.encode(), E._np_ptr(small), C.c_int64(small.nbytes)))
+    for name in E.StateLayout(g).arrays:
+        if name != "tvals":
+            with pytest.raises(RuntimeError, match=f"{'payload' if name == payload else name}: wrong size"):
+                g2.set_array(name, st[name].reshape(-1)[:-1])
+    bad = st["list_off"].copy()
+    bad[0] = 1
+    with pytest.raises(RuntimeError, match=r"list_off\[0\] must be 0"):
+        g2.set_array("list_off", bad)
+    g2.set_array("list_off", st["list_off"])
+    for v in (-1, 1 << 31):
+        bad = st["ids"].copy()
+        bad[3] = v
+        with pytest.raises(RuntimeError, match=r"ids must be in \[0, 2\^31\)"):
+            g2.set_array("ids", bad)
+    with pytest.raises(RuntimeError, match="import: centroids and list_off are required"):
+        _import_without(fresh(), st, "centroids")
+    if "codebooks" in st:
+        with pytest.raises(RuntimeError, match="import: codebooks are required"):
+            _import_without(fresh(), st, "codebooks")
 
 
 def test_ivfpq_larger_property():

@@ -538,6 +538,14 @@ def test_pqr_limits():
         g2.set_state(dict(st, ids=bad))
     with pytest.raises(RuntimeError, match="refine_codes: wrong size"):
         g2.set_state(dict(st, refine_codes=st["refine_codes"][:-1]))
+    with pytest.raises(RuntimeError, match="refine_codebooks: wrong size"):
+        g2.set_array("refine_codebooks", st["refine_codebooks"].reshape(-1)[:-1])
+    from tests.test_gpu_parity import _import_without
+
+    for skip, msg in (("refine_codebooks", "refine_codebooks are required"),
+                      ("refine_codes", "refine_codes of every vector are required")):
+        with pytest.raises(RuntimeError, match="import: " + msg):
+            _import_without(_pair(64, 4, 8, 8)[0], st, skip)
 
 
 @pytest.mark.gpu

@@ -578,6 +578,13 @@ def test_rflat_limits(rflat_oracle):
         g2.set_state(dict(st, ids=bad))
     with pytest.raises(RuntimeError, match="refine_vecs: wrong size"):
         g2.set_state(dict(st, refine_vecs=st["refine_vecs"][:-1]))
+    with pytest.raises(RuntimeError, match=r"sq_trained: wrong size \(2 \* d floats"):
+        g2.set_array("sq_trained", st["sq_trained"][:1])
+    from tests.test_gpu_parity import _import_without
+
+    for skip, msg in (("sq_trained", "sq_trained is required"), ("refine_vecs", "refine_vecs of every vector are required")):
+        with pytest.raises(RuntimeError, match="import: " + msg):
+            _import_without(_gpu("ivf_sq8", 64, 4), st, skip)
 
 
 @pytest.mark.gpu
