@@ -16,12 +16,12 @@
 //
 //   K_fs1 pq_fs_lut_kernel    one CTA per query: the fp32 table in shared memory, its quantization,
 //                             LUTq u8[q][M][16] and (1 / a, b) to the workspace
-//   K_fs2 scan_pq_fs_kernel   one CTA per (query, group of probes), one lane per vector, as K4n
-//                             (dfx_scan_pq4_dev.cuh): the u8 table lives in M / 8 registers per lane
+//   K_fs2 scan_pq_fs_kernel   the list-scan skeleton (dfx_scan_dev.cuh), one lane per vector: the
+//                             u8 table lives in M / 8 registers per lane
 //   K_fs3 fs_dequant_kernel   the selected rows' D: (float)acc -> fmaf(acc, 1 / a, b); padding stays
 #pragma once
 #include "dfx_common.cuh"
-#include "dfx_topk.cuh"
+#include "dfx_scan_dev.cuh"
 
 // shared memory of pq_fs_lut_kernel: the query, the fp32 table, mn and span per sub-quantizer, a
 static inline size_t dfx_pq_fs_lut_smem(int d, int M) { return (size_t)(d + M * 16 + 2 * M + 4) * 4; }
@@ -86,12 +86,6 @@ pq_fs_lut_kernel(const float* __restrict__ Q, int d, int M, int dsub, const floa
         out[idx] = (uint8_t)(uint32_t)floorf(__fmaf_rn(s_lut[idx] - s_mn[idx >> 4], a, 0.5f));
 }
 
-// shared memory of one scan CTA: 4 per-warp candidate buffers of `cap` composites (MAT: none)
-static inline size_t dfx_pq_fs_smem(int cap) { return (size_t)4 * cap * 8; }
-
-// MAT (k > 1024): `part` is the candidate buffer; every vector's composite goes to slot
-// coff[q][p] + (position in list) (dfx_cand_store) instead of the per-warp queues.
-//
 //   * The table: lane L's word j holds LUTq[8j + 2c + (L >> 4)][L & 15] in byte c (c = 0..3), so one
 //     SHFL of word m >> 3 from lane ((m & 1) << 4) | code_m returns LUTq[m][code_m] in byte
 //     (m >> 1) & 3.  Byte c of word j is lutq[q][128 j + 32 c + L]: four coalesced byte loads.
@@ -112,87 +106,45 @@ scan_pq_fs_kernel(const uint8_t* __restrict__ lutq, const int32_t* __restrict__ 
     static_assert(MT >= 8 && MT <= 128 && MT % 8 == 0, "FastScan: M % 8 == 0, 8 <= M <= 128");
     constexpr int NW = MT / 8;  // 32-bit code words per row = 32-bit table words per lane
     DFX_DYN_SMEM(unsigned char, smem_raw, 16);
-    uint64_t* s_buf = reinterpret_cast<uint64_t*>(smem_raw);
-    const int64_t q = blockIdx.x / ngroups;
-    const int g = blockIdx.x % ngroups;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const ScanProbes pr(keys, nullptr, list_off, nprobe, G, ngroups);
+    const int lane = threadIdx.x & 31;
 
     uint32_t T[NW];
     {
-        const uint8_t* lq = lutq + q * (int64_t)MT * 16 + lane;
+        const uint8_t* lq = lutq + pr.q * (int64_t)MT * 16 + lane;
 #pragma unroll
         for (int j = 0; j < NW; j++)
             T[j] = (uint32_t)__ldg(lq + 128 * j) | ((uint32_t)__ldg(lq + 128 * j + 32) << 8) |
                    ((uint32_t)__ldg(lq + 128 * j + 64) << 16) | ((uint32_t)__ldg(lq + 128 * j + 96) << 24);
     }
-    WarpTopK wt;
-    if constexpr (!MAT) wt.init(s_buf + (size_t)warp * cap, cap, k);
+    ScanSink<MAT, 128> sink(reinterpret_cast<uint64_t*>(smem_raw), cap, k, part, coff);
 
-    const int p_end = min(nprobe, (g + 1) * G);
-    for (int p = g * G; p < p_end; p++) {
-        const int l = keys[q * nprobe + p];
-        if (l < 0) continue;
-        const int64_t beg = list_off[l], end = list_off[l + 1];
-        int64_t cbase = 0;  // MAT: slot of row i is cbase + i
-        if constexpr (MAT) cbase = coff[q * (nprobe + 1) + p] - beg;
-        for (int64_t base = beg + warp * 32; base < end; base += 128) {  // warp-uniform trip count
-            const int64_t i = base + lane;
-            const bool valid = i < end;
-            const int64_t r = valid ? i : base;  // tail lanes: the warp's first row
-            uint32_t w[NW];
-            if constexpr (NW % 4 == 0) {
-                const uint4* cp = reinterpret_cast<const uint4*>(codes + r * (MT / 2));
+    dfx_scan_lanes<false>(pr, sink, [&](int64_t i, bool valid, int64_t base, float) {
+        const int64_t r = valid ? i : base;  // tail lanes: the warp's first row
+        uint32_t w[NW];
+        dfx_load_code_words(codes + r * (MT / 2), w);
+        const uint32_t my_id = (uint32_t)__ldg(ids + r);  // loaded with the codes: no dependent load on admission
+        uint32_t acc0 = 0, acc1 = 0, acc2 = 0, acc3 = 0;
 #pragma unroll
-                for (int c = 0; c < NW / 4; c++) {
-                    const uint4 v4 = __ldg(cp + c);
-                    w[4 * c + 0] = v4.x;
-                    w[4 * c + 1] = v4.y;
-                    w[4 * c + 2] = v4.z;
-                    w[4 * c + 3] = v4.w;
-                }
-            } else if constexpr (NW % 2 == 0) {
-                const uint2* cp = reinterpret_cast<const uint2*>(codes + r * (MT / 2));
-#pragma unroll
-                for (int c = 0; c < NW / 2; c++) {
-                    const uint2 v2 = __ldg(cp + c);
-                    w[2 * c + 0] = v2.x;
-                    w[2 * c + 1] = v2.y;
-                }
-            } else {
-                const uint32_t* cp = reinterpret_cast<const uint32_t*>(codes + r * (MT / 2));
-#pragma unroll
-                for (int c = 0; c < NW; c++) w[c] = __ldg(cp + c);
-            }
-            const uint32_t my_id = (uint32_t)__ldg(ids + r);  // loaded with the codes: no dependent load on admission
-            uint32_t acc0 = 0, acc1 = 0, acc2 = 0, acc3 = 0;
-#pragma unroll
-            for (int j = 0; j < NW; j++) {
-                const uint32_t lo = w[j] & 0x0f0f0f0fu;
-                const uint32_t hi = ((w[j] >> 4) & 0x0f0f0f0fu) | 0x10101010u;
-                // sub-quantizers 8j + 2c + h: byte c of the code word and of the table word
-                acc0 += __shfl_sync(0xffffffffu, T[j], (int)lo) & 0xffu;
-                acc0 += __shfl_sync(0xffffffffu, T[j], (int)hi) & 0xffu;
-                acc1 += __shfl_sync(0xffffffffu, T[j], (int)(lo >> 8)) & 0xff00u;
-                acc1 += __shfl_sync(0xffffffffu, T[j], (int)(hi >> 8)) & 0xff00u;
-                acc2 += __shfl_sync(0xffffffffu, T[j], (int)(lo >> 16)) & 0xff0000u;
-                acc2 += __shfl_sync(0xffffffffu, T[j], (int)(hi >> 16)) & 0xff0000u;
-                acc3 += __shfl_sync(0xffffffffu, T[j], (int)(lo >> 24)) >> 24;
-                acc3 += __shfl_sync(0xffffffffu, T[j], (int)(hi >> 24)) >> 24;
-            }
-            // (float)acc, exact (acc <= 128 * 255 < 2^23), built as 2^23 + acc minus 2^23 rather than by
-            // an I2F, which issues at an eighth of the FFMA rate on sm_90
-            const uint32_t acc = acc0 + (acc1 >> 8) + (acc2 >> 16) + acc3;
-            const float v = __uint_as_float(0x4B000000u | acc) - 8388608.f;
-            if constexpr (MAT) {
-                if (valid) dfx_cand_store(part, cbase + i, v, my_id);
-            } else {
-                uint32_t sec = 0;
-                const bool want = valid && wt.admits(v, [&] { return my_id; }, sec);
-                wt.push_lanes(want, v, sec);
-            }
+        for (int j = 0; j < NW; j++) {
+            const uint32_t lo = w[j] & 0x0f0f0f0fu;
+            const uint32_t hi = ((w[j] >> 4) & 0x0f0f0f0fu) | 0x10101010u;
+            // sub-quantizers 8j + 2c + h: byte c of the code word and of the table word
+            acc0 += __shfl_sync(0xffffffffu, T[j], (int)lo) & 0xffu;
+            acc0 += __shfl_sync(0xffffffffu, T[j], (int)hi) & 0xffu;
+            acc1 += __shfl_sync(0xffffffffu, T[j], (int)(lo >> 8)) & 0xff00u;
+            acc1 += __shfl_sync(0xffffffffu, T[j], (int)(hi >> 8)) & 0xff00u;
+            acc2 += __shfl_sync(0xffffffffu, T[j], (int)(lo >> 16)) & 0xff0000u;
+            acc2 += __shfl_sync(0xffffffffu, T[j], (int)(hi >> 16)) & 0xff0000u;
+            acc3 += __shfl_sync(0xffffffffu, T[j], (int)(lo >> 24)) >> 24;
+            acc3 += __shfl_sync(0xffffffffu, T[j], (int)(hi >> 24)) >> 24;
         }
-    }
-    if constexpr (!MAT) cta_merge_and_write<128>(wt, s_buf, cap, k, part + ((int64_t)q * ngroups + g) * k);
+        // (float)acc, exact (acc <= 128 * 255 < 2^23), built as 2^23 + acc minus 2^23 rather than by
+        // an I2F, which issues at an eighth of the FFMA rate on sm_90
+        const uint32_t acc = acc0 + (acc1 >> 8) + (acc2 >> 16) + acc3;
+        return ScanCand{__uint_as_float(0x4B000000u | acc) - 8388608.f, my_id};
+    });
+    sink.finish(pr);
 }
 
 // the selected rows of a query chunk: D = fmaf(acc, 1 / a, b) where an entry exists (I >= 0); the

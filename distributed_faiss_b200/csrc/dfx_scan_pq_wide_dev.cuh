@@ -24,14 +24,14 @@
 //     coff[q][p] + (position in list) (dfx_cand_store), and the CTA's shared memory is the table only.
 #pragma once
 #include "dfx_common.cuh"
-#include "dfx_topk.cuh"
+#include "dfx_scan_dev.cuh"
 
 constexpr int PQW_KSUB = 256;
 constexpr int PQW_MAX_M = 128;  // one query's fp32 table (M x 256 x 4 B) must fit in one CTA's shared memory
 
-// shared memory of one CTA: the table, then NW per-warp candidate buffers of `cap` composites
-static inline size_t dfx_pq_wide_smem(int M, int threads, int cap) {
-    return (size_t)M * PQW_KSUB * 4 + (size_t)(threads / 32) * cap * 8;
+// shared memory of one CTA: the table, then the candidate queues
+static inline size_t dfx_pq_wide_smem(int M, int threads, int cap, bool mat) {
+    return (size_t)M * PQW_KSUB * 4 + dfx_scan_queue_smem(threads, cap, mat);
 }
 
 // MT: M when it is a multiple of 16 known at compile time (16-byte code loads), else 0 (any M % 4 == 0)

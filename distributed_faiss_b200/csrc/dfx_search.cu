@@ -13,6 +13,7 @@
 //   K_fs pq_fs_lut / scan_pq_fs / fs_dequant   IVF-PQ FastScan: u8 quantized table, integer sums
 //                         (dfx_scan_pq_fs_dev.cuh)
 //   K2/5 scan_rows        inverted-list scan of fp32 rows / fp16 / 8-bit residual codes
+//                         K4n, K_fs and K2/5 share the probe loop and candidate sink of dfx_scan_dev.cuh
 //   K_off cand_offsets    k > 1024: slots of each query's candidate row (the list scans then write
 //                         every vector's composite, MAT = true, and select_cand picks the k best)
 //   K_r  pqr_refine       IVF-PQR: re-ranks the k' = k * k_factor candidates of the IVF-PQ stage on
@@ -207,6 +208,7 @@ void dfx_launch_select_comp(const uint64_t* comp, int64_t nrows, int n, int64_t 
 }
 
 #include "dfx_pq_prep_dev.cuh"
+#include "dfx_scan_dev.cuh"
 #include "dfx_scan_pq_wide_dev.cuh"
 #include "dfx_scan_pq4_dev.cuh"
 #include "dfx_scan_pq_fs_dev.cuh"
@@ -327,7 +329,6 @@ __device__ __forceinline__ float dfx_sq8_component(uint32_t w, uint32_t sel, flo
     return __fmaf_rn(__fmaf_rn(c, DFX_SQ8_SCALE, DFX_SQ8_BIAS), vdiff, vmin);
 }
 
-// MAT (k > 1024): as scan_pq_kernel, every vector's composite goes to its slot of the candidate row
 template <int MODE, int U = 4, bool MAT = false>
 __global__ void __launch_bounds__(128)
 scan_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent,
@@ -341,9 +342,8 @@ scan_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ c
     float* s_vmin = s_q + 2 * d;                        // MODE 3: vmin, then vdiff
     float* s_vdiff = s_q + 3 * d;
     const int dpad = (MODE == 3) ? 4 * d : (MODE == 2) ? 2 * d : d;
-    uint64_t* s_buf = reinterpret_cast<uint64_t*>(smem_raw + (((size_t)dpad * 4 + 15) / 16) * 16);
-    const int64_t q = blockIdx.x / ngroups;
-    const int g = blockIdx.x % ngroups;
+    const ScanProbes pr(keys, nullptr, list_off, nprobe, G, ngroups);
+    const int64_t q = pr.q;
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
 
     for (int i = tid; i < d; i += 128) {
@@ -355,22 +355,18 @@ scan_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ c
             s_vdiff[i] = sq_trained[d + i];
         }
     }
-    WarpTopK wt;
-    if constexpr (!MAT) wt.init(s_buf + (size_t)warp * cap, cap, k);
+    ScanSink<MAT, 128> sink(reinterpret_cast<uint64_t*>(smem_raw + (((size_t)dpad * 4 + 15) / 16) * 16), cap, k,
+                            part, coff);
     __syncthreads();
 
-    const int p_end = min(nprobe, (g + 1) * G);
-    for (int p = g * G; p < p_end; p++) {
-        const int l = keys[q * nprobe + p];
-        if (l < 0) continue;
+    const auto residual = [&](int l) {
         if (MODE >= 2) {
             __syncthreads();
             for (int i = tid; i < d; i += 128) s_q[i] = s_q0[i] - cent[(size_t)l * d + i];
             __syncthreads();
         }
-        const int64_t beg = list_off[l], end = list_off[l + 1];
-        int64_t cbase = 0;  // MAT: slot of row i is cbase + i
-        if constexpr (MAT) cbase = coff[q * (nprobe + 1) + p] - beg;
+    };
+    pr.for_each_list<false>(sink, residual, [&](int64_t beg, int64_t end, float) {
         for (int64_t base = beg + warp * U; base < end; base += 4 * U) {
             float acc[U];
             uint32_t vid[U];
@@ -443,17 +439,11 @@ scan_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ c
                 const int64_t i = base + u;
                 float v = dfx_warp_butterfly(acc[u]);
                 if (MODE == 0) v = -v;
-                if constexpr (MAT) {
-                    if (lane == u && i < end) dfx_cand_store(part, cbase + i, v, vid[u]);
-                } else {
-                    uint32_t sec = 0;
-                    if (i < end && wt.admits(v, [&] { return vid[u]; }, sec))
-                        wt.push_uniform(v, sec);
-                }
+                sink.push_uniform(i < end, u, i, v, vid[u]);
             }
         }
-    }
-    if constexpr (!MAT) cta_merge_and_write<128>(wt, s_buf, cap, k, part + ((int64_t)q * ngroups + g) * k);
+    });
+    sink.finish(pr);
 }
 
 // =====================================================================================
@@ -920,7 +910,7 @@ static IvfPlan plan_ivf(dfx_index* idx, int64_t nq, int64_t k64) {
     if (p.family == ScanFamily::PqWide) {
         const size_t optin = (size_t)dfx_smem_optin();
         for (int t : {512, 256, 128}) {
-            if (dfx_pq_wide_smem(idx->M, t, p.mat ? 0 : p.cap) <= optin) {
+            if (dfx_pq_wide_smem(idx->M, t, p.cap, p.mat) <= optin) {
                 p.wide_threads = t;
                 break;
             }
@@ -930,7 +920,7 @@ static IvfPlan plan_ivf(dfx_index* idx, int64_t nq, int64_t k64) {
         DFX_REQUIRE(p.wide_threads > 0,
                     "IVF-PQ with " + std::to_string(idx->M) + " sub-quantizers at k=" + std::to_string(k) +
                         ": the distance table and the candidate queues need " +
-                        std::to_string(dfx_pq_wide_smem(idx->M, 128, p.cap)) +
+                        std::to_string(dfx_pq_wide_smem(idx->M, 128, p.cap, p.mat)) +
                         " bytes of shared memory per thread block, the device allows " + std::to_string(optin));
     }
     DFX_REQUIRE(!p.refine || p.rflat || idx->inv_valid, "IVF-PQR search: the id -> position map is not built");
@@ -955,6 +945,7 @@ static bool launch_list_scan(dfx_index* idx, const IvfPlan& p, const float* xq, 
                              cudaStream_t st) {
     const int d = idx->cfg.d, M = idx->M, ksub = idx->ksub, k = p.k, cap = p.cap, nprobe = p.nprobe;
     const unsigned grid = (unsigned)(qc * ngroups);
+    const size_t queues = dfx_scan_queue_smem(128, cap, p.mat);  // the 128-thread scans' candidate queues
     if (p.family == ScanFamily::Pq || p.family == ScanFamily::PqWide || p.family == ScanFamily::Pq4) {
         // K3: each query's [M][ksub] table (w_lut; the wide scan builds its own) and the exact
         // |q - c|^2 of its probed lists (w_dis0)
@@ -974,20 +965,19 @@ static bool launch_list_scan(dfx_index* idx, const IvfPlan& p, const float* xq, 
             DFX_LAUNCH(pq_fs_lut_kernel, (unsigned)qc, 256, dfx_pq_fs_lut_smem(d, M), st, xq, d, M, idx->dsub,
                        idx->codebooks.as<float>(), idx->w_lut.as<uint8_t>(), idx->w_dis0.as<float2>());
             const bool found = dispatch_int(PqMByEight{}, M, [&](auto MT) {
-                launch_scan(p.mat ? scan_pq_fs_kernel<MT, true> : scan_pq_fs_kernel<MT>, grid, 128,
-                            p.mat ? 0 : dfx_pq_fs_smem(cap), st, idx->w_lut.as<uint8_t>(), keys, nprobe, G, ngroups,
-                            idx->list_off.as<int64_t>(), idx->payload.as<uint8_t>(), idx->ids.as<int32_t>(), k, cap,
-                            part, coff);
+                launch_scan(p.mat ? scan_pq_fs_kernel<MT, true> : scan_pq_fs_kernel<MT>, grid, 128, queues, st,
+                            idx->w_lut.as<uint8_t>(), keys, nprobe, G, ngroups, idx->list_off.as<int64_t>(),
+                            idx->payload.as<uint8_t>(), idx->ids.as<int32_t>(), k, cap, part, coff);
             });
             DFX_REQUIRE(found, "IVF-PQ FastScan: no list scan for M=" + std::to_string(M));
             return false;
         }
         case ScanFamily::Pq4: {
             const bool found = dispatch_int(PqMByEight{}, M, [&](auto MT) {
-                launch_scan(p.mat ? scan_pq4_kernel<MT, true> : scan_pq4_kernel<MT>, grid, 128,
-                            p.mat ? 0 : dfx_pq4_smem(cap), st, idx->w_lut.as<float>(), idx->w_dis0.as<float>(), keys,
-                            nprobe, G, ngroups, idx->list_off.as<int64_t>(), idx->payload.as<uint8_t>(),
-                            idx->tvals.as<float>(), idx->ids.as<int32_t>(), k, cap, part, coff);
+                launch_scan(p.mat ? scan_pq4_kernel<MT, true> : scan_pq4_kernel<MT>, grid, 128, queues, st,
+                            idx->w_lut.as<float>(), idx->w_dis0.as<float>(), keys, nprobe, G, ngroups,
+                            idx->list_off.as<int64_t>(), idx->payload.as<uint8_t>(), idx->tvals.as<float>(),
+                            idx->ids.as<int32_t>(), k, cap, part, coff);
             });
             DFX_REQUIRE(found, "IVF-PQ with 4-bit codes: no list scan for M=" + std::to_string(M));
             return false;
@@ -998,7 +988,7 @@ static bool launch_list_scan(dfx_index* idx, const IvfPlan& p, const float* xq, 
             dfx_launch_scan_pq_il2_mat(idx, xq, qc, keys, nprobe, G, ngroups, part, coff, st);
             return false;
         case ScanFamily::PqWide: {
-            const size_t smem = dfx_pq_wide_smem(M, p.wide_threads, p.mat ? 0 : cap);
+            const size_t smem = dfx_pq_wide_smem(M, p.wide_threads, cap, p.mat);
             const int mt = (M == 128 || M == 96) ? M : 0;  // any other M % 4 == 0: 32-bit code loads
             dispatch_int(IntList<128, 96, 0>{}, mt, [&](auto MT) {
                 dispatch_int(IntList<512, 256, 128>{}, p.wide_threads, [&](auto THREADS) {
@@ -1012,7 +1002,7 @@ static bool launch_list_scan(dfx_index* idx, const IvfPlan& p, const float* xq, 
             return false;
         }
         case ScanFamily::Pq: {
-            const size_t smem = (size_t)M * ksub * 4 + (p.mat ? 0 : (size_t)4 * cap * 8);
+            const size_t smem = (size_t)M * ksub * 4 + queues;
             const int mt = (M == 8 || M == 16 || M == 32 || M == 64) ? M : 0;  // other M: padded to 64 with +0
             dispatch_int(IntList<8, 16, 32, 64, 0>{}, mt, [&](auto MT) {
                 launch_scan(p.mat ? scan_pq_kernel<MT, true> : scan_pq_kernel<MT>, grid, 128, smem, st,
@@ -1025,7 +1015,7 @@ static bool launch_list_scan(dfx_index* idx, const IvfPlan& p, const float* xq, 
         case ScanFamily::Rows: {
             // shared memory: the query; + the raw query (SQ16); + vmin and vdiff (SQ8)
             const int dq = (p.kind == DFX_IVF_SQ8) ? 4 * d : (p.kind == DFX_IVF_SQ16) ? 2 * d : d;
-            const size_t smem = (((size_t)dq * 4 + 15) / 16) * 16 + (p.mat ? 0 : (size_t)4 * cap * 8);
+            const size_t smem = (((size_t)dq * 4 + 15) / 16) * 16 + queues;
             // vectors in flight per warp: rows of up to 1 KB need 8 to cover the DRAM latency,
             // longer rows keep 4 (rows_inflight overrides)
             const int inflight = idx->rows_inflight ? idx->rows_inflight : (idx->row_bytes() <= 1024 ? 8 : 4);
