@@ -23,8 +23,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
-from bench_other_configs import card, timed  # noqa: E402
+import kind_bench as kb  # noqa: E402
 from distributed_faiss_b200 import engine  # noqa: E402
 from tests import oracle_sq8 as S  # noqa: E402
 
@@ -64,36 +63,23 @@ def main():
     assert torch.cuda.is_available(), "bench_large_k measures the GPU: no CUDA device"
     d, n, nlist, nprobe, nq = 128, int(os.environ.get("LARGE_K_BENCH_N", 10_000_000)), 4096, 32, 1000
     rounds, reps = 3, 5
-    step = 1_000_000
-    out = {"card": card(), "setup": {"d": d, "n": n, "nlist": nlist, "nprobe": nprobe, "nq": nq, "ks": KS,
-                                     "rounds": rounds, "reps_per_round": reps}}
-    synth = engine.Synth(1234, d, 16, 1, 1.0, 0.02, ngroups=max(1, n // 10), eps=0.01, delta=0.1)
-    rows = torch.randint(0, n, (nq,), dtype=torch.int64, generator=torch.Generator().manual_seed(1)).cuda()
-    xq_t = synth.rows(0, nq, rows_t=rows, noise_stream=7)
-    xs = xq_t[:32].cpu().numpy()
+    out = {"card": kb.card(), "setup": {"d": d, "n": n, "nlist": nlist, "nprobe": nprobe, "nq": nq, "ks": KS,
+                                        "rounds": rounds, "reps_per_round": reps}}
+    ds = kb.Dataset(d, n, nq, step=1_000_000)
+    xq_t, xs = ds.xq, ds.sample()
 
     for name, kind, M in (("ivf_pq_M32", engine.KIND_IVF_PQ, 32), ("ivf_sq8", engine.KIND_IVF_SQ8, 0)):
-        g = engine.GpuIndex(kind, d, engine.METRIC_L2, nlist=nlist, pq_m=M)
-        g.set_param("kmeans_niter", 10)
-        g.set_param("max_points_per_centroid", 64)
-        g.train_dev(synth.rows(0, 64 * nlist))
-        for r0 in range(0, n, step):
-            g.add_dev(synth.rows(r0, min(step, n - r0)))
-        g.finalize()
-        g.nprobe = nprobe
-        o = S.make_index(engine.KIND_NAMES[kind], d, metric=S.O.METRIC_L2, nlist=nlist, M=M)
-        o.set_state(g.get_state())
-        o.nprobe = nprobe
+        g = ds.fill(engine.GpuIndex(kind, d, engine.METRIC_L2, nlist=nlist, pq_m=M), nlist, nprobe)
+        o = kb.mirror(S.make_index(engine.KIND_NAMES[kind], d, metric=S.O.METRIC_L2, nlist=nlist, M=M), g, nprobe)
         lens = np.sort(np.diff(o.list_off))[::-1]
         res = {"candidate_row_bound": int(lens[:nprobe].sum())}
         for k in KS:
-            Dg, Ig = g.search(xs, k)
-            Do, Io = o.search(xs, k)
+            bit_exact = kb.same_arrays(g.search(xs, k), o.search(xs, k))
             g.search_dev(xq_t, k)
             ndis = g.last_stats()["ndis"]
-            batch = [timed(lambda: g.search_dev(xq_t, k), iters=reps) for _ in range(rounds)]
+            batch = [kb.timed(lambda: g.search_dev(xq_t, k), iters=reps) for _ in range(rounds)]
             r = {
-                "bit_exact_vs_oracle_32q": bool(np.array_equal(Dg, Do) and np.array_equal(Ig, Io)),
+                "bit_exact_vs_oracle_32q": bit_exact,
                 "ndis": ndis,
                 "batch_ms": float(np.median(batch)), "batch_ms_rounds": batch,
                 "kernels_us": kernel_breakdown(lambda: g.search_dev(xq_t, k), reps),

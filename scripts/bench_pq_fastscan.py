@@ -26,13 +26,9 @@ import json
 import os
 import sys
 
-import numpy as np
-import torch
-
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
-from bench_other_configs import card, timed  # noqa: E402
+import kind_bench as kb  # noqa: E402
 from distributed_faiss_b200 import engine  # noqa: E402
 from oracle import oracle as O  # noqa: E402
 from tests.oracle_pq_fs import OracleIVFPQFastScan  # noqa: E402
@@ -44,80 +40,40 @@ CASES = (("fs_M32", "fs", 32), ("pq4_M32", "pq4", 32), ("fs_M64", "fs", 64), ("p
 def main():
     d, n, nlist, nprobe, nq, k = 128, int(os.environ.get("FS_BENCH_N", 10_000_000)), 4096, 32, 1000, 10
     rounds, reps = 3, 10
-    step = 1_000_000
-    out = {"card": card(), "setup": {"d": d, "n": n, "nlist": nlist, "nprobe": nprobe, "nq": nq, "k": k,
-                                     "rounds": rounds, "reps_per_round": reps}}
-    synth = engine.Synth(1234, d, 16, 1, 1.0, 0.02, ngroups=max(1, n // 10), eps=0.01, delta=0.1)
-    rows = torch.randint(0, n, (nq,), dtype=torch.int64, generator=torch.Generator().manual_seed(1)).cuda()
-    xq_t = synth.rows(0, nq, rows_t=rows, noise_stream=7)
+    out = {"card": kb.card(), "setup": {"d": d, "n": n, "nlist": nlist, "nprobe": nprobe, "nq": nq, "k": k,
+                                        "rounds": rounds, "reps_per_round": reps}}
+    ds = kb.Dataset(d, n, nq, step=1_000_000)
+    ds.exact(k)
+    xs = ds.sample()
 
-    flat = engine.GpuIndex(engine.KIND_FLAT, d, engine.METRIC_L2)
-    flat.reserve(n)
-    for r0 in range(0, n, step):
-        flat.add_dev(synth.rows(r0, min(step, n - r0)))
-    exact = flat.search_dev(xq_t, k)[1].cpu().numpy()
-    del flat
-    torch.cuda.empty_cache()
-
-    shards, res = {}, {}
-    cent0 = off0 = None
+    cases, res = [], {}
+    same_lists = kb.SameLists()
     for name, what, M in CASES:
         kind = engine.KIND_IVF_PQ_FS if what == "fs" else engine.KIND_IVF_PQ
-        g = engine.GpuIndex(kind, d, engine.METRIC_L2, nlist=nlist, pq_m=M, pq_nbits=4)
-        g.set_param("kmeans_niter", 10)
-        g.set_param("max_points_per_centroid", 64)
-        g.train_dev(synth.rows(0, 64 * nlist))
-        for r0 in range(0, n, step):
-            g.add_dev(synth.rows(r0, min(step, n - r0)))
-        g.finalize()
-        g.nprobe = nprobe
-        cent, off = g.get_centroids(), g.get_array("list_off")
-        if cent0 is None:
-            cent0, off0 = cent, off
-        I = g.search_dev(xq_t, k)[1].cpu().numpy()
-        xs = xq_t[:32].cpu().numpy()
-        Dg, Ig = g.search(xs, k)
+        g = ds.fill(engine.GpuIndex(kind, d, engine.METRIC_L2, nlist=nlist, pq_m=M, pq_nbits=4), nlist, nprobe)
+        same = same_lists(g)
         if what == "fs":
             o = OracleIVFPQFastScan(d, nlist, M)
         else:
             o = O.make_index("ivf_pq", d, metric=O.METRIC_L2, nlist=nlist, M=M, nbits=4)
-        o.set_state(g.get_state())
-        o.nprobe = nprobe
-        Do, Io = o.search(xs, k)
-        del o
         row_bytes = M // 2 + 4 + (4 if what == "pq4" else 0)
         res[name] = {
             "M": M, "row_bytes_per_vector": row_bytes,
-            "recall_at_10": float(np.mean([len(set(a) & set(b)) / k for a, b in zip(I, exact)])),
-            "same_centroids_and_lists_as_fs_M32": bool(np.array_equal(cent, cent0) and np.array_equal(off, off0)),
-            "bit_exact_vs_oracle_32q": bool(np.array_equal(Dg, Do) and np.array_equal(Ig, Io)),
+            "recall_at_10": ds.recall(g, k),
+            "same_centroids_and_lists_as_fs_M32": same,
+            "bit_exact_vs_oracle_32q": kb.same_arrays(g.search(xs, k), kb.mirror(o, g, nprobe).search(xs, k)),
             "batch_ms_rounds": [], "scan_kernel_ms_rounds": [],
         }
-        shards[name] = g
+        del o
+        cases.append((name, g, 0, False))
         print(json.dumps({name: res[name]}), flush=True)
 
-    for _ in range(rounds):
-        for name, _, _ in CASES:
-            g = shards[name]
-            res[name]["batch_ms_rounds"].append(timed(lambda: g.search_dev(xq_t, k)))
-            g.profile(True)
-            for _ in range(reps):
-                g.search_dev(xq_t, k)
-            torch.cuda.synchronize()
-            scan_ms, _ = g.profile_read()
-            g.profile(False)
-            res[name]["scan_kernel_ms_rounds"].append(scan_ms / reps)
-            res[name]["ndis"] = g.last_stats()["ndis"]
-
+    kb.time_rounds(cases, res, ds.xq, k, rounds, reps)
     for name, _, M in CASES:
         r = res[name]
-        scan_ms = float(np.median(r["scan_kernel_ms_rounds"]))
         ndis, rb = r["ndis"], r["row_bytes_per_vector"]
-        scan_s = scan_ms * 1e-3
+        scan_s = r["scan_kernel_ms"] * 1e-3
         r.update({
-            "batch_ms": float(np.median(r["batch_ms_rounds"])), "scan_kernel_ms": scan_ms,
-            "scan_kernel_ms_min_max": [min(r["scan_kernel_ms_rounds"]), max(r["scan_kernel_ms_rounds"])],
-            "qps": nq / float(np.median(r["batch_ms_rounds"])) * 1e3,
             "vectors_per_s": ndis / scan_s, "lookups_per_s": ndis * M / scan_s,
             "row_GBps": ndis * rb / scan_s / 1e9, "row_fraction_of_hbm": ndis * rb / scan_s / HBM_BPS,
         })

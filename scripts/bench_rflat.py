@@ -3,7 +3,7 @@
 on the stored fp32 rows by rflat_refine_kernel) against the plain codec shards and IVF-Flat on one H100.
 
 Shards: d = 128, nlist 4096, nprobe 32, 1 000 device-resident queries, k = 10, on the two datasets of
-scripts/bench_pq_refine.py (RFLAT_BENCH_DATASETS picks one), RFLAT_BENCH_N (default 10M) vectors each:
+scripts/kind_bench.py (RFLAT_BENCH_DATASETS picks one), RFLAT_BENCH_N (default 10M) vectors each:
   bench      the bench generator (bench.py's defaults: near-duplicate groups, low intrinsic dimension)
   clustered  the same generator as plain clustered data: 10 000 Gaussian clusters in 16 dimensions,
              no near-duplicate groups, per-row noise in all 128
@@ -27,14 +27,11 @@ import json
 import os
 import sys
 
-import numpy as np
 import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, os.path.join(ROOT, "scripts"))
-from bench_other_configs import card, timed  # noqa: E402
-from bench_pq_refine import DATASETS  # noqa: E402
+import kind_bench as kb  # noqa: E402
 from distributed_faiss_b200 import engine  # noqa: E402
 from tests.oracle_rflat import make_rflat  # noqa: E402
 
@@ -51,104 +48,46 @@ def plain_copy(g, kind, d, nlist, M, nbits):
     return p
 
 
-def run_dataset(name, p, d, n, nlist, nprobe, nq, k, rounds, reps, step=1_000_000):
-    ngroups = max(1, n // p["groups_per"]) if p["groups_per"] else 0
-    if ngroups:
-        ngroups = max(p["nclusters"], ngroups // p["nclusters"] * p["nclusters"])
-    synth = engine.Synth(1234, d, p["r"], p["nclusters"], p["sigma"], p["sigma_q"], ngroups=ngroups, eps=p["eps"],
-                         delta=p["delta"])
-    rows = torch.randint(0, n, (nq,), dtype=torch.int64, generator=torch.Generator().manual_seed(1)).cuda()
-    xq_t = synth.rows(0, nq, rows_t=rows, noise_stream=7)
-    xs = xq_t[:32].cpu().numpy()
+def run_dataset(name, p, d, n, nlist, nprobe, nq, k, rounds, reps):
+    ds = kb.Dataset(d, n, nq, step=1_000_000, **p)
+    xs = ds.sample()
+    ds.exact(k)
 
-    def fill(g):
-        g.set_param("kmeans_niter", 10)
-        g.set_param("max_points_per_centroid", 64)
-        g.train_dev(synth.rows(0, 64 * nlist))
-        g.reserve(n)
-        for r0 in range(0, n, step):
-            g.add_dev(synth.rows(r0, min(step, n - r0)))
-        g.finalize()
-        g.nprobe = nprobe
-
-    flat = engine.GpuIndex(engine.KIND_FLAT, d, engine.METRIC_L2)
-    flat.reserve(n)
-    for r0 in range(0, n, step):
-        flat.add_dev(synth.rows(r0, min(step, n - r0)))
-    exact = flat.search_dev(xq_t, k)[1].cpu().numpy()
-    del flat
-    torch.cuda.empty_cache()
-
-    def recall(g):
-        I = g.search_dev(xq_t, k)[1].cpu().numpy()
-        return float(np.mean([len(set(a) & set(b)) / k for a, b in zip(I, exact)]))
-
-    cases, res = [], {}   # (case name, shard, k_factor or 0)
-    ivf = engine.GpuIndex(engine.KIND_IVF_FLAT, d, engine.METRIC_L2, nlist=nlist)
-    fill(ivf)
-    cent0, off0 = ivf.get_centroids(), ivf.get_array("list_off")
-    cases.append(("IVF-Flat", ivf, 0))
-    res["IVF-Flat"] = {"bytes_per_vector_stored": 4 * d + 4, "recall_at_10": recall(ivf)}
+    cases, res = [], {}   # (case name, shard, k_factor or 0, whether it re-ranks)
+    same_lists = kb.SameLists()
+    ivf = ds.fill(engine.GpuIndex(engine.KIND_IVF_FLAT, d, engine.METRIC_L2, nlist=nlist), nlist, nprobe, reserve=True)
+    same_lists(ivf)
+    cases.append(("IVF-Flat", ivf, 0, False))
+    res["IVF-Flat"] = {"bytes_per_vector_stored": 4 * d + 4, "recall_at_10": ds.recall(ivf, k)}
     for codec, kind, kname, M, nbits in CODECS:
         g = engine.GpuIndex(kind, d, engine.METRIC_L2, nlist=nlist, pq_m=M, pq_nbits=nbits, refine_flat=True)
-        fill(g)
-        same = bool(np.array_equal(g.get_centroids(), cent0) and np.array_equal(g.get_array("list_off"), off0))
+        ds.fill(g, nlist, nprobe, reserve=True)
+        same = same_lists(g)
         plain = plain_copy(g, kind, d, nlist, M, nbits)
         plain.nprobe = nprobe
         row = (M if nbits == 8 else M // 2) + (8 if nbits == 8 else 4)   # code (+ t-value) + id
-        cases.append((codec, plain, 0))
-        res[codec] = {"bytes_per_vector_stored": row, "recall_at_10": recall(plain),
+        cases.append((codec, plain, 0, False))
+        res[codec] = {"bytes_per_vector_stored": row, "recall_at_10": ds.recall(plain, k),
                       "same_centroids_and_lists_as_IVF_Flat": same}
-        o = make_rflat(kname, d, nlist, M)
-        o.set_state(g.get_state())
-        o.nprobe = nprobe
+        o = kb.mirror(make_rflat(kname, d, nlist, M), g, nprobe)
         for kf in K_FACTORS:
             case = f"{codec},RFlat x{kf}"
             g.set_param("k_factor", kf)
             o.k_factor = float(kf)
-            Dg, Ig = g.search(xs, k)
-            Do, Io = o.search(xs, k)
-            cases.append((case, g, kf))
-            res[case] = {"bytes_per_vector_stored": row + 4 * d, "k_first_stage": k * kf, "recall_at_10": recall(g),
-                         "same_centroids_and_lists_as_IVF_Flat": same,
-                         "bit_exact_vs_oracle_32q": bool(np.array_equal(Dg, Do) and np.array_equal(Ig, Io)),
-                         "gather_bytes": nq * k * kf * 4 * d}
+            bit_exact = kb.same_arrays(g.search(xs, k), o.search(xs, k))
+            cases.append((case, g, kf, True))
+            res[case] = {"bytes_per_vector_stored": row + 4 * d, "k_first_stage": k * kf,
+                         "recall_at_10": ds.recall(g, k), "same_centroids_and_lists_as_IVF_Flat": same,
+                         "bit_exact_vs_oracle_32q": bit_exact, "gather_bytes": nq * k * kf * 4 * d}
         del o
-        for case in [c for c, _, _ in cases if c.startswith(codec)]:
+        for case in [c for c, _, _, _ in cases if c.startswith(codec)]:
             print(json.dumps({name: {case: res[case]}}), flush=True)
-    for r in res.values():
-        r.update(batch_ms_rounds=[], scan_kernel_ms_rounds=[], refine_ms_rounds=[])
 
-    for _ in range(rounds):
-        for case, g, kf in cases:
-            if kf:
-                g.set_param("k_factor", kf)
-            res[case]["batch_ms_rounds"].append(timed(lambda: g.search_dev(xq_t, k)))
-            g.profile(True)
-            for _ in range(reps):
-                g.search_dev(xq_t, k)
-            torch.cuda.synchronize()
-            if kf:
-                res[case]["refine_ms_rounds"].append(g.get_param("refine_ms") / reps)
-            scan_ms, _ = g.profile_read()
-            g.profile(False)
-            res[case]["scan_kernel_ms_rounds"].append(scan_ms / reps)
-            res[case]["ndis"] = g.last_stats()["ndis"]
-
-    for case, _, kf in cases:
-        r = res[case]
-        r.update({
-            "batch_ms": float(np.median(r["batch_ms_rounds"])),
-            "scan_kernel_ms": float(np.median(r["scan_kernel_ms_rounds"])),
-            "scan_kernel_ms_min_max": [min(r["scan_kernel_ms_rounds"]), max(r["scan_kernel_ms_rounds"])],
-            "qps": nq / float(np.median(r["batch_ms_rounds"])) * 1e3,
-        })
+    kb.time_rounds(cases, res, ds.xq, k, rounds, reps)
+    for case, _, kf, _ in cases:
         if kf:
-            r["refine_ms"] = float(np.median(r["refine_ms_rounds"]))
-            r["refine_ms_min_max"] = [min(r["refine_ms_rounds"]), max(r["refine_ms_rounds"])]
+            r = res[case]
             r["gather_share_of_hbm_peak"] = r["gather_bytes"] / (r["refine_ms"] * 1e-3) / HBM_PEAK
-        else:
-            del r["refine_ms_rounds"]
     del cases
     torch.cuda.empty_cache()
     return res
@@ -157,10 +96,10 @@ def run_dataset(name, p, d, n, nlist, nprobe, nq, k, rounds, reps, step=1_000_00
 def main():
     d, n, nlist, nprobe, nq, k = 128, int(os.environ.get("RFLAT_BENCH_N", 10_000_000)), 4096, 32, 1000, 10
     rounds, reps = 3, 10
-    out = {"card": card(), "setup": {"d": d, "n": n, "nlist": nlist, "nprobe": nprobe, "nq": nq, "k": k,
-                                     "k_factors": K_FACTORS, "rounds": rounds, "reps_per_round": reps}}
-    for name in os.environ.get("RFLAT_BENCH_DATASETS", ",".join(DATASETS)).split(","):
-        out[name] = run_dataset(name, DATASETS[name], d, n, nlist, nprobe, nq, k, rounds, reps)
+    out = {"card": kb.card(), "setup": {"d": d, "n": n, "nlist": nlist, "nprobe": nprobe, "nq": nq, "k": k,
+                                        "k_factors": K_FACTORS, "rounds": rounds, "reps_per_round": reps}}
+    for name in os.environ.get("RFLAT_BENCH_DATASETS", ",".join(kb.DATASETS)).split(","):
+        out[name] = run_dataset(name, kb.DATASETS[name], d, n, nlist, nprobe, nq, k, rounds, reps)
     print(json.dumps(out, indent=1))
 
 
