@@ -38,10 +38,15 @@ struct DfxError {
 // every kernel launch goes through this so that dfx_launch_count() is honest
 #ifdef DFX_EMU
 // CPU emulator build (tests/emu/, never a product build): the kernel runs on the fiber SIMT
-// runtime, one CTA after the other, synchronously
+// runtime, one CTA after the other, synchronously.  Every launch is recorded so that tests can
+// tell which instantiation a search ran (tests/emu/emu_simt_impl.cpp, dfx_emu_launch_log).  The
+// recorder is weak: an emulator build whose runtime does not define it records nothing.
+__attribute__((weak)) void dfx_emu_record_launch(const void* kernel);
 #define DFX_LAUNCH(kernel, grid, block, smem, stream, ...)                                      \
     do {                                                                                        \
         const dim3 _g(grid), _b(block);                                                         \
+        const auto _kfn = kernel;                                                               \
+        if (dfx_emu_record_launch) dfx_emu_record_launch(reinterpret_cast<const void*>(_kfn));  \
         simt::launch3(_g.x, _g.y, _b.x, (size_t)(smem), [&]() { kernel(__VA_ARGS__); });         \
         g_dfx_launches.fetch_add(1, std::memory_order_relaxed);                                 \
     } while (0)

@@ -990,15 +990,23 @@ static bool launch_list_scan(dfx_index* idx, const IvfPlan& p, const float* xq, 
         case ScanFamily::PqWide: {
             const size_t smem = dfx_pq_wide_smem(M, p.wide_threads, cap, p.mat);
             const int mt = (M == 128 || M == 96) ? M : 0;  // any other M % 4 == 0: 32-bit code loads
+            // M = 96 never takes 128 threads on a device that opts in to 232448 B (sm_90): at 256
+            // threads the largest queues (k <= 1024, cap = 2048) take 96 KB of table + 8 warps x 2048
+            // x 8 B = 229376 B.  So <96, 128> is not instantiated; a device that offers less is refused.
+            bool found = false;
             dispatch_int(IntList<128, 96, 0>{}, mt, [&](auto MT) {
-                dispatch_int(IntList<512, 256, 128>{}, p.wide_threads, [&](auto THREADS) {
+                const auto launch = [&](auto THREADS) {
                     launch_scan(p.mat ? scan_pq_wide_kernel<MT, 512, true> : scan_pq_wide_kernel<MT, THREADS>, grid,
                                 p.wide_threads, smem, st, xq, d, M, idx->dsub, idx->codebooks.as<float>(),
                                 idx->w_dis0.as<float>(), keys, nprobe, G, ngroups, idx->list_off.as<int64_t>(),
                                 idx->payload.as<uint8_t>(), idx->tvals.as<float>(), idx->ids.as<int32_t>(), k, cap,
                                 part, coff);
-                });
+                };
+                if constexpr (MT == 96) found = dispatch_int(IntList<512, 256>{}, p.wide_threads, launch);
+                else found = dispatch_int(IntList<512, 256, 128>{}, p.wide_threads, launch);
             });
+            DFX_REQUIRE(found, "IVF-PQ with " + std::to_string(M) + " sub-quantizers: no list scan of " +
+                                   std::to_string(p.wide_threads) + " threads");
             return false;
         }
         case ScanFamily::Pq: {
