@@ -635,62 +635,62 @@ __device__ __forceinline__ float screen_tol(const ScreenTol& t, int64_t row, flo
     return rel * sc + SCREEN_TOL_CENTRED * (t.cmax2c + 2.f * sc) + t.raw * (t.cmax2 + 2.f * s) + 1e-30f;
 }
 // "the selected groups may not be all that matter": the G-th (last) selected group is itself
-// within the tolerance, so an unselected group could be too -> the row is re-done exactly
-__device__ __forceinline__ bool screen_overflow(const int32_t* __restrict__ groups, int64_t row, int G, int ng,
-                                                const float* __restrict__ gmin, float thr) {
-    if (G >= ng) return false;  // every group is selected
-    const int gl = groups[row * G + G - 1];
-    return gl >= 0 && gmin[row * ng + gl] <= thr;
+// within the tolerance, so an unselected group could be too -> the row is re-done exactly.
+// last = the minimum of the G-th selected group, NaN (never within) when every group is selected.
+__device__ __forceinline__ float screen_last_min(const int32_t* __restrict__ groups, int64_t row, int G, int ng,
+                                                 const float* __restrict__ gmin) {
+    const int gl = G < ng ? groups[row * G + G - 1] : -1;
+    return gl >= 0 ? gmin[row * ng + gl] : __int_as_float(0x7fc00000);
 }
 // The decide threshold of a row, t + tol with t = the nprobe-th smallest group minimum (inf when
 // there are fewer groups than probes: nothing is pruned).  A row with more near-ties than
 // selected groups is queued for tc_exact_rows_kernel.  ovf = [overflow rows, rows that the FAST
 // tolerance would overflow (counted by PRECISE launches for the AUTO mode), row list ...].
+// t and last as the selection left them (decide_rows_kernel holds both in registers).
+__device__ __forceinline__ float screen_threshold(float t, float last, int64_t row, const ScreenTol& tol,
+                                                  int32_t* __restrict__ ovf) {
+    const float thr = t + screen_tol(tol, row, tol.rel);
+    if (last <= thr) ovf[2 + atomicAdd(&ovf[0], 1)] = (int32_t)row;
+    if (tol.rel_fast > 0.f && last <= t + screen_tol(tol, row, tol.rel_fast)) atomicAdd(&ovf[1], 1);
+    return thr;
+}
+// the same from the selected groups in global memory ([rows][G], -1 = none)
 __device__ __forceinline__ float screen_threshold(const int32_t* __restrict__ groups, int64_t row, int G, int nprobe,
                                                   int ng, const float* __restrict__ gmin, const ScreenTol& tol,
                                                   int32_t* __restrict__ ovf) {
     const int gk = (nprobe <= G) ? groups[row * G + nprobe - 1] : -1;
     const float t = gk >= 0 ? gmin[row * ng + gk] : __int_as_float(0x7f800000);
-    const float thr = t + screen_tol(tol, row, tol.rel);
-    if (screen_overflow(groups, row, G, ng, gmin, thr)) ovf[2 + atomicAdd(&ovf[0], 1)] = (int32_t)row;
-    if (tol.rel_fast > 0.f && screen_overflow(groups, row, G, ng, gmin, t + screen_tol(tol, row, tol.rel_fast)))
-        atomicAdd(&ovf[1], 1);
-    return thr;
+    return screen_threshold(t, screen_last_min(groups, row, G, ng, gmin), row, tol, ovf);
 }
-// Can a selected group (o = row * ng + group) still matter?  Only if its minimum is within the
-// threshold (the return value); then through all 32 columns if its runner-up is within it too
-// (expand, which means nothing for a group that is not live), otherwise through its arg-min
-// column alone.  Neither load waits for the other's compare.
-__device__ __forceinline__ bool group_live(const float* __restrict__ gmin, const float* __restrict__ gmin2,
-                                           int64_t o, float thr, bool& expand) {
-    expand = gmin2[o] <= thr;
-    return gmin[o] <= thr;
+// Can a selected group (minimum m1, runner-up m2) still matter?  Only if its minimum is within
+// the threshold (the return value); then through all 32 columns if its runner-up is within it
+// too (expand, which means nothing for a group that is not live), otherwise through its arg-min
+// column alone.
+__device__ __forceinline__ bool group_live(float m1, float m2, float thr, bool& expand) {
+    expand = m2 <= thr;
+    return m1 <= thr;
 }
 
-// The G (<= 32) smallest group minima of a row, ascending by (value, group): one warp per row.
+// The G (<= 32) smallest group minima of a row, ascending by (value, group), by one warp: lane r
+// gets the composite (value, group) of the r-th, NONE from lane G on.
 //   1. every lane takes the minimum of its n/32 values; the G-th smallest of those 32 lane
 //      minima, B, bounds the answer from above (G different lanes hold a value <= B);
-//   2. the values <= B are collected (a few dozen at most in practice) into a per-warp buffer;
+//   2. the values <= B are collected (a few dozen at most in practice) into buf, the warp's CAP
+//      slots of shared memory;
 //   3. the buffer is bitonic-sorted by the warp and the first G entries are kept.
 // Exact for any input; if more than CAP values are <= B (massive ties) the row falls back to
 // G rounds of warp arg-min.  ~10x fewer instructions than G x n compare rounds.
 // Two levels (fine != nullptr): `coarse` holds the minimum of every FINE_PER = 4 consecutive
 // groups (one 128-column tile of the screening kernel, written by its epilogue) -- steps 1-3 run
-// on the n / 4 tile minima, then the 4 G groups of the G smallest tiles are sorted and the first
-// G kept.  The G smallest groups always lie in the G smallest tiles: a group g outside them
-// would have G tiles, each holding a group with (minimum, index) below g's, before it.
+// on the n / 4 tile minima, then the G smallest of the 4 G groups of the G smallest tiles are
+// merged in registers.  The G smallest groups always lie in the G smallest tiles: a group g
+// outside them would have G tiles, each holding a group with (minimum, index) below g's, before it.
 template <int CAP>
-__global__ void __launch_bounds__(256)
-topg_collect_kernel(const float* __restrict__ coarse, int64_t nq, int n, int G, const float* __restrict__ fine,
-                    int n_fine, int32_t* __restrict__ groups) {
+__device__ __forceinline__ uint64_t topg_select_row(const float* __restrict__ g, int n, int G,
+                                                    const float* __restrict__ fine, int n_fine, uint64_t* buf,
+                                                    int lane) {
     constexpr int FINE_PER = 4;
-    static_assert(CAP >= 32 * FINE_PER, "the expansion of 32 tiles must fit the buffer");
-    __shared__ uint64_t s_buf[8][CAP];
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t row = (int64_t)blockIdx.x * 8 + warp;
-    if (row >= nq) return;
-    const float* g = coarse + row * n;
-    uint64_t* buf = s_buf[warp];
+    static_assert(CAP >= 32 && (CAP & (CAP - 1)) == 0, "the sorted buffer is a power of two >= 32");
     // (n <= 512, the usual case -- 65 536 lists = 512 tiles: the row is loaded ONCE, 16 independent
     // loads per lane, and both passes run on registers; the loops below were bound by one L2
     // latency per iteration)
@@ -720,20 +720,11 @@ topg_collect_kernel(const float* __restrict__ coarse, int64_t nq, int n, int G, 
         }
     }
     const uint64_t x = dfx_warp_sort32_asc(lmin, lane);  // the 32 lane minima, ascending by lane
-    const int gth = min(G, 32) - 1;
-    const uint64_t bound = __shfl_sync(0xffffffffu, x, gth);  // G-th smallest lane minimum
+    const uint64_t bound = __shfl_sync(0xffffffffu, x, G - 1);  // G-th smallest lane minimum
     // 2. collect everything <= bound
     int cnt = 0;
     bool overflow = false;
-    for (int j0 = 0, it = 0; j0 < n; j0 += 32, it++) {
-        const int j = j0 + lane;
-        float gv = 0.f;
-        if (in_regs) {
-#pragma unroll
-            for (int i = 0; i < REGV; i++) gv = (i == it) ? rv[i] : gv;  // rv[it] without local memory
-        } else if (j < n) {
-            gv = g[j];
-        }
+    auto collect = [&](int j, float gv) {  // lanes j0 .. j0 + 31 of one warp-uniform step
         const uint64_t c = (j < n) ? dfx_comp(gv, (uint32_t)j) : DFX_COMP_NONE;
         const bool want = c <= bound && c != DFX_COMP_NONE;
         const unsigned mask = __ballot_sync(0xffffffffu, want);
@@ -743,10 +734,16 @@ topg_collect_kernel(const float* __restrict__ coarse, int64_t nq, int n, int G, 
             cnt += __popc(mask);
             if (cnt > CAP) overflow = true;
         }
+    };
+    if (in_regs) {
+#pragma unroll
+        for (int i = 0; i < REGV; i++)
+            if (32 * i < n) collect(lane + 32 * i, rv[i]);
+    } else {
+        for (int j0 = 0; j0 < n; j0 += 32) collect(j0 + lane, j0 + lane < n ? g[j0 + lane] : 0.f);
     }
-    int P = 32;
     if (!overflow) {
-        P = dfx_warp_sort_buf(buf, cnt, lane);  // 3. sort the candidates
+        dfx_warp_sort_buf(buf, cnt, lane);  // 3. sort the candidates (padded to >= 32 slots)
     } else {
         // fallback: G rounds of "smallest composite above the previous pick", left in buf[0..G)
         uint64_t prev = 0;
@@ -767,26 +764,35 @@ topg_collect_kernel(const float* __restrict__ coarse, int64_t nq, int n, int G, 
         }
         __syncwarp();
     }
-    if (fine) {  // second level: the groups of the G smallest tiles
-        const uint64_t tc_ = (lane < G && (overflow || lane < P)) ? buf[lane] : DFX_COMP_NONE;
-        __syncwarp();
-        const float* f = fine + row * n_fine;
+    uint64_t sel = lane < G ? buf[lane] : DFX_COMP_NONE;
+    __syncwarp();  // buf is free again
+    if (fine) {  // second level: the 32 smallest of the 4 groups of each selected tile
+        uint64_t fc[FINE_PER];
 #pragma unroll
         for (int j = 0; j < FINE_PER; j++) {
-            const int64_t gi = (int64_t)(uint32_t)tc_ * FINE_PER + j;
-            buf[lane * FINE_PER + j] =
-                (tc_ != DFX_COMP_NONE && gi < n_fine) ? dfx_comp(f[gi], (uint32_t)gi) : DFX_COMP_NONE;
+            const int64_t gi = (int64_t)(uint32_t)sel * FINE_PER + j;
+            fc[j] = (sel != DFX_COMP_NONE && gi < n_fine) ? dfx_comp(fine[gi], (uint32_t)gi) : DFX_COMP_NONE;
         }
-        __syncwarp();
-        P = dfx_warp_sort_buf(buf, 32 * FINE_PER, lane);
-        overflow = false;
+        sel = dfx_warp_sort32_asc(fc[0], lane);
+#pragma unroll
+        for (int j = 1; j < FINE_PER; j++) sel = dfx_warp_merge_sorted32(sel, dfx_warp_sort32_asc(fc[j], lane), lane);
+        if (lane >= G) sel = DFX_COMP_NONE;
     }
-    for (int r = lane; r < G; r += 32) {
-        const uint64_t c = (overflow || r < P) ? buf[r] : DFX_COMP_NONE;
-        groups[row * G + r] = (c == DFX_COMP_NONE) ? -1 : (int32_t)(uint32_t)c;
-    }
+    return sel;
 }
-
+// the selection above for a row per warp -> groups[row][0..G) (-1 = none), G <= 32
+template <int CAP>
+__global__ void __launch_bounds__(256)
+topg_collect_kernel(const float* __restrict__ coarse, int64_t nq, int n, int G, const float* __restrict__ fine,
+                    int n_fine, int32_t* __restrict__ groups) {
+    __shared__ uint64_t s_buf[8][CAP];
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t row = (int64_t)blockIdx.x * 8 + warp;
+    if (row >= nq) return;
+    const uint64_t c = topg_select_row<CAP>(coarse + row * n, n, G, fine ? fine + row * n_fine : nullptr, n_fine,
+                                            s_buf[warp], lane);
+    if (lane < G) groups[row * G + lane] = (c == DFX_COMP_NONE) ? -1 : (int32_t)(uint32_t)c;
+}
 // exact canonical fp32 values of the candidates.
 //   MODE 0: out[row][c] = comp(value, centroid) for every candidate slot (NONE for unused slots)
 //   MODE 1: write the arg-min centroid to assign[row]
@@ -824,7 +830,7 @@ rerank_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent
             if (gid >= 0) {
                 const int64_t o = row * ng + gid;
                 bool expand;
-                const bool live = group_live(gmin, gmin2, o, thr, expand) && (expand || (c & 31) == (int)gargc[o]);
+                const bool live = group_live(gmin[o], gmin2[o], thr, expand) && (expand || (c & 31) == (int)gargc[o]);
                 const int64_t col = (int64_t)gid * 32 + (c & 31);
                 if (live && col < nlist)
                     comp = dfx_comp(dfx_rank_value(dfx_dot_seqk(s_q, cent + col * d, d), metric, cnorm, col),
@@ -862,15 +868,57 @@ rerank_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent
     }
 }
 
-// Search path, nprobe <= 32 and G <= 64: the same decision as rerank_kernel<2>, one WARP per
-// query instead of one 128-thread CTA.  rerank_kernel<2> spends a whole CTA on a query although
-// only ~9 candidates per query survive the screening: 128 threads walk 512 candidate slots of
-// which a handful are live, then a block-wide sort.  Here: lanes own the selected groups, live
-// candidates are compacted into a per-warp list (arg-min column, or all 32 columns of a group
-// whose runner-up is within the tolerance), each lane evaluates one candidate in the canonical
-// seq-k order, and the nprobe smallest come out of a register bitonic network.  The candidate set
-// is a superset of the true top-nprobe for any tolerance >= the screening error, so the keys are
-// identical to rerank_kernel<2>'s.
+// ---- the exact re-rank of a row by one warp (rerank2_kernel, decide_rows_kernel): lanes own the
+// selected groups, live candidates are compacted into a per-warp list (arg-min column, or all 32
+// columns of a group whose runner-up is within the tolerance), each lane evaluates one candidate
+// in the canonical seq-k order, and the nprobe smallest come out of a register bitonic network.
+// The candidate set is a superset of the true top-nprobe for any tolerance >= the screening error,
+// so the keys are identical to rerank_kernel<2>'s.
+// Appends this step's 32 groups (gid -1 = none; live / expand per group_live, argc = the arg-min
+// column) to s_cand[cnt ..), returns the new count.
+__device__ __forceinline__ int decide_add_candidates(int gid, bool live, bool expand, int argc, int64_t nlist,
+                                                     int32_t* __restrict__ s_cand, int cnt, int lane) {
+    expand = live && expand;
+    const bool single = live && !expand && ((int64_t)gid * 32 + argc) < nlist;
+    const unsigned ms = __ballot_sync(0xffffffffu, single);
+    if (single) s_cand[cnt + __popc(ms & ((1u << lane) - 1u))] = gid * 32 + argc;
+    cnt += __popc(ms);
+    unsigned me = __ballot_sync(0xffffffffu, expand);
+    while (me) {  // rare: a group whose runner-up cannot be ruled out contributes all its columns
+        const int src = __ffs((int)me) - 1;
+        me &= me - 1;
+        const int eg = __shfl_sync(0xffffffffu, gid, src);
+        const int64_t col = (int64_t)eg * 32 + lane;
+        const bool ok = col < nlist;
+        const unsigned mo = __ballot_sync(0xffffffffu, ok);
+        if (ok) s_cand[cnt + __popc(mo & ((1u << lane) - 1u))] = (int32_t)col;
+        cnt += __popc(mo);
+    }
+    return cnt;
+}
+// exact canonical values of the cnt candidates, 32 at a time; keys_row[0 .. nprobe) = the
+// nprobe (<= 32) smallest, ascending (-1 = none)
+__device__ __forceinline__ void decide_exact_keys(const float* __restrict__ s_q, int d, const float* __restrict__ cent,
+                                                  const float* __restrict__ cnorm, int metric,
+                                                  const int32_t* __restrict__ s_cand, int cnt, int nprobe,
+                                                  int32_t* __restrict__ keys_row, int lane) {
+    __syncwarp();
+    uint64_t kept = DFX_COMP_NONE;
+    for (int c0 = 0; c0 < cnt; c0 += 32) {
+        uint64_t comp = DFX_COMP_NONE;
+        if (c0 + lane < cnt) {
+            const int64_t col = s_cand[c0 + lane];
+            comp = dfx_comp(dfx_rank_value(dfx_dot_seqk(s_q, cent + col * d, d), metric, cnorm, col), (uint32_t)col);
+        }
+        kept = dfx_warp_merge_sorted32(kept, dfx_warp_sort32_asc(comp, lane), lane);
+    }
+    if (lane < nprobe) keys_row[lane] = (kept == DFX_COMP_NONE) ? -1 : (int32_t)(uint32_t)kept;
+}
+
+// Search path, nprobe <= 32 and G <= 64 groups selected by tc_select_groups (the shapes that
+// decide_rows_kernel below does not take): the same decision as rerank_kernel<2>, one WARP per
+// query instead of one 128-thread CTA, which would spend 128 threads on 512 candidate slots of
+// which a handful are live, then a block-wide sort.
 constexpr int RR2_WARPS = 4;
 __global__ void __launch_bounds__(RR2_WARPS * 32)
 rerank2_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent, const float* __restrict__ cnorm,
@@ -890,7 +938,6 @@ rerank2_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cen
     float thr = 0.f;
     if (lane == 0) thr = screen_threshold(groups, row, G, nprobe, ng, gmin, tol, ovf);
     thr = __shfl_sync(0xffffffffu, thr, 0);
-    // ---- candidate list: one entry for a live group's arg-min column, 32 for an expanded group
     int cnt = 0;
     for (int g0 = 0; g0 < G; g0 += 32) {
         const int gi = g0 + lane;
@@ -901,41 +948,69 @@ rerank2_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cen
             gid = groups[row * G + gi];
             if (gid >= 0) {
                 const int64_t o = row * ng + gid;
-                live = group_live(gmin, gmin2, o, thr, expand);
-                expand = live && expand;
+                live = group_live(gmin[o], gmin2[o], thr, expand);
                 argc = (int)gargc[o];
             }
         }
-        const bool single = live && !expand && ((int64_t)gid * 32 + argc) < nlist;
-        const unsigned ms = __ballot_sync(0xffffffffu, single);
-        if (single) s_cand[cnt + __popc(ms & ((1u << lane) - 1u))] = gid * 32 + argc;
-        cnt += __popc(ms);
-        unsigned me = __ballot_sync(0xffffffffu, expand);
-        while (me) {  // rare: a group whose runner-up cannot be ruled out contributes all its columns
-            const int src = __ffs((int)me) - 1;
-            me &= me - 1;
-            const int eg = __shfl_sync(0xffffffffu, gid, src);
-            const int64_t col = (int64_t)eg * 32 + lane;
-            const bool ok = col < nlist;
-            const unsigned mo = __ballot_sync(0xffffffffu, ok);
-            if (ok) s_cand[cnt + __popc(mo & ((1u << lane) - 1u))] = (int32_t)col;
-            cnt += __popc(mo);
-        }
+        cnt = decide_add_candidates(gid, live, expand, argc, nlist, s_cand, cnt, lane);
     }
-    __syncwarp();
-    // ---- exact canonical values, 32 candidates at a time; keep the 32 smallest composites
-    uint64_t kept = DFX_COMP_NONE;
-    for (int c0 = 0; c0 < cnt; c0 += 32) {
-        uint64_t comp = DFX_COMP_NONE;
-        if (c0 + lane < cnt) {
-            const int64_t col = s_cand[c0 + lane];
-            comp = dfx_comp(dfx_rank_value(dfx_dot_seqk(s_q, cent + col * d, d), metric, cnorm, col), (uint32_t)col);
-        }
-        kept = dfx_warp_merge_sorted32(kept, dfx_warp_sort32_asc(comp, lane), lane);
-    }
-    if (lane < nprobe) keys[row * nprobe + lane] = (kept == DFX_COMP_NONE) ? -1 : (int32_t)(uint32_t)kept;
+    decide_exact_keys(s_q, d, cent, cnorm, metric, s_cand, cnt, nprobe, keys + row * nprobe, lane);
 }
 
+// Search path, G <= 32 groups of ng >= 128 (the two-level selection; the bench shape): the whole
+// decide stage of a row by one warp, from the screening summary to the keys.  topg_select_row
+// leaves lane r with the r-th smallest selected group; the group's minimum is the value of its
+// composite, so the threshold, the overflow test and the liveness of a group need no load; only
+// the runner-up and the arg-min column of the selected groups are read, together with the query
+// row.  Nothing goes through global memory between the selection and the re-rank.
+// Per warp: the selection buffer (later the candidate list), then the row's query.
+constexpr int DECIDE_WARPS = 8;
+constexpr int DECIDE_CAP = 256;
+__host__ __device__ __forceinline__ size_t decide_slots(int G) {  // bytes: DECIDE_CAP composites or G x 32 columns
+    return (size_t)DECIDE_CAP * 8 > (size_t)G * 32 * 4 ? (size_t)DECIDE_CAP * 8 : (size_t)G * 32 * 4;
+}
+static size_t decide_rows_smem(int d, int G) {
+    return DECIDE_WARPS * (decide_slots(G) + (size_t)(d + 3) / 4 * 4 * 4);
+}
+__global__ void __launch_bounds__(DECIDE_WARPS * 32)
+decide_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent,
+                   const float* __restrict__ cnorm, int64_t nlist, int metric, const float* __restrict__ tmin,
+                   const float* __restrict__ gmin, const float* __restrict__ gmin2,
+                   const uint8_t* __restrict__ gargc, int ng, int G, int nprobe, ScreenTol tol, int64_t nrows,
+                   int32_t* __restrict__ keys, int32_t* __restrict__ ovf) {
+    DFX_DYN_SMEM(unsigned char, dr_smem, 16);
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int64_t row = (int64_t)blockIdx.x * DECIDE_WARPS + warp;
+    if (row >= nrows) return;  // whole warps leave; no block-wide barrier below
+    const size_t slots = decide_slots(G);
+    unsigned char* own = dr_smem + (size_t)warp * (slots + (size_t)(d + 3) / 4 * 4 * 4);
+    uint64_t* buf = reinterpret_cast<uint64_t*>(own);
+    int32_t* s_cand = reinterpret_cast<int32_t*>(own);  // once the selection is done with buf
+    float* s_q = reinterpret_cast<float*>(own + slots);
+    const int nt = ng / 4;
+    const uint64_t sel = topg_select_row<DECIDE_CAP>(tmin + row * nt, nt, G, gmin + row * ng, ng, buf, lane);
+    const int gid = (sel == DFX_COMP_NONE) ? -1 : (int32_t)(uint32_t)sel;
+    float m2 = 0.f;
+    int argc = 0;
+    if (gid >= 0) {
+        m2 = gmin2[row * ng + gid];
+        argc = (int)gargc[row * ng + gid];
+    }
+    for (int i = lane; i < d; i += 32) s_q[i] = Q[row * d + i];
+    // gmin of the lane's group (dfx_key2f gives back gmin + 0: -0 reads as +0, which no
+    // comparison below tells apart); t and last as screen_threshold(groups, ...) defines them
+    const float nan = __int_as_float(0x7fc00000), inf = __int_as_float(0x7f800000);
+    const float m1 = (gid >= 0) ? dfx_key2f((uint32_t)(sel >> 32)) : nan;
+    const float tk = __shfl_sync(0xffffffffu, gid >= 0 ? m1 : inf, nprobe <= G ? nprobe - 1 : 0);
+    const float tl = __shfl_sync(0xffffffffu, m1, G - 1);
+    float thr = 0.f;
+    if (lane == 0) thr = screen_threshold(nprobe <= G ? tk : inf, G < ng ? tl : nan, row, tol, ovf);
+    thr = __shfl_sync(0xffffffffu, thr, 0);
+    bool expand = false;
+    const bool live = gid >= 0 && group_live(m1, m2, thr, expand);
+    const int cnt = decide_add_candidates(gid, live, expand, argc, nlist, s_cand, 0, lane);
+    decide_exact_keys(s_q, d, cent, cnorm, metric, s_cand, cnt, nprobe, keys + row * nprobe, lane);
+}
 // assign fast path: one thread per row decides from the screening summary alone when the best
 // group's arg-min column is unambiguous (no other column within tol); other rows are queued
 // for the exact evaluation above.
@@ -949,8 +1024,7 @@ __global__ void assign_resolve_kernel(const int32_t* __restrict__ groups, const 
     const int g0 = groups[row * G + 0], g1 = (G > 1) ? groups[row * G + 1] : -1;
     const int64_t o0 = row * ng + g0;
     const float thr = gmin[o0] + screen_tol(tol, row, tol.rel);
-    if (tol.rel_fast > 0.f &&
-        screen_overflow(groups, row, G, ng, gmin, gmin[o0] + screen_tol(tol, row, tol.rel_fast)))
+    if (tol.rel_fast > 0.f && screen_last_min(groups, row, G, ng, gmin) <= gmin[o0] + screen_tol(tol, row, tol.rel_fast))
         atomicAdd(&ovf[1], 1);  // AUTO mode statistic: FAST would send this row to the exact fallback
     const bool clear = gmin2[o0] > thr && (g1 < 0 || gmin[row * ng + g1] > thr);
     if (clear) {
@@ -1271,33 +1345,41 @@ static void tc_select_groups(const float* gmin, const float* tmin, int64_t nrows
     }
 }
 
-// what the decide stage reads: the screening summary [rows][ng], the G selected groups per row,
-// and the overflow record [overflow rows, FAST-would-overflow rows, row list ...], zeroed
+// what the decide stage reads: the screening summary [rows][ng] and its tile minima
+// [rows][ng / 4], the G selected groups per row (tc_screen_chunk only), and the overflow record
+// [overflow rows, FAST-would-overflow rows, row list ...], zeroed
 struct Screened {
     const float* gmin;
     const float* gmin2;
     const uint8_t* gargc;
+    const float* tmin;
     const int32_t* groups;
     int32_t* ovf;
 };
-// screen a chunk of `rows` rows against a table (as tc_screen) and select their G groups; the
-// workspace is sized for chunks of up to rmax rows
-static Screened tc_screen_chunk(dfx_index* idx, int d, const float* d_x, int64_t rows, int64_t rmax, int ng, int G,
-                                const dfx_tc_table& tab, int npl, int64_t nlist, int metric, cudaStream_t st) {
+// screen a chunk of `rows` rows against a table (as tc_screen); the workspace is sized for chunks
+// of up to rmax rows
+static Screened tc_screen_summary(dfx_index* idx, int d, const float* d_x, int64_t rows, int64_t rmax, int ng,
+                                  const dfx_tc_table& tab, int npl, int64_t nlist, int metric, cudaStream_t st) {
     idx->tc_gmin.reserve((size_t)rmax * ng * 4);
     idx->tc_gmin2.reserve((size_t)rmax * ng * 4);
     idx->tc_gargc.reserve((size_t)rmax * ng);
-    idx->tc_groups.reserve((size_t)rmax * G * 4);
     idx->tc_tmin.reserve((size_t)rmax * (ng / 4 + 1) * 4);
     float* gmin = idx->tc_gmin.as<float>();
     float* tmin = idx->tc_tmin.as<float>();
     tc_screen(idx, d, d_x, rows, tab, npl, nlist, metric, gmin, idx->tc_gmin2.as<float>(), idx->tc_gargc.as<uint8_t>(),
               tmin, st);
-    tc_select_groups(gmin, tmin, rows, ng, G, idx->tc_groups.as<int32_t>(), st);
     idx->tc_ovf.reserve((size_t)(rows + 2) * 4);
     DFX_CUDA(cudaMemsetAsync(idx->tc_ovf.p, 0, 8, st));
-    return {gmin, idx->tc_gmin2.as<float>(), idx->tc_gargc.as<uint8_t>(), idx->tc_groups.as<int32_t>(),
-            idx->tc_ovf.as<int32_t>()};
+    return {gmin, idx->tc_gmin2.as<float>(), idx->tc_gargc.as<uint8_t>(), tmin, nullptr, idx->tc_ovf.as<int32_t>()};
+}
+// the same, then the G groups of every row selected into tc_groups
+static Screened tc_screen_chunk(dfx_index* idx, int d, const float* d_x, int64_t rows, int64_t rmax, int ng, int G,
+                                const dfx_tc_table& tab, int npl, int64_t nlist, int metric, cudaStream_t st) {
+    Screened s = tc_screen_summary(idx, d, d_x, rows, rmax, ng, tab, npl, nlist, metric, st);
+    idx->tc_groups.reserve((size_t)rmax * G * 4);
+    tc_select_groups(s.gmin, s.tmin, rows, ng, G, idx->tc_groups.as<int32_t>(), st);
+    s.groups = idx->tc_groups.as<int32_t>();
+    return s;
 }
 
 // the screening summary alone (dfx_debug_tc_screen): gmin / gmin2 float [nq][ng] and gargc u8
@@ -1339,10 +1421,21 @@ void dfx_tc_coarse_search(dfx_index* idx, const float* d_x, int64_t nq, int npro
         const int64_t qc = std::min(QC, nq - q0);
         const float* xq = d_x + q0 * d;
         int32_t* kq = keys + q0 * nprobe;
-        const Screened s = tc_screen_chunk(idx, d, xq, qc, qmax, ng, G, idx->tc_tab, fast ? 1 : 2, nlist, metric, st);
+        // G <= 32 groups of ng >= 128 (the two-level selection): the whole decide stage in one kernel
+        const bool fused = G <= 32 && ng >= 128 && d % 4 == 0;
+        const int npl = fast ? 1 : 2;
+        const Screened s = fused ? tc_screen_summary(idx, d, xq, qc, qmax, ng, idx->tc_tab, npl, nlist, metric, st)
+                                 : tc_screen_chunk(idx, d, xq, qc, qmax, ng, G, idx->tc_tab, npl, nlist, metric, st);
         const ScreenTol tol = tc_tol(idx, idx->tc_tab, d, fast);
         const int P_cand = dfx_next_pow2(G * 32 < 32 ? 32 : G * 32);
-        if (nprobe <= 32 && G <= 64 && d % 4 == 0) {  // warp per query
+        if (fused) {
+            const size_t smem = decide_rows_smem(d, G);
+            if (smem > 48 * 1024)
+                DFX_CUDA(cudaFuncSetAttribute(decide_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            DFX_LAUNCH(decide_rows_kernel, (unsigned)dfx_ceil_div(qc, DECIDE_WARPS), DECIDE_WARPS * 32, smem, st, xq,
+                       d, cent, cnorm, nlist, metric, s.tmin, s.gmin, s.gmin2, s.gargc, ng, G, nprobe, tol, qc, kq,
+                       s.ovf);
+        } else if (nprobe <= 32 && G <= 64 && d % 4 == 0) {  // warp per query
             const size_t smem = (size_t)RR2_WARPS * ((d + 3) / 4 * 4) * 4 + (size_t)RR2_WARPS * G * 32 * 4;
             if (smem > 48 * 1024)
                 DFX_CUDA(cudaFuncSetAttribute(rerank2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));

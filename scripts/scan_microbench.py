@@ -26,8 +26,8 @@ class A:
 
 
 # the kernels of one IVF-PQ shard search, in launch order
-BREAKDOWN_KERNELS = ("f16_rows_kernel", "tc_coarse_kernel", "topg_collect_kernel", "rerank2_kernel",
-                     "tc_exact_rows_kernel", "scan_pq_il2_kernel")
+BREAKDOWN_KERNELS = ("f16_rows_kernel", "tc_coarse_kernel", "decide_rows_kernel", "tc_exact_rows_kernel",
+                     "scan_pq_il2_kernel")
 TC_PEAK_TFLOPS = 989.0  # H100 SXM data sheet, dense fp16 with fp32 accumulation
 
 
