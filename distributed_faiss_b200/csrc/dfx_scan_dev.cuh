@@ -1,6 +1,6 @@
-// dfx_scan_dev.cuh -- the skeleton of the IVF list scans scan_rows_kernel (dfx_search.cu),
-// scan_pq4_kernel and scan_pq_fs_kernel, and the queue sizing of every list scan but
-// scan_pq_il2_kernel (included by their files; also compiled by the CPU emulator, tests/emu/).
+// dfx_scan_dev.cuh -- the skeleton of every IVF list scan but scan_pq_il2_kernel: scan_rows_kernel
+// and scan_pq_kernel (dfx_search.cu), scan_pq_wide_kernel, scan_pq4_kernel and scan_pq_fs_kernel, and
+// their queue sizing (included by their files; also compiled by the CPU emulator, tests/emu/).
 //
 // One CTA scans the lists of one query's group of G consecutive probes (blockIdx.x = q * ngroups + g)
 // and leaves the k best of them in the group's row of `part`.  A scan writes its table staging and

@@ -5,7 +5,8 @@
 // (reference index.py:43-48 with code_size > 64, or "IVF{n},PQ{M}" at index.py:385-396):
 //   v = dis0 + (t + S),  S = halving-tree sum over P = 128 of lut[m][code_m] (oracle pq_sum,
 //   positions m >= M hold +0).
-// Reads the row-major codes (M bytes per vector), one lane per vector, like scan_pq_kernel.
+// Reads the row-major codes (M bytes per vector), one lane per vector, like scan_pq_kernel; the probe
+// loop, the walk and the candidate sink are the list-scan skeleton (dfx_scan_dev.cuh).
 //
 //   * The query's table, lut[m][j] = -2 * ip_seq(q_m, P[m][j]), is built in the prologue straight
 //     into dynamic shared memory (M x 256 x 4 B: 96 KB at M = 96, 128 KB at M = 128).  A global
@@ -20,8 +21,7 @@
 //     the row-major table is kept, so the arithmetic order is the oracle's without any remapping.
 //   * THREADS (128 / 256 / 512) is chosen by the driver so that the table and one WarpTopK queue
 //     per warp fit in the device's shared memory.
-//   * MAT (k > 1024): `part` is the candidate buffer; every vector's composite goes to slot
-//     coff[q][p] + (position in list) (dfx_cand_store), and the CTA's shared memory is the table only.
+//   * MAT (k > 1024): the CTA's shared memory is the table only.
 #pragma once
 #include "dfx_common.cuh"
 #include "dfx_scan_dev.cuh"
@@ -45,17 +45,14 @@ scan_pq_wide_kernel(const float* __restrict__ Q, int d, int Mrt, int dsub, const
     DFX_DYN_SMEM(unsigned char, smem_raw, 16);
     const int M = (MT > 0) ? MT : Mrt;
     float* s_lut = reinterpret_cast<float*>(smem_raw);  // [M][256]
-    uint64_t* s_buf = reinterpret_cast<uint64_t*>(smem_raw + (size_t)M * PQW_KSUB * 4);
-    const int64_t q = blockIdx.x / ngroups;
-    const int g = blockIdx.x % ngroups;
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const ScanProbes pr(keys, dis0, list_off, nprobe, G, ngroups);
 
     // K3: entry e = m * 256 + j; a warp covers 32 consecutive j of one m (query loads are broadcasts,
     // codebook loads one contiguous run, table stores conflict-free).  seq-k order, as pq_prep_kernel.
     {
-        const float* qrow = Q + q * d;
+        const float* qrow = Q + pr.q * d;
 #pragma unroll 4
-        for (int e = tid; e < M * PQW_KSUB; e += THREADS) {
+        for (int e = threadIdx.x; e < M * PQW_KSUB; e += THREADS) {
             const float* qm = qrow + (e >> 8) * dsub;
             const float* p = codebooks + (size_t)e * dsub;
             float acc = 0.f;
@@ -63,73 +60,57 @@ scan_pq_wide_kernel(const float* __restrict__ Q, int d, int Mrt, int dsub, const
             s_lut[e] = -2.f * acc;
         }
     }
-    WarpTopK wt;
-    if constexpr (!MAT) wt.init(s_buf + (size_t)warp * cap, cap, k);
+    ScanSink<MAT, THREADS> sink(reinterpret_cast<uint64_t*>(smem_raw + (size_t)M * PQW_KSUB * 4), cap, k, part,
+                                coff);
     __syncthreads();
 
-    const int p_end = min(nprobe, (g + 1) * G);
-    for (int p = g * G; p < p_end; p++) {
-        const int l = keys[q * nprobe + p];
-        if (l < 0) continue;
-        const float d0 = dis0[q * nprobe + p];
-        const int64_t beg = list_off[l], end = list_off[l + 1];
-        int64_t cbase = 0;  // MAT: slot of row i is cbase + i
-        if constexpr (MAT) cbase = coff[q * (nprobe + 1) + p] - beg;
-        for (int64_t base = beg + warp * 32; base < end; base += THREADS) {
-            const int64_t i = base + lane;
-            const bool valid = i < end;
-            float v = 0.f;
-            uint32_t my_id = DFX_SEC_NONE;  // loaded with the code: never a dependent load on admission
-            if (valid) {
-                my_id = (uint32_t)__ldg(ids + i);
-                float s[64];  // s[m] = lut[m][c_m] + lut[m + 64][c_{m+64}]: the tree's first level
-                if (MT > 0) {
-                    static_assert(MT % 16 == 0, "MT must be a multiple of 16");
-                    const uint4* cp = reinterpret_cast<const uint4*>(codes + i * (int64_t)M);
+    dfx_scan_lanes<true>(pr, sink, [&](int64_t i, bool valid, int64_t, float d0) {
+        float v = 0.f;
+        uint32_t my_id = DFX_SEC_NONE;  // loaded with the code: never a dependent load on admission
+        if (valid) {
+            my_id = (uint32_t)__ldg(ids + i);
+            float s[64];  // s[m] = lut[m][c_m] + lut[m + 64][c_{m+64}]: the tree's first level
+            if (MT > 0) {
+                static_assert(MT % 16 == 0, "MT must be a multiple of 16");
+                const uint4* cp = reinterpret_cast<const uint4*>(codes + i * (int64_t)M);
 #pragma unroll
-                    for (int c = 0; c < 4; c++) {  // m = 16 c .. 16 c + 15
-                        constexpr int NH = (MT - 64) / 16;  // 16-code chunks of the upper half
-                        const bool hv = c < NH;
-                        const uint4 lo = __ldg(cp + c);
-                        const uint4 hi = hv ? __ldg(cp + 4 + c) : make_uint4(0u, 0u, 0u, 0u);
-                        const uint32_t wl[4] = {lo.x, lo.y, lo.z, lo.w};
-                        const uint32_t wh[4] = {hi.x, hi.y, hi.z, hi.w};
+                for (int c = 0; c < 4; c++) {  // m = 16 c .. 16 c + 15
+                    constexpr int NH = (MT - 64) / 16;  // 16-code chunks of the upper half
+                    const bool hv = c < NH;
+                    const uint4 lo = __ldg(cp + c);
+                    const uint4 hi = hv ? __ldg(cp + 4 + c) : make_uint4(0u, 0u, 0u, 0u);
+                    const uint32_t wl[4] = {lo.x, lo.y, lo.z, lo.w};
+                    const uint32_t wh[4] = {hi.x, hi.y, hi.z, hi.w};
 #pragma unroll
-                        for (int w = 0; w < 4; w++)
-#pragma unroll
-                            for (int b = 0; b < 4; b++) {
-                                const int m = 16 * c + 4 * w + b;
-                                const float a = s_lut[m * PQW_KSUB + ((wl[w] >> (8 * b)) & 255u)];
-                                s[m] = hv ? a + s_lut[(m + 64) * PQW_KSUB + ((wh[w] >> (8 * b)) & 255u)]
-                                          : a + 0.f;
-                            }
-                    }
-                } else {
-                    const uint32_t* cp = reinterpret_cast<const uint32_t*>(codes + i * (int64_t)M);
-#pragma unroll
-                    for (int w = 0; w < 16; w++) {  // m = 4 w .. 4 w + 3
-                        const bool hv = 4 * w + 64 < M;  // M % 4 == 0: the whole word is in or out
-                        const uint32_t lo = __ldg(cp + w);
-                        const uint32_t hi = hv ? __ldg(cp + 16 + w) : 0u;
+                    for (int w = 0; w < 4; w++)
 #pragma unroll
                         for (int b = 0; b < 4; b++) {
-                            const int m = 4 * w + b;
-                            const float a = s_lut[m * PQW_KSUB + ((lo >> (8 * b)) & 255u)];
-                            s[m] = hv ? a + s_lut[(m + 64) * PQW_KSUB + ((hi >> (8 * b)) & 255u)] : a + 0.f;
+                            const int m = 16 * c + 4 * w + b;
+                            const float a = s_lut[m * PQW_KSUB + ((wl[w] >> (8 * b)) & 255u)];
+                            s[m] = hv ? a + s_lut[(m + 64) * PQW_KSUB + ((wh[w] >> (8 * b)) & 255u)] : a + 0.f;
                         }
+                }
+            } else {
+                const uint32_t* cp = reinterpret_cast<const uint32_t*>(codes + i * (int64_t)M);
+#pragma unroll
+                for (int w = 0; w < 16; w++) {  // m = 4 w .. 4 w + 3
+                    const bool hv = 4 * w + 64 < M;  // M % 4 == 0: the whole word is in or out
+                    const uint32_t lo = __ldg(cp + w);
+                    const uint32_t hi = hv ? __ldg(cp + 16 + w) : 0u;
+#pragma unroll
+                    for (int b = 0; b < 4; b++) {
+                        const int m = 4 * w + b;
+                        const float a = s_lut[m * PQW_KSUB + ((lo >> (8 * b)) & 255u)];
+                        s[m] = hv ? a + s_lut[(m + 64) * PQW_KSUB + ((hi >> (8 * b)) & 255u)] : a + 0.f;
                     }
                 }
-                dfx_halving_tree<32>(s);
-                v = d0 + (__ldg(tvals + i) + s[0]);
             }
-            if constexpr (MAT) {
-                if (valid) dfx_cand_store(part, cbase + i, v, my_id);
-            } else {
-                uint32_t sec = 0;
-                const bool want = valid && wt.admits(v, [&] { return my_id; }, sec);
-                wt.push_lanes(want, v, sec);
-            }
+            dfx_halving_tree<32>(s);
+            v = d0 + (__ldg(tvals + i) + s[0]);
         }
-    }
-    if constexpr (!MAT) cta_merge_and_write<THREADS>(wt, s_buf, cap, k, part + ((int64_t)q * ngroups + g) * k);
+        return ScanCand{v, my_id};
+    });
+    // sink.finish(pr), but into row blockIdx.x (= q * ngroups + g) of `part`: keeping q and g live across
+    // the scan costs 8 to 32 B more stack at 64 registers (DESIGN.md section 4.9)
+    if constexpr (!MAT) cta_merge_and_write<THREADS>(sink.wt, sink.s_buf, cap, k, part + (int64_t)blockIdx.x * k);
 }
