@@ -38,15 +38,6 @@ __device__ __forceinline__ float dfx_ld_stream_f(const float* p) {
     return r;
 #endif
 }
-__device__ __forceinline__ uint32_t dfx_ld_stream_u(const int32_t* p) {
-#ifdef DFX_EMU
-    return (uint32_t)*p;
-#else
-    uint32_t r;
-    asm volatile("ld.global.nc.L1::no_allocate.u32 %0, [%1];" : "=r"(r) : "l"(p));
-    return r;
-#endif
-}
 // read-only global load that may stay in L1 (gathers)
 __device__ __forceinline__ uint32_t dfx_ld_nc_u(const int32_t* p) {
 #ifdef DFX_EMU
@@ -81,85 +72,6 @@ __device__ __forceinline__ float dfx_lds_f32(uint32_t addr) {
 #else
     float r;
     asm volatile("ld.shared.f32 %0, [%1];" : "=f"(r) : "r"(addr));
-    return r;
-#endif
-}
-
-// ---- bulk asynchronous copies global -> shared (TMA engine) with mbarrier completion.
-// One barrier = one phase-tracked byte counter: `expect` announces the bytes of a phase, every
-// `copy` delivers some of them, `wait(parity)` returns once the phase of that parity is complete
-// (parity 0 for the first use of a barrier, then 1, 0, ...).  Emulator: the word holds
-// (pending bytes << 32 | completed phases); copies are synchronous.
-__device__ __forceinline__ void dfx_bulk_init(uint64_t* bar) {
-#ifdef DFX_EMU
-    *bar = 0;
-#else
-    const uint32_t a = (uint32_t)__cvta_generic_to_shared(bar);
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(a) : "memory");
-#endif
-}
-// after the init of all barriers of a CTA, by the initialising thread, before the CTA barrier
-__device__ __forceinline__ void dfx_bulk_init_fence() {
-#ifndef DFX_EMU
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-#endif
-}
-__device__ __forceinline__ void dfx_bulk_expect(uint64_t* bar, uint32_t bytes) {
-#ifdef DFX_EMU
-    *bar += (uint64_t)bytes << 32;
-#else
-    const uint32_t a = (uint32_t)__cvta_generic_to_shared(bar);
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(a), "r"(bytes) : "memory");
-#endif
-}
-__device__ __forceinline__ void dfx_bulk_copy(void* dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
-#ifdef DFX_EMU
-    memcpy(dst_smem, src, bytes);
-    *bar -= (uint64_t)bytes << 32;
-    if ((*bar >> 32) == 0) *bar += 1;  // phase complete
-#else
-    const uint32_t a = (uint32_t)__cvta_generic_to_shared(bar);
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"((uint32_t)__cvta_generic_to_shared(dst_smem)), "l"(src), "r"(bytes), "r"(a)
-                 : "memory");
-#endif
-}
-__device__ __forceinline__ void dfx_bulk_wait_parity(uint64_t* bar, uint32_t parity) {
-#ifdef DFX_EMU
-    while (((uint32_t)*reinterpret_cast<volatile uint64_t*>(bar) & 1u) == parity) simt::yield();
-#else
-    const uint32_t a = (uint32_t)__cvta_generic_to_shared(bar);
-    uint32_t done;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done)
-            : "r"(a), "r"(parity)
-            : "memory");
-    } while (!done);
-#endif
-}
-// single-use form (one barrier, one copy): one thread: init; __syncthreads(); the same thread:
-// issue; every thread: wait.
-__device__ __forceinline__ void dfx_bulk_init_one(uint64_t* bar) {
-    dfx_bulk_init(bar);
-    dfx_bulk_init_fence();
-}
-__device__ __forceinline__ void dfx_bulk_issue(void* dst_smem, const void* src, uint32_t bytes, uint64_t* bar) {
-    dfx_bulk_expect(bar, bytes);
-    dfx_bulk_copy(dst_smem, src, bytes, bar);
-}
-__device__ __forceinline__ void dfx_bulk_wait(uint64_t* bar) { dfx_bulk_wait_parity(bar, 0u); }
-// 16-byte and 4-byte shared-memory loads by address
-__device__ __forceinline__ uint4 dfx_lds_v4(uint32_t addr) {
-#ifdef DFX_EMU
-    return *reinterpret_cast<const uint4*>(simt::smem_ptr(addr));
-#else
-    uint4 r;
-    asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];" : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w) : "r"(addr));
     return r;
 #endif
 }

@@ -646,7 +646,8 @@ __device__ __forceinline__ float screen_last_min(const int32_t* __restrict__ gro
 // there are fewer groups than probes: nothing is pruned).  A row with more near-ties than
 // selected groups is queued for tc_exact_rows_kernel.  ovf = [overflow rows, rows that the FAST
 // tolerance would overflow (counted by PRECISE launches for the AUTO mode), row list ...].
-// t and last as the selection left them (decide_rows_kernel holds both in registers).
+// t and last as the selection left them (decide_rows_kernel holds both in registers when it
+// selects the groups itself).
 __device__ __forceinline__ float screen_threshold(float t, float last, int64_t row, const ScreenTol& tol,
                                                   int32_t* __restrict__ ovf) {
     const float thr = t + screen_tol(tol, row, tol.rel);
@@ -868,7 +869,7 @@ rerank_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent
     }
 }
 
-// ---- the exact re-rank of a row by one warp (rerank2_kernel, decide_rows_kernel): lanes own the
+// ---- the exact re-rank of a row by one warp (decide_rows_kernel): lanes own the
 // selected groups, live candidates are compacted into a per-warp list (arg-min column, or all 32
 // columns of a group whose runner-up is within the tolerance), each lane evaluates one candidate
 // in the canonical seq-k order, and the nprobe smallest come out of a register bitonic network.
@@ -915,72 +916,37 @@ __device__ __forceinline__ void decide_exact_keys(const float* __restrict__ s_q,
     if (lane < nprobe) keys_row[lane] = (kept == DFX_COMP_NONE) ? -1 : (int32_t)(uint32_t)kept;
 }
 
-// Search path, nprobe <= 32 and G <= 64 groups selected by tc_select_groups (the shapes that
-// decide_rows_kernel below does not take): the same decision as rerank_kernel<2>, one WARP per
-// query instead of one 128-thread CTA, which would spend 128 threads on 512 candidate slots of
-// which a handful are live, then a block-wide sort.
-constexpr int RR2_WARPS = 4;
-__global__ void __launch_bounds__(RR2_WARPS * 32)
-rerank2_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent, const float* __restrict__ cnorm,
-               int64_t nlist, int metric, const int32_t* __restrict__ groups, int G, int nprobe,
-               const float* __restrict__ gmin, const float* __restrict__ gmin2, const uint8_t* __restrict__ gargc,
-               int ng, ScreenTol tol, int64_t nrows, int32_t* __restrict__ keys, int32_t* __restrict__ ovf) {
-    DFX_DYN_SMEM(unsigned char, rr2_smem, 16);
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t row = (int64_t)blockIdx.x * RR2_WARPS + warp;
-    if (row >= nrows) return;  // whole warps leave; no block-wide barrier below
-    const int dq = (d + 3) / 4 * 4;
-    float* s_q = reinterpret_cast<float*>(rr2_smem) + (size_t)warp * dq;
-    int32_t* s_cand = reinterpret_cast<int32_t*>(rr2_smem + (size_t)RR2_WARPS * dq * 4) + (size_t)warp * G * 32;
-#pragma unroll 4
-    for (int i = lane; i < d; i += 32) s_q[i] = Q[row * d + i];
-    __syncwarp();
-    float thr = 0.f;
-    if (lane == 0) thr = screen_threshold(groups, row, G, nprobe, ng, gmin, tol, ovf);
-    thr = __shfl_sync(0xffffffffu, thr, 0);
-    int cnt = 0;
-    for (int g0 = 0; g0 < G; g0 += 32) {
-        const int gi = g0 + lane;
-        int gid = -1;
-        bool live = false, expand = false;
-        int argc = 0;
-        if (gi < G) {
-            gid = groups[row * G + gi];
-            if (gid >= 0) {
-                const int64_t o = row * ng + gid;
-                live = group_live(gmin[o], gmin2[o], thr, expand);
-                argc = (int)gargc[o];
-            }
-        }
-        cnt = decide_add_candidates(gid, live, expand, argc, nlist, s_cand, cnt, lane);
-    }
-    decide_exact_keys(s_q, d, cent, cnorm, metric, s_cand, cnt, nprobe, keys + row * nprobe, lane);
-}
-
-// Search path, G <= 32 groups of ng >= 128 (the two-level selection; the bench shape): the whole
-// decide stage of a row by one warp, from the screening summary to the keys.  topg_select_row
-// leaves lane r with the r-th smallest selected group; the group's minimum is the value of its
-// composite, so the threshold, the overflow test and the liveness of a group need no load; only
-// the runner-up and the arg-min column of the selected groups are read, together with the query
-// row.  Nothing goes through global memory between the selection and the re-rank.
-// Per warp: the selection buffer (later the candidate list), then the row's query.
-constexpr int DECIDE_WARPS = 8;
+// Search path, nprobe <= 32 and G <= 64: the decide stage of a row by one warp, from the
+// screening summary to the keys.  LEVELS says where the row's groups come from:
+//   2: topg_select_row on the tile minima, then on gmin (G <= 32 of ng >= 128; the bench shape);
+//   1: topg_select_row on gmin alone (G <= 32 of 32 <= ng < 128);
+//   0: given in groups[row][0 .. G), from tc_select_groups (33 <= G <= 64).
+// A selection in the kernel leaves lane r with the r-th smallest selected group; the group's
+// minimum is the value of its composite, so the threshold, the overflow test and the liveness of
+// a group need no load; only the runner-up and the arg-min column of the selected groups are
+// read, together with the query row.  Nothing goes through global memory between the selection
+// and the re-rank.  Given groups are walked in slices of 32, one per lane.
+// Per warp: the selection buffer (later the candidate list), then the row's query.  Warps per
+// CTA: 8, or 4 on given groups, where 8 took 4-9 % longer at 2048 lists (4096 queries, d = 128,
+// H100 80GB HBM3 at 700 W).
 constexpr int DECIDE_CAP = 256;
+__host__ __device__ constexpr int decide_warps(int levels) { return levels > 0 ? 8 : 4; }
 __host__ __device__ __forceinline__ size_t decide_slots(int G) {  // bytes: DECIDE_CAP composites or G x 32 columns
     return (size_t)DECIDE_CAP * 8 > (size_t)G * 32 * 4 ? (size_t)DECIDE_CAP * 8 : (size_t)G * 32 * 4;
 }
-static size_t decide_rows_smem(int d, int G) {
-    return DECIDE_WARPS * (decide_slots(G) + (size_t)(d + 3) / 4 * 4 * 4);
+static size_t decide_rows_smem(int d, int G, int warps) {
+    return warps * (decide_slots(G) + (size_t)(d + 3) / 4 * 4 * 4);
 }
-__global__ void __launch_bounds__(DECIDE_WARPS * 32)
+template <int LEVELS>
+__global__ void __launch_bounds__(decide_warps(LEVELS) * 32)
 decide_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent,
                    const float* __restrict__ cnorm, int64_t nlist, int metric, const float* __restrict__ tmin,
                    const float* __restrict__ gmin, const float* __restrict__ gmin2,
                    const uint8_t* __restrict__ gargc, int ng, int G, int nprobe, ScreenTol tol, int64_t nrows,
-                   int32_t* __restrict__ keys, int32_t* __restrict__ ovf) {
+                   int32_t* __restrict__ keys, int32_t* __restrict__ ovf, const int32_t* __restrict__ groups) {
     DFX_DYN_SMEM(unsigned char, dr_smem, 16);
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int64_t row = (int64_t)blockIdx.x * DECIDE_WARPS + warp;
+    const int64_t row = (int64_t)blockIdx.x * decide_warps(LEVELS) + warp;
     if (row >= nrows) return;  // whole warps leave; no block-wide barrier below
     const size_t slots = decide_slots(G);
     unsigned char* own = dr_smem + (size_t)warp * (slots + (size_t)(d + 3) / 4 * 4 * 4);
@@ -988,7 +954,9 @@ decide_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__
     int32_t* s_cand = reinterpret_cast<int32_t*>(own);  // once the selection is done with buf
     float* s_q = reinterpret_cast<float*>(own + slots);
     const int nt = ng / 4;
-    const uint64_t sel = topg_select_row<DECIDE_CAP>(tmin + row * nt, nt, G, gmin + row * ng, ng, buf, lane);
+    uint64_t sel = DFX_COMP_NONE;
+    if constexpr (LEVELS == 2) sel = topg_select_row<DECIDE_CAP>(tmin + row * nt, nt, G, gmin + row * ng, ng, buf, lane);
+    if constexpr (LEVELS == 1) sel = topg_select_row<DECIDE_CAP>(gmin + row * ng, ng, G, nullptr, 0, buf, lane);
     const int gid = (sel == DFX_COMP_NONE) ? -1 : (int32_t)(uint32_t)sel;
     float m2 = 0.f;
     int argc = 0;
@@ -997,18 +965,35 @@ decide_rows_kernel(const float* __restrict__ Q, int d, const float* __restrict__
         argc = (int)gargc[row * ng + gid];
     }
     for (int i = lane; i < d; i += 32) s_q[i] = Q[row * d + i];
-    // gmin of the lane's group (dfx_key2f gives back gmin + 0: -0 reads as +0, which no
-    // comparison below tells apart); t and last as screen_threshold(groups, ...) defines them
-    const float nan = __int_as_float(0x7fc00000), inf = __int_as_float(0x7f800000);
-    const float m1 = (gid >= 0) ? dfx_key2f((uint32_t)(sel >> 32)) : nan;
-    const float tk = __shfl_sync(0xffffffffu, gid >= 0 ? m1 : inf, nprobe <= G ? nprobe - 1 : 0);
-    const float tl = __shfl_sync(0xffffffffu, m1, G - 1);
     float thr = 0.f;
-    if (lane == 0) thr = screen_threshold(nprobe <= G ? tk : inf, G < ng ? tl : nan, row, tol, ovf);
-    thr = __shfl_sync(0xffffffffu, thr, 0);
-    bool expand = false;
-    const bool live = gid >= 0 && group_live(m1, m2, thr, expand);
-    const int cnt = decide_add_candidates(gid, live, expand, argc, nlist, s_cand, 0, lane);
+    int cnt = 0;
+    if constexpr (LEVELS == 0) {
+        if (lane == 0) thr = screen_threshold(groups, row, G, nprobe, ng, gmin, tol, ovf);
+        thr = __shfl_sync(0xffffffffu, thr, 0);
+        for (int g0 = 0; g0 < G; g0 += 32) {
+            const int gg = g0 + lane < G ? groups[row * G + g0 + lane] : -1;
+            bool live = false, expand = false;
+            int ac = 0;
+            if (gg >= 0) {
+                const int64_t o = row * ng + gg;
+                live = group_live(gmin[o], gmin2[o], thr, expand);
+                ac = (int)gargc[o];
+            }
+            cnt = decide_add_candidates(gg, live, expand, ac, nlist, s_cand, cnt, lane);
+        }
+    } else {
+        // gmin of the lane's group (dfx_key2f gives back gmin + 0: -0 reads as +0, which no
+        // comparison below tells apart); t and last as screen_threshold(groups, ...) defines them
+        const float nan = __int_as_float(0x7fc00000), inf = __int_as_float(0x7f800000);
+        const float m1 = (gid >= 0) ? dfx_key2f((uint32_t)(sel >> 32)) : nan;
+        const float tk = __shfl_sync(0xffffffffu, gid >= 0 ? m1 : inf, nprobe <= G ? nprobe - 1 : 0);
+        const float tl = __shfl_sync(0xffffffffu, m1, G - 1);
+        if (lane == 0) thr = screen_threshold(nprobe <= G ? tk : inf, G < ng ? tl : nan, row, tol, ovf);
+        thr = __shfl_sync(0xffffffffu, thr, 0);
+        bool expand = false;
+        const bool live = gid >= 0 && group_live(m1, m2, thr, expand);
+        cnt = decide_add_candidates(gid, live, expand, argc, nlist, s_cand, 0, lane);
+    }
     decide_exact_keys(s_q, d, cent, cnorm, metric, s_cand, cnt, nprobe, keys + row * nprobe, lane);
 }
 // assign fast path: one thread per row decides from the screening summary alone when the best
@@ -1346,7 +1331,7 @@ static void tc_select_groups(const float* gmin, const float* tmin, int64_t nrows
 }
 
 // what the decide stage reads: the screening summary [rows][ng] and its tile minima
-// [rows][ng / 4], the G selected groups per row (tc_screen_chunk only), and the overflow record
+// [rows][ng / 4], the G selected groups per row (when asked for), and the overflow record
 // [overflow rows, FAST-would-overflow rows, row list ...], zeroed
 struct Screened {
     const float* gmin;
@@ -1356,10 +1341,10 @@ struct Screened {
     const int32_t* groups;
     int32_t* ovf;
 };
-// screen a chunk of `rows` rows against a table (as tc_screen); the workspace is sized for chunks
-// of up to rmax rows
-static Screened tc_screen_summary(dfx_index* idx, int d, const float* d_x, int64_t rows, int64_t rmax, int ng,
-                                  const dfx_tc_table& tab, int npl, int64_t nlist, int metric, cudaStream_t st) {
+// screen a chunk of `rows` rows against a table (as tc_screen), then, for G > 0, select the G
+// groups of every row into tc_groups; the workspace is sized for chunks of up to rmax rows
+static Screened tc_screen_chunk(dfx_index* idx, int d, const float* d_x, int64_t rows, int64_t rmax, int ng, int G,
+                                const dfx_tc_table& tab, int npl, int64_t nlist, int metric, cudaStream_t st) {
     idx->tc_gmin.reserve((size_t)rmax * ng * 4);
     idx->tc_gmin2.reserve((size_t)rmax * ng * 4);
     idx->tc_gargc.reserve((size_t)rmax * ng);
@@ -1370,16 +1355,13 @@ static Screened tc_screen_summary(dfx_index* idx, int d, const float* d_x, int64
               tmin, st);
     idx->tc_ovf.reserve((size_t)(rows + 2) * 4);
     DFX_CUDA(cudaMemsetAsync(idx->tc_ovf.p, 0, 8, st));
-    return {gmin, idx->tc_gmin2.as<float>(), idx->tc_gargc.as<uint8_t>(), tmin, nullptr, idx->tc_ovf.as<int32_t>()};
-}
-// the same, then the G groups of every row selected into tc_groups
-static Screened tc_screen_chunk(dfx_index* idx, int d, const float* d_x, int64_t rows, int64_t rmax, int ng, int G,
-                                const dfx_tc_table& tab, int npl, int64_t nlist, int metric, cudaStream_t st) {
-    Screened s = tc_screen_summary(idx, d, d_x, rows, rmax, ng, tab, npl, nlist, metric, st);
-    idx->tc_groups.reserve((size_t)rmax * G * 4);
-    tc_select_groups(s.gmin, s.tmin, rows, ng, G, idx->tc_groups.as<int32_t>(), st);
-    s.groups = idx->tc_groups.as<int32_t>();
-    return s;
+    int32_t* groups = nullptr;
+    if (G > 0) {
+        idx->tc_groups.reserve((size_t)rmax * G * 4);
+        groups = idx->tc_groups.as<int32_t>();
+        tc_select_groups(gmin, tmin, rows, ng, G, groups, st);
+    }
+    return {gmin, idx->tc_gmin2.as<float>(), idx->tc_gargc.as<uint8_t>(), tmin, groups, idx->tc_ovf.as<int32_t>()};
 }
 
 // the screening summary alone (dfx_debug_tc_screen): gmin / gmin2 float [nq][ng] and gargc u8
@@ -1421,26 +1403,23 @@ void dfx_tc_coarse_search(dfx_index* idx, const float* d_x, int64_t nq, int npro
         const int64_t qc = std::min(QC, nq - q0);
         const float* xq = d_x + q0 * d;
         int32_t* kq = keys + q0 * nprobe;
-        // G <= 32 groups of ng >= 128 (the two-level selection): the whole decide stage in one kernel
-        const bool fused = G <= 32 && ng >= 128 && d % 4 == 0;
+        // nprobe <= 32: the decide stage by one warp per row, on groups it selects itself where
+        // topg_select_row takes the shape (G <= 32), else on those tc_select_groups selected
+        const bool warp_rows = nprobe <= 32 && G <= 64 && d % 4 == 0;
+        const int levels = !warp_rows || G > 32 || ng < 32 ? 0 : ng >= 128 ? 2 : 1;
         const int npl = fast ? 1 : 2;
-        const Screened s = fused ? tc_screen_summary(idx, d, xq, qc, qmax, ng, idx->tc_tab, npl, nlist, metric, st)
-                                 : tc_screen_chunk(idx, d, xq, qc, qmax, ng, G, idx->tc_tab, npl, nlist, metric, st);
+        const Screened s = tc_screen_chunk(idx, d, xq, qc, qmax, ng, levels > 0 ? 0 : G, idx->tc_tab, npl, nlist,
+                                           metric, st);
         const ScreenTol tol = tc_tol(idx, idx->tc_tab, d, fast);
         const int P_cand = dfx_next_pow2(G * 32 < 32 ? 32 : G * 32);
-        if (fused) {
-            const size_t smem = decide_rows_smem(d, G);
+        if (warp_rows) {
+            auto kern = levels == 2 ? decide_rows_kernel<2> : levels == 1 ? decide_rows_kernel<1> : decide_rows_kernel<0>;
+            const int warps = decide_warps(levels);
+            const size_t smem = decide_rows_smem(d, G, warps);
             if (smem > 48 * 1024)
-                DFX_CUDA(cudaFuncSetAttribute(decide_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            DFX_LAUNCH(decide_rows_kernel, (unsigned)dfx_ceil_div(qc, DECIDE_WARPS), DECIDE_WARPS * 32, smem, st, xq,
-                       d, cent, cnorm, nlist, metric, s.tmin, s.gmin, s.gmin2, s.gargc, ng, G, nprobe, tol, qc, kq,
-                       s.ovf);
-        } else if (nprobe <= 32 && G <= 64 && d % 4 == 0) {  // warp per query
-            const size_t smem = (size_t)RR2_WARPS * ((d + 3) / 4 * 4) * 4 + (size_t)RR2_WARPS * G * 32 * 4;
-            if (smem > 48 * 1024)
-                DFX_CUDA(cudaFuncSetAttribute(rerank2_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-            DFX_LAUNCH(rerank2_kernel, (unsigned)dfx_ceil_div(qc, RR2_WARPS), RR2_WARPS * 32, smem, st, xq, d, cent,
-                       cnorm, nlist, metric, s.groups, G, nprobe, s.gmin, s.gmin2, s.gargc, ng, tol, qc, kq, s.ovf);
+                DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            DFX_LAUNCH(kern, (unsigned)dfx_ceil_div(qc, warps), warps * 32, smem, st, xq, d, cent, cnorm, nlist, metric,
+                       s.tmin, s.gmin, s.gmin2, s.gargc, ng, G, nprobe, tol, qc, kq, s.ovf, s.groups);
         } else if (P_cand <= 4096) {  // fused: candidates never leave the SM
             auto kern = rerank_kernel<2>;
             const size_t smem = ((size_t)d * 4 + 15) / 16 * 16 + (size_t)P_cand * 8;

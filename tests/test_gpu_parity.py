@@ -446,7 +446,7 @@ def test_tensor_core_near_tie_overflow_is_redone_exactly():
     st = g.get_state()
     assert np.array_equal(st["list_off"], o.list_off) and np.array_equal(st["ids"], o.ids)
     xq = np.concatenate([cent[cols[0]][None] + 0.01 * rs.randn(40, d), xb[300:340]]).astype(np.float32)
-    for nprobe in (1, 4, 20, 40):                      # 40 > 32: the rerank_kernel<2> branch
+    for nprobe in (1, 4, 20, 40):                      # decide_rows_kernel<0> (all 64 groups kept); 40 > 32: rerank_kernel<2>
         g.nprobe = nprobe; o.nprobe = nprobe
         Do, Io = o.search(xq, 10)
         for mode in (2, 1, 0):
@@ -471,7 +471,7 @@ def test_tensor_core_many_groups_select_from_all_candidates():
     """nlist 8192 = 256 groups of 32 lists: nprobe 128 keeps G = 136 groups, more candidate slots
     (G x 32 > 4096) than the fused decide kernel sorts in shared memory, so every candidate's exact
     composite is written out (rerank_kernel<0>) and the top-nprobe selected from them; nprobe 1 / 7
-    take the warp-per-query kernel and 40 the fused one.  Centroids come from set_state (no
+    take decide_rows_kernel and 40 rerank_kernel<2>.  Centroids come from set_state (no
     training), rows are assigned by the tensor-core screening (dfx_tc_assign)."""
     from oracle import oracle as O
 
