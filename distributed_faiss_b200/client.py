@@ -286,6 +286,37 @@ class IndexClient:
             out_scores.append(np.array([s for s, _ in kept], dtype=np.float32).reshape(-1, 1))
         return out_scores, out_meta
 
+    def range_search(self, query: np.ndarray, radius: float, index_id: str) -> Tuple[np.ndarray, np.ndarray, List]:
+        """Every indexed vector within `radius` of each query, faiss's `range_search` over all shards:
+        `(lims int64[nq + 1], scores float32[lims[-1]], meta)`, query i's results at lims[i]:lims[i + 1]
+        and `meta` a flat list of their metadata.  A shard keeps what its `search` would score with a
+        distance strictly inside the radius: L2 distance < radius, or inner product > radius, by the
+        shard's search metric (a `flat` index is always inner product; the codecs search in L2 whatever
+        `metric` says).  Each query's results are merged best first; among equal scores the earlier
+        shard, then the shard's own order, comes first.  The scores are faiss's values: unlike
+        `search`, which negates them for metric "dot" as the reference does, they are never negated.
+        Always over the sockets, also when a search plane is attached."""
+        results = self._all(lambda s: s.range_search(index_id, query, radius))
+        metrics = {int(r[3]) for r in results}
+        if len(metrics) > 1:
+            raise RuntimeError(f"range_search: the shards of index {index_id!r} report different search metrics "
+                               f"{sorted(metrics)}; their distances cannot be merged")
+        maximize = metrics == {0}  # faiss METRIC_INNER_PRODUCT
+        nq = int(np.asarray(query).shape[0])
+        qs, scores, meta = [], [], []
+        for lims, D, m, _ in results:
+            qs.append(np.repeat(np.arange(nq, dtype=np.int64), np.diff(lims)))
+            scores.append(np.asarray(D, dtype=np.float32))
+            meta.extend(m)
+        q = np.concatenate(qs)
+        D = np.concatenate(scores)
+        # the concatenation is shard-major and each shard's segment is sorted, so a stable sort by
+        # (query, score) keeps shard order and then the shard's order among equal scores
+        order = np.lexsort((-D if maximize else D, q))
+        lims = np.zeros(nq + 1, dtype=np.int64)
+        np.cumsum(np.bincount(q, minlength=nq), out=lims[1:])
+        return lims, D[order], [meta[i] for i in order.tolist()]
+
     # ---- NCCL data plane (spmd.SearchPlane): same contracts, one collective instead of S RPCs
     def _get_meta_kind(self, index_id: str) -> str:
         kind = self._meta_kind.get(index_id)

@@ -386,6 +386,62 @@ int dfx_search(dfx_index* idx, int64_t nq, const float* x, int64_t k, float* D, 
     DFX_API_END
 }
 
+int dfx_range_search_dev(dfx_index* idx, int64_t nq, const float* d_x, float radius, int64_t* d_lims, int64_t* total,
+                         void* stream) {
+    DFX_API_BEGIN
+    DFX_REQUIRE(idx && d_lims && total, "null argument");
+    std::lock_guard<std::mutex> lk(idx->mu);
+    DeviceGuard g(idx->cfg.device);
+    idx->join_dev_if_other((cudaStream_t)stream);
+    dfx_range_impl(idx, nq, d_x, radius, d_lims, total, (cudaStream_t)stream);
+    idx->note_dev((cudaStream_t)stream);
+    DFX_API_END
+}
+int dfx_range_fetch_dev(dfx_index* idx, float* d_D, int64_t* d_I, void* stream) {
+    DFX_API_BEGIN
+    DFX_REQUIRE(idx, "null argument");
+    std::lock_guard<std::mutex> lk(idx->mu);
+    DeviceGuard g(idx->cfg.device);
+    idx->join_dev_if_other((cudaStream_t)stream);
+    dfx_range_fetch_impl(idx, d_D, d_I, (cudaStream_t)stream);
+    idx->note_dev((cudaStream_t)stream);
+    DFX_API_END
+}
+int dfx_range_search(dfx_index* idx, int64_t nq, const float* x, float radius, int64_t* lims) {
+    DFX_API_BEGIN
+    DFX_REQUIRE(idx && lims, "null argument");
+    DFX_REQUIRE(nq >= 0, "nq must be >= 0");
+    std::lock_guard<std::mutex> lk(idx->mu);
+    DeviceGuard g(idx->cfg.device);
+    idx->join_dev();
+    const size_t xb = (size_t)nq * idx->cfg.d * 4;
+    idx->w_q.reserve(std::max<size_t>(xb, 4));
+    idx->r_lims.reserve((size_t)(nq + 1) * 8);
+    if (xb) DFX_CUDA(cudaMemcpyAsync(idx->w_q.p, x, xb, cudaMemcpyHostToDevice, idx->stream));
+    int64_t total = 0;
+    dfx_range_impl(idx, nq, idx->w_q.as<float>(), radius, idx->r_lims.as<int64_t>(), &total, idx->stream);
+    DFX_CUDA(cudaMemcpyAsync(lims, idx->r_lims.p, (size_t)(nq + 1) * 8, cudaMemcpyDeviceToHost, idx->stream));
+    DFX_CUDA(cudaStreamSynchronize(idx->stream));
+    DFX_API_END
+}
+int dfx_range_fetch(dfx_index* idx, float* D, int64_t* I) {
+    DFX_API_BEGIN
+    DFX_REQUIRE(idx, "null argument");
+    std::lock_guard<std::mutex> lk(idx->mu);
+    DeviceGuard g(idx->cfg.device);
+    idx->join_dev();
+    const int64_t n = std::max<int64_t>(idx->r_total, 0);
+    idx->w_D.reserve((size_t)std::max<int64_t>(n, 1) * 4);
+    idx->w_I.reserve((size_t)std::max<int64_t>(n, 1) * 8);
+    dfx_range_fetch_impl(idx, idx->w_D.as<float>(), idx->w_I.as<int64_t>(), idx->stream);
+    if (n) {
+        DFX_CUDA(cudaMemcpyAsync(D, idx->w_D.p, (size_t)n * 4, cudaMemcpyDeviceToHost, idx->stream));
+        DFX_CUDA(cudaMemcpyAsync(I, idx->w_I.p, (size_t)n * 8, cudaMemcpyDeviceToHost, idx->stream));
+    }
+    DFX_CUDA(cudaStreamSynchronize(idx->stream));
+    DFX_API_END
+}
+
 int dfx_reconstruct(dfx_index* idx, int64_t n, const int64_t* ids, float* out) {
     DFX_API_BEGIN
     std::lock_guard<std::mutex> lk(idx->mu);

@@ -154,6 +154,16 @@ struct dfx_index {
     int64_t last_nq = 0, last_nprobe = 0;
     bool last_keys_valid = false;
 
+    // range search (dfx_search.cu, "Range search"): the results of the last one, r_total composites
+    // (r_comp) with their query (r_qidx), grouped by query and sorted; r_total = -1 when there are none
+    // to fetch.  r_comp2 / r_qidx2 are the sorts' spare buffers, r_cnt / r_off a piece's per-query
+    // counts and offsets, r_tot the per-query totals of the call, r_qn FLAT L2's |q|^2, r_lims the
+    // host entry point's lims.
+    DevBuf r_comp, r_qidx, r_comp2, r_qidx2, r_cnt, r_off, r_tot, r_tmp, r_qn, r_lims;
+    int64_t r_total = -1;
+    int r_metric = 0;
+    bool r_qnorm = false;  // the mapping adds r_qn back (FLAT L2)
+
     // bumped by every call that can change what a search launches (train / add / finalize /
     // import / set_param / set_nprobe): CUDA-graph replays of a search are keyed on it
     std::atomic<long long> generation{0};
@@ -251,6 +261,12 @@ void dfx_filter_compact_impl(int64_t nq, int64_t kin, int64_t kout, const float*
 void dfx_map_ids_impl(int64_t n, const int64_t* d_ids, const int64_t* d_table, int64_t* d_out,
                       cudaStream_t st);
 void dfx_stats_impl(dfx_index* idx, int64_t* ndis, cudaStream_t st);
+// range search of nq device queries: d_lims int64[nq + 1] (device), *total = lims[nq] (host);
+// synchronises once per piece and once at the end.  The results stay in r_comp / r_qidx until
+// dfx_range_fetch_impl maps them to (D, I)
+void dfx_range_impl(dfx_index* idx, int64_t nq, const float* d_x, float radius, int64_t* d_lims, int64_t* total,
+                    cudaStream_t st);
+void dfx_range_fetch_impl(dfx_index* idx, float* d_D, int64_t* d_I, cudaStream_t st);
 
 void dfx_launch_select_comp(const uint64_t* comp, int64_t nrows, int n, int64_t ld, int k, int32_t* keys,
                             cudaStream_t st);

@@ -28,7 +28,10 @@
 #include "dfx_select.cuh"
 #include "dfx_topk.cuh"
 #include "dfx_ptx.cuh"
+#include <cub/cub.cuh>
+#include <cmath>
 #include <utility>
+#include <vector>
 
 // =====================================================================================
 // K1a: values GEMM (fp32 FFMA).  acc = fmaf(q[k], x[k], acc), k ascending.
@@ -168,6 +171,20 @@ struct CompLoader {  // a row of composites
         return comp[row * ld + e];
     }
 };
+// the faiss distance of composite c (not DFX_COMP_NONE) of query row `row`: the inner product back
+// from its negation (IP), or the L2 value, with |q|^2 added back and clamped at 0 when qnorm is given
+// (FLAT L2).  Every result a search or a range search reports goes through here.
+__device__ __forceinline__ float dfx_result_distance(uint64_t c, int metric, const float* qnorm, int64_t row) {
+    float v = dfx_key2f((uint32_t)(c >> 32));
+    if (metric == DFX_METRIC_IP) {
+        v = -v;
+    } else if (qnorm) {
+        v = v + qnorm[row];
+        v = v < 0.f ? 0.f : v;
+    }
+    return v;
+}
+
 struct ResultWriter {  // composites -> faiss-style (D, I)
     float* D;
     int64_t* I;
@@ -179,14 +196,7 @@ struct ResultWriter {  // composites -> faiss-style (D, I)
             D[row * k + j] = (metric == DFX_METRIC_IP) ? -FLT_MAX : FLT_MAX;
             I[row * k + j] = -1;
         } else {
-            float v = dfx_key2f((uint32_t)(c >> 32));
-            if (metric == DFX_METRIC_IP) {
-                v = -v;
-            } else if (qnorm) {
-                v = v + qnorm[row];
-                v = v < 0.f ? 0.f : v;
-            }
-            D[row * k + j] = v;
+            D[row * k + j] = dfx_result_distance(c, metric, qnorm, row);
             I[row * k + j] = (int64_t)(uint32_t)c;
         }
     }
@@ -825,8 +835,9 @@ struct IvfPlan {
 
 // Every refusal of the IVF path is here, in this order, so a refused search launches nothing (the M
 // checks of launch_list_scan only guard shapes dfx_create refuses).  Runs after the pending rows are
-// finalized, which can change the layout (idx->il).
-static IvfPlan plan_ivf(dfx_index* idx, int64_t nq, int64_t k64) {
+// finalized, which can change the layout (idx->il).  A range search (range, k64 = 1) takes the
+// candidate rows whatever its radius.
+static IvfPlan plan_ivf(dfx_index* idx, int64_t nq, int64_t k64, bool range = false) {
     IvfPlan p{};
     // IVF-PQR and the flat refinement: the base kind's search for k' = (int64)(k * k_factor)
     // candidates (faiss's float product) into workspace rows, re-ranked per query chunk down to
@@ -853,13 +864,14 @@ static IvfPlan plan_ivf(dfx_index* idx, int64_t nq, int64_t k64) {
     const int64_t nlist = idx->cfg.nlist;
     const int nprobe = p.nprobe = (int)std::min<int64_t>(std::max<int64_t>(idx->nprobe, 1), nlist);
     DFX_REQUIRE(nprobe <= 4096, "nprobe <= 4096");
-    p.mat = k > 1024;
+    p.mat = range || k > 1024;
     const int64_t part_max = (int64_t)1 << 24;  // composites of a chunk's partial results / candidates (128 MiB)
     if (p.mat) {
         DFX_REQUIRE(idx->h_len_top.size() == (size_t)nlist + 1, "IVF search: list lengths are not known");
         p.ld = std::max<int64_t>(idx->h_len_top[(size_t)nprobe], 1);
         DFX_REQUIRE(p.ld <= part_max,
-                    "IVF search at k=" + std::to_string(k) + " with nprobe=" + std::to_string(nprobe) +
+                    (range ? std::string("IVF range search") : "IVF search at k=" + std::to_string(k)) +
+                        " with nprobe=" + std::to_string(nprobe) +
                         ": one query's candidates can reach " + std::to_string(p.ld) +
                         " vectors (the nprobe longest lists), more than the 16777216 (128 MiB) of a query chunk");
     }
@@ -1027,6 +1039,22 @@ static bool launch_list_scan(dfx_index* idx, const IvfPlan& p, const float* xq, 
     return false;
 }
 
+// K1: the nprobe lists each query of a chunk probes -- tensor cores (screen) + canonical fp32
+// (decide), or plain FFMA
+static void coarse_probes(dfx_index* idx, const IvfPlan& p, const float* xq, int64_t qc, int32_t* keys,
+                          cudaStream_t st) {
+    const int64_t nlist = idx->cfg.nlist;
+    if (p.use_tc) {
+        dfx_tc_coarse_search(idx, xq, qc, p.nprobe, keys, st);
+    } else {
+        idx->w_vals.reserve((size_t)p.QC * nlist * 4);
+        dfx_launch_gemm_values(xq, qc, idx->centroids.as<float>(), idx->cnorm.as<float>(), nlist, idx->cfg.d,
+                               idx->cfg.metric, idx->w_vals.as<float>(), nlist, st);
+        dfx_launch_select_cols(idx->w_vals.as<float>(), qc, (int)nlist, nlist, p.nprobe, 0, keys, nullptr, nullptr,
+                               0, st);
+    }
+}
+
 void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, float* d_D,
                      int64_t* d_I, cudaStream_t st) {
     DFX_REQUIRE(idx->trained || idx->cfg.kind == DFX_FLAT, "index is not trained");
@@ -1034,11 +1062,12 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
     if (nq <= 0) return;
     if (idx->n_pending > 0) dfx_finalize_impl(idx, st);
     idx->last_keys_valid = false;
+    idx->r_total = -1;
     if (idx->cfg.kind == DFX_FLAT) return search_flat(idx, nq, d_x, k64, d_D, d_I, st);
 
     const IvfPlan p = plan_ivf(idx, nq, k64);
     const int d = idx->cfg.d, k = p.k, kout = p.kout, nprobe = p.nprobe;
-    const int64_t nlist = idx->cfg.nlist, QC = p.QC;
+    const int64_t QC = p.QC;
     idx->w_keys.reserve((size_t)nq * nprobe * 4);
     int32_t* keys_all = idx->w_keys.as<int32_t>();
     int64_t* coff = nullptr;  // k > 1024: [qc][nprobe + 1] slot offsets of the candidate rows
@@ -1059,16 +1088,7 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
         // where the scan's selection writes: the result rows, or (refinements) the first-stage rows
         float* outD = p.refine ? idx->w_rD.as<float>() : d_D + q0 * k;
         int64_t* outI = p.refine ? idx->w_rI.as<int64_t>() : d_I + q0 * k;
-        // K1: coarse quantizer -- tensor cores (screen) + canonical fp32 (decide), or plain FFMA
-        if (p.use_tc) {
-            dfx_tc_coarse_search(idx, xq, qc, nprobe, keys, st);
-        } else {
-            idx->w_vals.reserve((size_t)QC * nlist * 4);
-            dfx_launch_gemm_values(xq, qc, idx->centroids.as<float>(), idx->cnorm.as<float>(), nlist, d,
-                                   idx->cfg.metric, idx->w_vals.as<float>(), nlist, st);
-            dfx_launch_select_cols(idx->w_vals.as<float>(), qc, (int)nlist, nlist, nprobe, 0, keys,
-                                   nullptr, nullptr, 0, st);
-        }
+        coarse_probes(idx, p, xq, qc, keys, st);
         const int G = choose_group(qc, nprobe);
         const int ngroups = (nprobe + G - 1) / G;
         // k > 1024: `part` holds the candidate rows
@@ -1100,6 +1120,293 @@ void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, 
     idx->last_nq = nq;
     idx->last_nprobe = nprobe;
     idx->last_keys_valid = true;
+}
+
+// =====================================================================================
+// Range search: every vector a search of the same shard scores whose distance passes the radius
+// (L2: D < radius, IP: D > radius, strict as in faiss; NaN never passes), with the distances the
+// k-NN search reports.  FLAT scores the FFMA values tiles of search_flat, IVF the candidate rows of
+// k > 1024 (plan_ivf in range mode).  Each piece -- FLAT: one column tile of a query chunk, IVF: one
+// query chunk -- is counted per query (K_rc), scanned, read back (8 bytes, so the result buffers
+// grow to fit and the 2^27 limit is enforced before anything is written) and its passing composites
+// appended query by query (K_re).  Then each query's results are made contiguous (FLAT with several
+// tiles: a stable sort by query) and sorted by composite: segments of up to 2048 in shared memory
+// (K_rs), or, when one is longer, two stable device-wide sorts (by composite, then by query).
+// =====================================================================================
+static constexpr int64_t kRangeMaxResults = (int64_t)1 << 27;  // per call and shard (1.5 GiB of results)
+static constexpr int kRangeSortCap = 2048;
+
+__device__ __forceinline__ bool dfx_range_pass(float v, int metric, float radius) {
+    return metric == DFX_METRIC_IP ? v > radius : v < radius;
+}
+
+struct RangeCandRows {  // IVF: query q's candidate row of a chunk
+    const uint64_t* part;
+    const int64_t* coff;
+    int nprobe;
+    __device__ __forceinline__ int64_t start(int64_t q) const { return coff[q * (nprobe + 1)]; }
+    __device__ __forceinline__ int64_t size(int64_t q) const { return coff[q * (nprobe + 1) + nprobe] - start(q); }
+    __device__ __forceinline__ uint64_t comp(int64_t s, int64_t e) const { return part[s + e]; }
+};
+struct RangeTileRows {  // FLAT: query q's row of a values tile of nc columns from column c0
+    const float* vals;
+    int64_t ld, nc;
+    uint32_t c0;
+    __device__ __forceinline__ int64_t start(int64_t q) const { return q * ld; }
+    __device__ __forceinline__ int64_t size(int64_t) const { return nc; }
+    __device__ __forceinline__ uint64_t comp(int64_t s, int64_t e) const {
+        return dfx_comp(vals[s + e], c0 + (uint32_t)e);
+    }
+};
+
+// K_rc: one warp per query, cnt[q] = the entries of its row that pass
+template <class Rows>
+__global__ void __launch_bounds__(128)
+range_count_kernel(Rows rows, int64_t nq, int metric, const float* __restrict__ qnorm, float radius,
+                   int64_t* __restrict__ cnt) {
+    const int64_t q = (int64_t)blockIdx.x * 4 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (q >= nq) return;  // warp-uniform
+    const int64_t s = rows.start(q), n = rows.size(q);
+    long long c = 0;
+    for (int64_t e0 = 0; e0 < n; e0 += 32) {
+        const int64_t e = e0 + lane;
+        const bool pass = e < n && dfx_range_pass(dfx_result_distance(rows.comp(s, e), metric, qnorm, q), metric, radius);
+        c += __popc(__ballot_sync(0xffffffffu, pass));
+    }
+    if (lane == 0) cnt[q] = c;
+}
+
+// K_re: the same walk; the passing composites of query q go to out[off[q] ..] in row order (ballot
+// prefix) with their query q0 + q, and tot[q0 + q] adds them to the query's results of the call
+template <class Rows>
+__global__ void __launch_bounds__(128)
+range_emit_kernel(Rows rows, int64_t nq, int metric, const float* __restrict__ qnorm, float radius,
+                  const int64_t* __restrict__ off, int64_t q0, uint64_t* __restrict__ out, uint32_t* __restrict__ qout,
+                  int64_t* __restrict__ tot) {
+    const int64_t q = (int64_t)blockIdx.x * 4 + (threadIdx.x >> 5);
+    const int lane = threadIdx.x & 31;
+    if (q >= nq) return;  // warp-uniform
+    const int64_t s = rows.start(q), n = rows.size(q);
+    int64_t pos = off[q];
+    for (int64_t e0 = 0; e0 < n; e0 += 32) {
+        const int64_t e = e0 + lane;
+        uint64_t c = DFX_COMP_NONE;
+        bool pass = false;
+        if (e < n) {
+            c = rows.comp(s, e);
+            pass = dfx_range_pass(dfx_result_distance(c, metric, qnorm, q), metric, radius);
+        }
+        const unsigned m = __ballot_sync(0xffffffffu, pass);
+        if (pass) {
+            const int64_t i = pos + __popc(m & ((1u << lane) - 1u));
+            out[i] = c;
+            qout[i] = (uint32_t)(q0 + q);
+        }
+        pos += __popc(m);
+    }
+    if (lane == 0) tot[q0 + q] += off[q + 1] - off[q];
+}
+
+// K_rs: one CTA per query sorts its contiguous segment of at most kRangeSortCap composites
+__global__ void __launch_bounds__(256) range_sort_kernel(const int64_t* __restrict__ lims, uint64_t* __restrict__ comp) {
+    DFX_DYN_SMEM(unsigned char, smem_raw, 16);
+    uint64_t* s = reinterpret_cast<uint64_t*>(smem_raw);
+    const int64_t b = lims[blockIdx.x];
+    const int n = (int)(lims[blockIdx.x + 1] - b);
+    if (n < 2) return;  // CTA-uniform
+    int P = 2;
+    while (P < n) P <<= 1;
+    for (int e = threadIdx.x; e < P; e += 256) s[e] = e < n ? comp[b + e] : DFX_COMP_NONE;
+    dfx_block_bitonic_sort<256>(s, P);
+    for (int e = threadIdx.x; e < n; e += 256) comp[b + e] = s[e];
+}
+
+// K_rm: composites -> (D, I), the mapping of ResultWriter
+__global__ void range_map_kernel(const uint64_t* __restrict__ comp, const uint32_t* __restrict__ qidx, int64_t n,
+                                 int metric, const float* __restrict__ qnorm, float* __restrict__ D,
+                                 int64_t* __restrict__ I) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    const uint64_t c = comp[i];
+    D[i] = dfx_result_distance(c, metric, qnorm, qidx[i]);
+    I[i] = (int64_t)(uint32_t)c;
+}
+
+// grow a result buffer of `elem`-byte entries to hold `need`, keeping its first `keep` entries
+static void range_grow(DevBuf& b, int64_t need, int64_t keep, size_t elem, cudaStream_t st) {
+    if ((size_t)need * elem <= b.cap) return;
+    const int64_t n = std::min(kRangeMaxResults, std::max<int64_t>(need, (int64_t)(b.cap / elem) * 2));
+    b.reserve((size_t)n * elem, (size_t)keep * elem, st);
+}
+
+// one piece of qc queries from query q0: count, scan, read back, check the limit, grow, emit
+template <class Rows>
+static void range_piece(dfx_index* idx, const Rows& rows, int64_t q0, int64_t qc, int metric, const float* qnorm,
+                        float radius, int64_t& total, cudaStream_t st) {
+    int64_t* cnt = idx->r_cnt.as<int64_t>();
+    int64_t* off = idx->r_off.as<int64_t>();
+    const unsigned grid = (unsigned)dfx_ceil_div(qc, 4);
+    DFX_CUDA(cudaMemsetAsync(cnt + qc, 0, 8, st));
+    DFX_LAUNCH(range_count_kernel<Rows>, grid, 128, 0, st, rows, qc, metric, qnorm, radius, cnt);
+    size_t tb = 0;
+    DFX_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, cnt, off, (int)(qc + 1), st));
+    idx->r_tmp.reserve(std::max<size_t>(tb, 16));
+    DFX_CUDA(cub::DeviceScan::ExclusiveSum(idx->r_tmp.p, tb, cnt, off, (int)(qc + 1), st));
+    int64_t n = 0;
+    DFX_CUDA(cudaMemcpyAsync(&n, off + qc, 8, cudaMemcpyDeviceToHost, st));
+    DFX_CUDA(cudaStreamSynchronize(st));
+    DFX_REQUIRE(total + n <= kRangeMaxResults,
+                "range search: the results of this call exceed 134217728 (2^27) on one shard; split the query batch");
+    range_grow(idx->r_comp, total + n, total, 8, st);
+    range_grow(idx->r_qidx, total + n, total, 4, st);
+    DFX_LAUNCH(range_emit_kernel<Rows>, grid, 128, 0, st, rows, qc, metric, qnorm, radius, off, q0,
+               idx->r_comp.as<uint64_t>() + total, idx->r_qidx.as<uint32_t>() + total, idx->r_tot.as<int64_t>());
+    total += n;
+}
+
+// stable sort of n (key, value) pairs of the result buffers by key bits [0, bits), into the spare buffers,
+// which then become the result buffers
+template <class K, class V>
+static void range_sort_pairs(dfx_index* idx, DevBuf& keys, DevBuf& keys2, DevBuf& vals, DevBuf& vals2, int64_t n,
+                             int bits, cudaStream_t st) {
+    keys2.reserve((size_t)n * sizeof(K));
+    vals2.reserve((size_t)n * sizeof(V));
+    size_t tb = 0;
+    DFX_CUDA(cub::DeviceRadixSort::SortPairs(nullptr, tb, keys.as<K>(), keys2.as<K>(), vals.as<V>(), vals2.as<V>(),
+                                             (int)n, 0, bits, st));
+    idx->r_tmp.reserve(std::max<size_t>(tb, 16));
+    DFX_CUDA(cub::DeviceRadixSort::SortPairs(idx->r_tmp.p, tb, keys.as<K>(), keys2.as<K>(), vals.as<V>(),
+                                             vals2.as<V>(), (int)n, 0, bits, st));
+    std::swap(keys, keys2);
+    std::swap(vals, vals2);
+}
+
+void dfx_range_impl(dfx_index* idx, int64_t nq, const float* d_x, float radius, int64_t* d_lims, int64_t* total_out,
+                    cudaStream_t st) {
+    // every refusal before anything is launched
+    const int kind = idx->cfg.kind;
+    DFX_REQUIRE(idx->trained || kind == DFX_FLAT, "index is not trained");
+    DFX_REQUIRE(!std::isnan(radius), "range search: the radius is NaN");
+    DFX_REQUIRE(kind != DFX_IVF_PQ_FS,
+                "range search is not supported for IVF_PQ_FS (IVF-PQ FastScan) shards: their distances are "
+                "dequantized only after the selection");
+    DFX_REQUIRE(kind != DFX_IVF_PQR,
+                "range search is not supported for IVF_PQR (refined IVF-PQ) shards: a radius over two stages of "
+                "distances is not defined");
+    DFX_REQUIRE(!idx->rflat(),
+                "range search is not supported for shards with a flat refinement (refine_flat, \",RFlat\"): a "
+                "radius over two stages of distances is not defined");
+    DFX_REQUIRE(nq >= 0, "nq must be >= 0");
+    idx->r_total = -1;
+    idx->r_tot.reserve((size_t)(nq + 1) * 8);
+    int64_t* tot = idx->r_tot.as<int64_t>();
+    DFX_CUDA(cudaMemsetAsync(tot, 0, (size_t)(nq + 1) * 8, st));
+    if (nq == 0) {
+        DFX_CUDA(cudaMemsetAsync(d_lims, 0, 8, st));
+        idx->r_total = *total_out = 0;
+        return;
+    }
+    if (idx->n_pending > 0) dfx_finalize_impl(idx, st);
+    idx->last_keys_valid = false;
+    const int d = idx->cfg.d;
+    int64_t total = 0;
+    int metric = idx->cfg.metric;
+    const float* qnorm = nullptr;
+    bool grouped = true;  // the pieces left each query's results contiguous
+    if (kind == DFX_FLAT) {
+        // the values tiles of search_flat's FFMA path, query chunk by query chunk
+        const int64_t N = idx->n_sorted, NT = 32768, ntiles = dfx_ceil_div(N, NT);
+        const int64_t QC = std::min<int64_t>(nq, (32ll << 20) / NT);
+        grouped = ntiles <= 1;
+        if (metric == DFX_METRIC_L2) {
+            idx->r_qn.reserve((size_t)nq * 4);
+            qnorm = idx->r_qn.as<float>();
+            dfx_launch_row_norms(d_x, nq, d, idx->r_qn.as<float>(), st);
+        }
+        idx->w_vals.reserve((size_t)QC * NT * 4);
+        idx->r_cnt.reserve((size_t)(QC + 1) * 8);
+        idx->r_off.reserve((size_t)(QC + 1) * 8);
+        for (int64_t q0 = 0; q0 < nq; q0 += QC) {
+            const int64_t qc = std::min(QC, nq - q0);
+            for (int64_t t = 0; t < ntiles; t++) {
+                const int64_t c0 = t * NT, nc = std::min(NT, N - c0);
+                dfx_launch_gemm_values(d_x + q0 * d, qc, idx->payload.as<float>() + c0 * d,
+                                       idx->xnorm.as<float>() ? idx->xnorm.as<float>() + c0 : nullptr, nc, d, metric,
+                                       idx->w_vals.as<float>(), NT, st);
+                range_piece(idx, RangeTileRows{idx->w_vals.as<float>(), NT, nc, (uint32_t)c0}, q0, qc, metric,
+                            qnorm ? qnorm + q0 : nullptr, radius, total, st);
+            }
+        }
+    } else {
+        // the k > 1024 path of dfx_search_impl up to the candidate rows, whatever the radius
+        const IvfPlan p = plan_ivf(idx, nq, 1, true);
+        const int nprobe = p.nprobe;
+        metric = p.smetric;
+        idx->w_keys.reserve((size_t)nq * nprobe * 4);
+        idx->w_coff.reserve((size_t)p.QC * (nprobe + 1) * 8);
+        idx->r_cnt.reserve((size_t)(p.QC + 1) * 8);
+        idx->r_off.reserve((size_t)(p.QC + 1) * 8);
+        int64_t* coff = idx->w_coff.as<int64_t>();
+        for (int64_t q0 = 0; q0 < nq; q0 += p.QC) {
+            const int64_t qc = std::min(p.QC, nq - q0);
+            const float* xq = d_x + q0 * d;
+            int32_t* keys = idx->w_keys.as<int32_t>() + q0 * nprobe;
+            coarse_probes(idx, p, xq, qc, keys, st);
+            const int G = choose_group(qc, nprobe);
+            const int ngroups = (nprobe + G - 1) / G;
+            idx->w_part.reserve((size_t)qc * p.ld * 8);
+            uint64_t* part = idx->w_part.as<uint64_t>();
+            DFX_LAUNCH(cand_offsets_kernel, (unsigned)dfx_ceil_div(qc, 4), 128, 0, st, keys, qc, nprobe,
+                       idx->list_off.as<int64_t>(), p.ld, coff);
+            if (idx->prof_on) idx->prof_scan.begin(st);
+            launch_list_scan(idx, p, xq, qc, keys, G, ngroups, part, coff, nullptr, nullptr, st);
+            if (idx->prof_on) idx->prof_scan.end(st);
+            range_piece(idx, RangeCandRows{part, coff, nprobe}, q0, qc, metric, nullptr, radius, total, st);
+        }
+        idx->last_nq = nq;
+        idx->last_nprobe = nprobe;
+        idx->last_keys_valid = true;
+    }
+
+    // lims = the exclusive scan of the per-query totals (tot[nq] = 0); the longest segment picks the sort
+    size_t tb = 0;
+    DFX_CUDA(cub::DeviceScan::ExclusiveSum(nullptr, tb, tot, d_lims, (int)(nq + 1), st));
+    idx->r_tmp.reserve(std::max<size_t>(tb, 16));
+    DFX_CUDA(cub::DeviceScan::ExclusiveSum(idx->r_tmp.p, tb, tot, d_lims, (int)(nq + 1), st));
+    std::vector<int64_t> lims((size_t)nq + 1);
+    DFX_CUDA(cudaMemcpyAsync(lims.data(), d_lims, (size_t)(nq + 1) * 8, cudaMemcpyDeviceToHost, st));
+    DFX_CUDA(cudaStreamSynchronize(st));
+    int64_t longest = 0;
+    for (int64_t q = 0; q < nq; q++) longest = std::max(longest, lims[(size_t)q + 1] - lims[(size_t)q]);
+    int qbits = 1;  // the query index fits in qbits bits
+    while (qbits < 32 && (1ll << qbits) < nq) qbits++;
+    if (longest > kRangeSortCap) {
+        range_sort_pairs<uint64_t, uint32_t>(idx, idx->r_comp, idx->r_comp2, idx->r_qidx, idx->r_qidx2, total, 64, st);
+        range_sort_pairs<uint32_t, uint64_t>(idx, idx->r_qidx, idx->r_qidx2, idx->r_comp, idx->r_comp2, total, qbits,
+                                             st);
+    } else {
+        // the pieces of several tiles interleave the queries: regroup even when no query holds more than one
+        // result, or lims would hand one query's results to another
+        if (!grouped && total > 1)
+            range_sort_pairs<uint32_t, uint64_t>(idx, idx->r_qidx, idx->r_qidx2, idx->r_comp, idx->r_comp2, total,
+                                                 qbits, st);
+        if (longest > 1) {
+            const int P = dfx_next_pow2((int)longest);
+            DFX_LAUNCH(range_sort_kernel, (unsigned)nq, 256, (size_t)P * 8, st, d_lims, idx->r_comp.as<uint64_t>());
+        }
+    }
+    idx->r_metric = metric;
+    idx->r_qnorm = qnorm != nullptr;
+    idx->r_total = *total_out = total;
+}
+
+void dfx_range_fetch_impl(dfx_index* idx, float* d_D, int64_t* d_I, cudaStream_t st) {
+    DFX_REQUIRE(idx->r_total >= 0, "range fetch: no range search results (none ran, or a search ran since)");
+    if (idx->r_total == 0) return;
+    DFX_LAUNCH(range_map_kernel, (unsigned)dfx_ceil_div(idx->r_total, 256), 256, 0, st, idx->r_comp.as<uint64_t>(),
+               idx->r_qidx.as<uint32_t>(), idx->r_total, idx->r_metric,
+               idx->r_qnorm ? idx->r_qn.as<float>() : nullptr, d_D, d_I);
 }
 
 // =====================================================================================

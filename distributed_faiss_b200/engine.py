@@ -38,6 +38,7 @@ EXPORTED_SYMBOLS = [
     "dfx_reconstruct_dev", "dfx_map_ids_dev", "dfx_get_array", "dfx_set_array", "dfx_import_done",
     "dfx_last_stats", "dfx_profile_enable", "dfx_profile_read", "dfx_launch_count", "dfx_synth_init", "dfx_synth_rows_dev", "dfx_free",
     "dfx_last_error", "dfx_version", "dfx_debug_il_byte", "dfx_debug_tc_screen",
+    "dfx_range_search", "dfx_range_fetch", "dfx_range_search_dev", "dfx_range_fetch_dev",
 ]
 
 
@@ -213,6 +214,12 @@ class GpuIndex:
         _check(lib().dfx_set_nprobe(self._h, C.c_int64(int(v))))
 
     @property
+    def search_metric(self):
+        """The metric of the distances search and range_search report: `metric` for FLAT and IVF_FLAT;
+        L2 for the codecs, whose `metric` is the coarse quantizer's (the reference never forwards it)."""
+        return self.metric if self.kind in (KIND_FLAT, KIND_IVF_FLAT) else METRIC_L2
+
+    @property
     def generation(self):
         return int(lib().dfx_generation(self._h))
 
@@ -285,6 +292,21 @@ class GpuIndex:
         _check(lib().dfx_search_dev(self._h, C.c_int64(nq), C.c_void_p(x_t.data_ptr()), C.c_int64(k),
                                     C.c_void_p(D_t.data_ptr()), C.c_void_p(I_t.data_ptr()), C.c_void_p(st)))
         return D_t, I_t
+
+    def range_search(self, x, radius):
+        """faiss's `range_search(x, radius)`: (lims int64[nq + 1], D float32[lims[nq]], I int64[lims[nq]]);
+        query i's results are D[lims[i]:lims[i + 1]], best first.  L2 keeps D < radius, inner product
+        D > radius (search_metric; include/dfx.h, dfx_range_search)."""
+        x = _as_f32(x)
+        assert x.ndim == 2 and x.shape[1] == self.d, f"query must be [nq, {self.d}] float32"
+        nq = x.shape[0]
+        lims = np.empty((nq + 1,), dtype=np.int64)
+        _check(lib().dfx_range_search(self._h, C.c_int64(nq), _np_ptr(x), C.c_float(float(radius)), _np_ptr(lims)))
+        n = int(lims[nq])
+        D = np.empty((n,), dtype=np.float32)
+        I = np.empty((n,), dtype=np.int64)
+        _check(lib().dfx_range_fetch(self._h, _np_ptr(D), _np_ptr(I)))
+        return lims, D, I
 
     def reconstruct_rows(self, ids):
         ids = np.ascontiguousarray(ids, dtype=np.int64).reshape(-1)

@@ -310,6 +310,23 @@ class Index:
                 embs = None
         return scores, self._ids_to_meta(ids), embs
 
+    def range_search(self, query_batch: np.ndarray, radius: float) -> Tuple[np.ndarray, np.ndarray, List[object]]:
+        """faiss's range search on this shard: `(lims int64[nq + 1], scores float32[lims[-1]], meta)`,
+        query i's results at lims[i]:lims[i + 1], best first; `meta` is a flat list of lims[-1]
+        metadata entries.  L2 keeps scores < radius, inner product scores > radius (search_metric())."""
+        with self.index_lock:
+            if self.state != IndexState.TRAINED:
+                raise RuntimeError(f"Server index is not trained. state: {self.state}")
+            lims, scores, ids = self.faiss_index.range_search(query_batch, radius)
+        return lims, scores, self._ids_to_meta(ids)
+
+    def search_metric(self) -> int:
+        """the faiss metric of the distances the engine reports (not cfg.metric for the codecs)"""
+        with self.index_lock:
+            if self.faiss_index is None:
+                raise RuntimeError(f"Server index is not trained. state: {self.state}")
+            return int(self.faiss_index.search_metric)
+
     # ---- the NCCL data plane (spmd.SearchPlane) drives the engine directly, under the same rules
     def is_searchable(self) -> bool:
         """caller holds index_lock; same condition as search() (reference index.py:247)"""

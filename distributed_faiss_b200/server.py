@@ -158,6 +158,12 @@ class IndexServer:
     def search(self, index_id: str, query_batch: np.ndarray, top_k: int, return_embeddings: bool) -> Tuple:
         return self._get_index(index_id).search(query_batch, top_k=top_k, return_embeddings=return_embeddings)
 
+    def range_search(self, index_id: str, query_batch: np.ndarray, radius: float) -> Tuple:
+        """(lims, scores, meta, search metric) of this shard; IndexClient.range_search merges them"""
+        index = self._get_index(index_id)
+        lims, scores, meta = index.range_search(query_batch, radius)
+        return lims, scores, meta, index.search_metric()
+
     def search_ids(self, index_id: str, query_batch: np.ndarray, top_k: int):
         return self._get_index(index_id).search_ids(query_batch, top_k)
 

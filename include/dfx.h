@@ -143,6 +143,38 @@ int dfx_search(dfx_index *idx, int64_t nq, const float *x, int64_t k, float *D, 
 int dfx_search_dev(dfx_index *idx, int64_t nq, const float *d_x, int64_t k, float *d_D,
                    int64_t *d_I, void *stream);
 
+/* ---- range search: faiss_index.range_search(x, radius) of IndexFlat, IndexIVFFlat, IndexIVFPQ and
+ * IndexIVFScalarQuantizer, made deterministic.
+ * The vectors considered are the ones a dfx_search of the same shard scores: every row of FLAT,
+ * the rows of the nprobe probed lists of IVF (same coarse quantizer, same nprobe clamping).  A
+ * vector is returned when its distance D passes the radius strictly, as in faiss: D < radius for
+ * L2, D > radius for inner product (a distance equal to the radius is excluded; NaN never
+ * passes; +-inf radii are allowed, a NaN radius is refused).  The metric is the shard's SEARCH
+ * metric: cfg.metric for FLAT and IVF_FLAT, L2 for IVF_PQ, IVF_SQ16 and IVF_SQ8 (whose cfg.metric
+ * is the coarse quantizer's).  Every returned (D, I) pair is bit for bit the pair dfx_search at a
+ * large enough k reports for that id, and each query's results are sorted best first in the total
+ * order of the search (ranking value ascending, then id ascending; inner product descending).
+ * Served: FLAT, IVF_FLAT, IVF_PQ (8- and 4-bit codes, every layout), IVF_SQ16, IVF_SQ8.  Refused
+ * before anything is launched: IVF_PQ_FS (its distances are dequantized after the selection),
+ * IVF_PQR and refine_flat (a radius over two stages of distances is not defined), an untrained IVF
+ * index.  Limits: an IVF query chunk's candidates obey the rule of k > 1024 (the nprobe longest
+ * lists together at most 2^24 vectors), and one call returns at most 2^27 results; a call that
+ * would return more raises once its counts are known, returns nothing, and leaves the shard
+ * searchable (split the batch).
+ * dfx_range_search: x host [nq, d], lims host int64[nq + 1]; the results of query i are entries
+ * lims[i] .. lims[i + 1] - 1.  dfx_range_fetch then copies the lims[nq] entries into host D
+ * float32 and I int64.  The results stay in index-owned workspace until the next search or range
+ * search of the index, and can be fetched any number of times until then.
+ * dfx_range_search_dev: device queries and device d_lims, *total = lims[nq] on the host; it reads
+ * counts back, synchronising once per query chunk (FLAT: per chunk and 32768-row tile) and once at
+ * the end, so it cannot be captured in a CUDA graph.  dfx_range_fetch_dev maps the results into
+ * device d_D / d_I on the stream. */
+int dfx_range_search(dfx_index *idx, int64_t nq, const float *x, float radius, int64_t *lims);
+int dfx_range_fetch(dfx_index *idx, float *D, int64_t *I);
+int dfx_range_search_dev(dfx_index *idx, int64_t nq, const float *d_x, float radius, int64_t *d_lims,
+                         int64_t *total, void *stream);
+int dfx_range_fetch_dev(dfx_index *idx, float *d_D, int64_t *d_I, void *stream);
+
 /* faiss_index.search_and_reconstruct: decode rows by id (index.py:255); id -1 -> NaN row
  * (refine_flat: the stored fp32 row, as faiss reconstructs from the refine index) */
 int dfx_reconstruct(dfx_index *idx, int64_t n, const int64_t *ids, float *out);
@@ -231,7 +263,7 @@ int dfx_get_array(dfx_index *idx, const char *name, void *out, int64_t max_bytes
 int dfx_set_array(dfx_index *idx, const char *name, const void *in, int64_t nbytes);
 int dfx_import_done(dfx_index *idx);
 
-/* statistics of the most recent search (device work, synchronises):
+/* statistics of the most recent search or range search (device work, synchronises):
  * ndis = sum over (query, probed list) of the list length -- faiss's `ndis` (IVF_PQR: of the
  * IVF-PQ stage, refine_flat: of the base kind's stage; the re-ranked candidates are not counted). */
 int dfx_last_stats(dfx_index *idx, int64_t *ndis, int64_t *nq, int64_t *nprobe);
