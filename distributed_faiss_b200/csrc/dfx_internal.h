@@ -304,6 +304,8 @@ void dfx_tc_stats_sync(dfx_index* idx);  // wait for and fold in the statistics 
 void dfx_tc_prepare_centroids(dfx_index* idx, cudaStream_t st);
 void dfx_tc_coarse_search(dfx_index* idx, const float* d_x, int64_t nq, int nprobe, int32_t* keys,
                           cudaStream_t st);
+// the flat searches dfx_tc_flat_candidates serves (d as dfx_tc_supported, N >= 1024, k <= 100)
+bool dfx_tc_flat_covers(const dfx_index* idx, int k);
 int dfx_tc_flat_candidates(dfx_index* idx, const float* d_x, int64_t nq, int k, cudaStream_t st);
 void dfx_tc_debug_screen(dfx_index* idx, int64_t nq, const float* d_x, int npl, float* gmin, float* gmin2,
                          uint8_t* gargc, cudaStream_t st);

@@ -22,7 +22,7 @@
 //                         on the stored fp32 rows (dfx_rflat_dev.cuh), then K_sel picks the k best
 //   K6   merge            cross-shard merge (float_maxheap_array_t semantics)
 // Driver (dfx_search_impl): search_flat, or plan_ivf once per search (every refusal, before any launch)
-// and per query chunk K1 -> launch_list_scan -> K_sel / select_cand -> fs_dequant -> refine_candidates.
+// and per query chunk (ivf_chunks) K1 -> launch_list_scan -> K_sel / select_cand -> fs_dequant -> refine_candidates.
 // Arithmetic orders are the canonical ones of oracle/dfx_oracle.c (bit-exact parity).
 #include "dfx_internal.h"
 #include "dfx_select.cuh"
@@ -741,6 +741,37 @@ static int choose_group(int64_t nq, int nprobe) {
     return (int)G;
 }
 
+// FLAT L2: |q|^2 of every query into buf, added back to the distances the search reports; nullptr for
+// inner product
+static const float* query_norms(dfx_index* idx, int64_t nq, const float* d_x, DevBuf& buf, cudaStream_t st) {
+    if (idx->cfg.metric != DFX_METRIC_L2) return nullptr;
+    buf.reserve((size_t)nq * 4);
+    dfx_launch_row_norms(d_x, nq, idx->cfg.d, buf.as<float>(), st);
+    return buf.as<float>();
+}
+
+// The FFMA values of a flat shard (K1a), shared by search and range search: per chunk of up to 1024
+// queries, each tile of up to kFlatTile columns goes to w_vals (ld kFlatTile, 128 MB at most), and
+// tile(q0, qc, c0, nc) reads it before the next tile overwrites it.
+static constexpr int64_t kFlatTile = 32768;
+template <class Tile>
+static void flat_tiles(dfx_index* idx, int64_t nq, const float* d_x, cudaStream_t st, Tile&& tile) {
+    const int d = idx->cfg.d;
+    const int64_t N = idx->n_sorted;
+    const int64_t QC = std::min<int64_t>(nq, (32ll << 20) / kFlatTile);
+    const float* xnorm = idx->xnorm.as<float>();
+    idx->w_vals.reserve((size_t)QC * kFlatTile * 4);
+    for (int64_t q0 = 0; q0 < nq; q0 += QC) {
+        const int64_t qc = std::min(QC, nq - q0);
+        for (int64_t c0 = 0; c0 < N; c0 += kFlatTile) {
+            const int64_t nc = std::min(kFlatTile, N - c0);
+            dfx_launch_gemm_values(d_x + q0 * d, qc, idx->payload.as<float>() + c0 * d, xnorm ? xnorm + c0 : nullptr,
+                                   nc, d, idx->cfg.metric, idx->w_vals.as<float>(), kFlatTile, st);
+            tile(q0, qc, c0, nc);
+        }
+    }
+}
+
 static void search_flat(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, float* d_D, int64_t* d_I,
                         cudaStream_t st) {
     DFX_REQUIRE(k64 <= 4096, "flat search supports k <= 4096");
@@ -754,57 +785,31 @@ static void search_flat(dfx_index* idx, int64_t nq, const float* d_x, int64_t k6
         dfx_launch_select<128>(ldr, wr, nq, 0, k, st);
         return;
     }
-    float* qnorm_tc = nullptr;
-    if (idx->flat_tc && idx->tc_enabled) {  // screening on tensor cores + exact re-rank
+    const float* qnorm = query_norms(idx, nq, d_x, idx->w_dis0, st);
+    if (idx->flat_tc && idx->tc_enabled && dfx_tc_flat_covers(idx, k)) {  // screening on tensor cores + exact re-rank
         const int64_t ng = dfx_ceil_div(N, 128) * 4;
         const int64_t QT = std::max<int64_t>(128, ((64ll << 20) / (ng * 4)) / 128 * 128);
-        bool handled = true;
-        for (int64_t q0 = 0; q0 < nq && handled; q0 += QT) {
+        for (int64_t q0 = 0; q0 < nq; q0 += QT) {
             const int64_t qc = std::min(QT, nq - q0);
             const int ncand = dfx_tc_flat_candidates(idx, d_x + q0 * d, qc, k, st);
-            if (ncand == 0) {
-                handled = false;  // shape not covered (only possible on the first chunk)
-                break;
-            }
-            if (metric == DFX_METRIC_L2 && !qnorm_tc) {
-                idx->w_dis0.reserve((size_t)nq * 4);
-                qnorm_tc = idx->w_dis0.as<float>();
-                dfx_launch_row_norms(d_x, nq, d, qnorm_tc, st);
-            }
             CompLoader ldr{idx->tc_cand.as<uint64_t>(), ncand};
-            ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, metric, qnorm_tc ? qnorm_tc + q0 : nullptr};
+            ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, metric, qnorm ? qnorm + q0 : nullptr};
             dfx_launch_select<128>(ldr, wr, qc, ncand, k, st);
         }
-        if (handled) return;
+        return;
     }
-    const int64_t NT = 32768;
-    const int64_t ntiles = dfx_ceil_div(N, NT);
-    int64_t QC = (32ll << 20) / NT;  // 1024 queries per chunk (128 MB of values)
-    if (QC > nq) QC = nq;
-    idx->w_vals.reserve((size_t)QC * NT * 4);
-    idx->w_part.reserve((size_t)QC * ntiles * k * 8);
-    float* qnorm = nullptr;
-    if (metric == DFX_METRIC_L2) {
-        idx->w_dis0.reserve((size_t)nq * 4);
-        qnorm = idx->w_dis0.as<float>();
-        dfx_launch_row_norms(d_x, nq, d, qnorm, st);
-    }
-    for (int64_t q0 = 0; q0 < nq; q0 += QC) {
-        const int64_t qc = (nq - q0 < QC) ? (nq - q0) : QC;
-        for (int64_t t = 0; t < ntiles; t++) {
-            const int64_t c0 = t * NT;
-            const int64_t nc = (N - c0 < NT) ? (N - c0) : NT;
-            dfx_launch_gemm_values(d_x + q0 * d, qc, idx->payload.as<float>() + c0 * d,
-                                   idx->xnorm.as<float>() ? idx->xnorm.as<float>() + c0 : nullptr,
-                                   nc, d, metric, idx->w_vals.as<float>(), NT, st);
-            dfx_launch_select_cols(idx->w_vals.as<float>(), qc, (int)nc, NT, k, (uint32_t)c0,
-                                   nullptr, nullptr, idx->w_part.as<uint64_t>() + t * k,
-                                   ntiles * k, st);
-        }
-        CompLoader ldr{idx->w_part.as<uint64_t>(), ntiles * k};
+    // each tile's k best into the chunk's partial rows (slot t * k), then after a chunk's last tile the k
+    // best of all its tiles
+    const int64_t ntiles = dfx_ceil_div(N, kFlatTile);
+    flat_tiles(idx, nq, d_x, st, [&](int64_t q0, int64_t qc, int64_t c0, int64_t nc) {
+        idx->w_part.reserve((size_t)qc * ntiles * k * 8);
+        uint64_t* part = idx->w_part.as<uint64_t>();
+        dfx_launch_select_cols(idx->w_vals.as<float>(), qc, (int)nc, kFlatTile, k, (uint32_t)c0, nullptr, nullptr,
+                               part + c0 / kFlatTile * k, ntiles * k, st);
+        if (c0 + nc < N) return;
         ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, metric, qnorm ? qnorm + q0 : nullptr};
-        dfx_launch_select<128>(ldr, wr, qc, (int)(ntiles * k), k, st);
-    }
+        dfx_launch_select<128>(CompLoader{part, ntiles * k}, wr, qc, (int)(ntiles * k), k, st);
+    });
 }
 
 // the IVF list scans; plan_ivf picks one per search
@@ -1055,78 +1060,103 @@ static void coarse_probes(dfx_index* idx, const IvfPlan& p, const float* xq, int
     }
 }
 
-void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, float* d_D,
-                     int64_t* d_I, cudaStream_t st) {
-    DFX_REQUIRE(idx->trained || idx->cfg.kind == DFX_FLAT, "index is not trained");
-    DFX_REQUIRE(k64 >= 1, "k must be >= 1");
-    if (nq <= 0) return;
-    if (idx->n_pending > 0) dfx_finalize_impl(idx, st);
-    idx->last_keys_valid = false;
-    idx->r_total = -1;
-    if (idx->cfg.kind == DFX_FLAT) return search_flat(idx, nq, d_x, k64, d_D, d_I, st);
+// what the list scan of one query chunk leaves for the caller
+struct IvfChunk {
+    int64_t q0, qc;
+    const float* xq;       // the chunk's queries
+    uint64_t* part;        // the per-group partial results or, p.mat, the candidate rows
+    int64_t* coff;         // p.mat: [qc][nprobe + 1] slot offsets of the candidate rows
+    int ngroups;
+    float* outD;           // where the selection writes: the result rows, or (refinements) the first-stage rows
+    int64_t* outI;
+    bool final_written;    // the scan wrote outD, outI itself
+};
 
-    const IvfPlan p = plan_ivf(idx, nq, k64);
-    const int d = idx->cfg.d, k = p.k, kout = p.kout, nprobe = p.nprobe;
-    const int64_t QC = p.QC;
+// The query chunks of an IVF search or range search: per chunk of p.QC queries, its probes (K1), with
+// p.mat the slot offsets of its candidate rows (K_off), and its list scan (K3 + K4, the profiled scan
+// range); then chunk(c) takes what the scan left.  The probes of every query stay in w_keys for
+// dfx_last_stats.  A range search passes no result rows (d_D, d_I null).
+template <class Chunk>
+static void ivf_chunks(dfx_index* idx, const IvfPlan& p, int64_t nq, const float* d_x, float* d_D, int64_t* d_I,
+                       cudaStream_t st, Chunk&& chunk) {
+    const int d = idx->cfg.d, k = p.k, nprobe = p.nprobe;
     idx->w_keys.reserve((size_t)nq * nprobe * 4);
-    int32_t* keys_all = idx->w_keys.as<int32_t>();
-    int64_t* coff = nullptr;  // k > 1024: [qc][nprobe + 1] slot offsets of the candidate rows
-    if (p.mat) {
-        idx->w_coff.reserve((size_t)QC * (nprobe + 1) * 8);
-        coff = idx->w_coff.as<int64_t>();
-    }
+    if (p.mat) idx->w_coff.reserve((size_t)p.QC * (nprobe + 1) * 8);
     if (p.refine) {
-        idx->w_rD.reserve((size_t)QC * k * 4);
-        idx->w_rI.reserve((size_t)QC * k * 8);
-        idx->w_rcomp.reserve((size_t)QC * k * 8);
+        idx->w_rD.reserve((size_t)p.QC * k * 4);
+        idx->w_rI.reserve((size_t)p.QC * k * 8);
+        idx->w_rcomp.reserve((size_t)p.QC * k * 8);
     }
-
-    for (int64_t q0 = 0; q0 < nq; q0 += QC) {
-        const int64_t qc = (nq - q0 < QC) ? (nq - q0) : QC;
-        const float* xq = d_x + q0 * d;
-        int32_t* keys = keys_all + q0 * nprobe;
-        // where the scan's selection writes: the result rows, or (refinements) the first-stage rows
-        float* outD = p.refine ? idx->w_rD.as<float>() : d_D + q0 * k;
-        int64_t* outI = p.refine ? idx->w_rI.as<int64_t>() : d_I + q0 * k;
-        coarse_probes(idx, p, xq, qc, keys, st);
-        const int G = choose_group(qc, nprobe);
-        const int ngroups = (nprobe + G - 1) / G;
-        // k > 1024: `part` holds the candidate rows
-        idx->w_part.reserve(p.mat ? (size_t)qc * p.ld * 8 : (size_t)qc * ngroups * k * 8);
-        uint64_t* part = idx->w_part.as<uint64_t>();
+    IvfChunk c{};
+    c.coff = p.mat ? idx->w_coff.as<int64_t>() : nullptr;
+    for (c.q0 = 0; c.q0 < nq; c.q0 += p.QC) {
+        c.qc = std::min(p.QC, nq - c.q0);
+        c.xq = d_x + c.q0 * d;
+        c.outD = p.refine ? idx->w_rD.as<float>() : d_D ? d_D + c.q0 * k : nullptr;
+        c.outI = p.refine ? idx->w_rI.as<int64_t>() : d_I ? d_I + c.q0 * k : nullptr;
+        int32_t* keys = idx->w_keys.as<int32_t>() + c.q0 * nprobe;
+        coarse_probes(idx, p, c.xq, c.qc, keys, st);
+        const int G = choose_group(c.qc, nprobe);
+        c.ngroups = (nprobe + G - 1) / G;
+        idx->w_part.reserve(p.mat ? (size_t)c.qc * p.ld * 8 : (size_t)c.qc * c.ngroups * k * 8);
+        c.part = idx->w_part.as<uint64_t>();
         if (p.mat)
-            DFX_LAUNCH(cand_offsets_kernel, (unsigned)dfx_ceil_div(qc, 4), 128, 0, st, keys, qc, nprobe,
-                       idx->list_off.as<int64_t>(), p.ld, coff);
+            DFX_LAUNCH(cand_offsets_kernel, (unsigned)dfx_ceil_div(c.qc, 4), 128, 0, st, keys, c.qc, nprobe,
+                       idx->list_off.as<int64_t>(), p.ld, c.coff);
         if (idx->prof_on) idx->prof_scan.begin(st);
-        const bool final_written = launch_list_scan(idx, p, xq, qc, keys, G, ngroups, part, coff, outD, outI, st);
+        c.final_written = launch_list_scan(idx, p, c.xq, c.qc, keys, G, c.ngroups, c.part, c.coff, c.outD, c.outI, st);
         if (idx->prof_on) idx->prof_scan.end(st);
-        ResultWriter wr{outD, outI, k, p.smetric, nullptr};
-        if (p.mat) {
-            // P >= 2048 = sort_cap: a row of up to sort_cap candidates is sorted whole
-            const int P = dfx_next_pow2(k);
-            if ((size_t)P * 8 > 48 * 1024)  // a refinement's k' > 4096: opt in to more shared memory
-                DFX_CUDA(cudaFuncSetAttribute(select_cand_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                              P * 8));
-            DFX_LAUNCH(select_cand_kernel<256>, (unsigned)qc, 256, (size_t)P * 8, st, part, coff, nprobe, wr, k, P,
-                       2048);
-        } else if (!final_written) {
-            dfx_launch_select<128>(CompLoader{part, (int64_t)ngroups * k}, wr, qc, ngroups * k, k, st);
-        }
-        if (p.family == ScanFamily::Fs && !p.rflat)  // the flat refinement reads the first stage's ids only
-            DFX_LAUNCH(fs_dequant_kernel, (unsigned)dfx_ceil_div(qc * k, 256), 256, 0, st, outD, outI,
-                       qc * k, k, idx->w_dis0.as<float2>());
-        if (p.refine) refine_candidates(idx, xq, qc, k, kout, outI, d_D + q0 * kout, d_I + q0 * kout, st);
+        chunk(c);
     }
     idx->last_nq = nq;
     idx->last_nprobe = nprobe;
     idx->last_keys_valid = true;
 }
 
+// What every search and range search does first: the statistics of the last search and the results of
+// the last range search stop being valid, and rows added since the last call join the lists.
+static void begin_query(dfx_index* idx, cudaStream_t st) {
+    idx->last_keys_valid = false;
+    idx->r_total = -1;
+    if (idx->n_pending > 0) dfx_finalize_impl(idx, st);
+}
+
+void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, float* d_D,
+                     int64_t* d_I, cudaStream_t st) {
+    DFX_REQUIRE(idx->trained || idx->cfg.kind == DFX_FLAT, "index is not trained");
+    DFX_REQUIRE(k64 >= 1, "k must be >= 1");
+    if (nq <= 0) return;
+    begin_query(idx, st);
+    if (idx->cfg.kind == DFX_FLAT) return search_flat(idx, nq, d_x, k64, d_D, d_I, st);
+
+    const IvfPlan p = plan_ivf(idx, nq, k64);
+    const int k = p.k, kout = p.kout;
+    ivf_chunks(idx, p, nq, d_x, d_D, d_I, st, [&](const IvfChunk& c) {
+        ResultWriter wr{c.outD, c.outI, k, p.smetric, nullptr};
+        if (p.mat) {
+            // P >= 2048 = sort_cap: a row of up to sort_cap candidates is sorted whole
+            const int P = dfx_next_pow2(k);
+            if ((size_t)P * 8 > 48 * 1024)  // a refinement's k' > 4096: opt in to more shared memory
+                DFX_CUDA(cudaFuncSetAttribute(select_cand_kernel<256>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                              P * 8));
+            DFX_LAUNCH(select_cand_kernel<256>, (unsigned)c.qc, 256, (size_t)P * 8, st, c.part, c.coff, p.nprobe, wr,
+                       k, P, 2048);
+        } else if (!c.final_written) {
+            dfx_launch_select<128>(CompLoader{c.part, (int64_t)c.ngroups * k}, wr, c.qc, c.ngroups * k, k, st);
+        }
+        if (p.family == ScanFamily::Fs && !p.rflat)  // the flat refinement reads the first stage's ids only
+            DFX_LAUNCH(fs_dequant_kernel, (unsigned)dfx_ceil_div(c.qc * k, 256), 256, 0, st, c.outD, c.outI,
+                       c.qc * k, k, idx->w_dis0.as<float2>());
+        if (p.refine)
+            refine_candidates(idx, c.xq, c.qc, k, kout, c.outI, d_D + c.q0 * kout, d_I + c.q0 * kout, st);
+    });
+}
+
 // =====================================================================================
 // Range search: every vector a search of the same shard scores whose distance passes the radius
 // (L2: D < radius, IP: D > radius, strict as in faiss; NaN never passes), with the distances the
-// k-NN search reports.  FLAT scores the FFMA values tiles of search_flat, IVF the candidate rows of
-// k > 1024 (plan_ivf in range mode).  Each piece -- FLAT: one column tile of a query chunk, IVF: one
+// k-NN search reports.  FLAT calls flat_tiles, IVF calls ivf_chunks with the candidate rows of k > 1024
+// (plan_ivf in range mode).  Each piece -- FLAT: one column tile of a query chunk, IVF: one
 // query chunk -- is counted per query (K_rc), scanned, read back (8 bytes, so the result buffers
 // grow to fit and the 2^27 limit is enforced before anything is written) and its passing composites
 // appended query by query (K_re).  Then each query's results are made contiguous (FLAT with several
@@ -1244,6 +1274,8 @@ static void range_grow(DevBuf& b, int64_t need, int64_t keep, size_t elem, cudaS
 template <class Rows>
 static void range_piece(dfx_index* idx, const Rows& rows, int64_t q0, int64_t qc, int metric, const float* qnorm,
                         float radius, int64_t& total, cudaStream_t st) {
+    idx->r_cnt.reserve((size_t)(qc + 1) * 8);
+    idx->r_off.reserve((size_t)(qc + 1) * 8);
     int64_t* cnt = idx->r_cnt.as<int64_t>();
     int64_t* off = idx->r_off.as<int64_t>();
     const unsigned grid = (unsigned)dfx_ceil_div(qc, 4);
@@ -1298,75 +1330,32 @@ void dfx_range_impl(dfx_index* idx, int64_t nq, const float* d_x, float radius, 
                 "range search is not supported for shards with a flat refinement (refine_flat, \",RFlat\"): a "
                 "radius over two stages of distances is not defined");
     DFX_REQUIRE(nq >= 0, "nq must be >= 0");
-    idx->r_total = -1;
+    if (nq == 0) {  // no results, and nothing to finalize
+        idx->r_total = *total_out = 0;
+        DFX_CUDA(cudaMemsetAsync(d_lims, 0, 8, st));
+        return;
+    }
+    begin_query(idx, st);
     idx->r_tot.reserve((size_t)(nq + 1) * 8);
     int64_t* tot = idx->r_tot.as<int64_t>();
     DFX_CUDA(cudaMemsetAsync(tot, 0, (size_t)(nq + 1) * 8, st));
-    if (nq == 0) {
-        DFX_CUDA(cudaMemsetAsync(d_lims, 0, 8, st));
-        idx->r_total = *total_out = 0;
-        return;
-    }
-    if (idx->n_pending > 0) dfx_finalize_impl(idx, st);
-    idx->last_keys_valid = false;
-    const int d = idx->cfg.d;
     int64_t total = 0;
     int metric = idx->cfg.metric;
     const float* qnorm = nullptr;
     bool grouped = true;  // the pieces left each query's results contiguous
     if (kind == DFX_FLAT) {
-        // the values tiles of search_flat's FFMA path, query chunk by query chunk
-        const int64_t N = idx->n_sorted, NT = 32768, ntiles = dfx_ceil_div(N, NT);
-        const int64_t QC = std::min<int64_t>(nq, (32ll << 20) / NT);
-        grouped = ntiles <= 1;
-        if (metric == DFX_METRIC_L2) {
-            idx->r_qn.reserve((size_t)nq * 4);
-            qnorm = idx->r_qn.as<float>();
-            dfx_launch_row_norms(d_x, nq, d, idx->r_qn.as<float>(), st);
-        }
-        idx->w_vals.reserve((size_t)QC * NT * 4);
-        idx->r_cnt.reserve((size_t)(QC + 1) * 8);
-        idx->r_off.reserve((size_t)(QC + 1) * 8);
-        for (int64_t q0 = 0; q0 < nq; q0 += QC) {
-            const int64_t qc = std::min(QC, nq - q0);
-            for (int64_t t = 0; t < ntiles; t++) {
-                const int64_t c0 = t * NT, nc = std::min(NT, N - c0);
-                dfx_launch_gemm_values(d_x + q0 * d, qc, idx->payload.as<float>() + c0 * d,
-                                       idx->xnorm.as<float>() ? idx->xnorm.as<float>() + c0 : nullptr, nc, d, metric,
-                                       idx->w_vals.as<float>(), NT, st);
-                range_piece(idx, RangeTileRows{idx->w_vals.as<float>(), NT, nc, (uint32_t)c0}, q0, qc, metric,
-                            qnorm ? qnorm + q0 : nullptr, radius, total, st);
-            }
-        }
+        qnorm = query_norms(idx, nq, d_x, idx->r_qn, st);  // dfx_range_fetch_impl reads r_qn
+        grouped = idx->n_sorted <= kFlatTile;
+        flat_tiles(idx, nq, d_x, st, [&](int64_t q0, int64_t qc, int64_t c0, int64_t nc) {
+            range_piece(idx, RangeTileRows{idx->w_vals.as<float>(), kFlatTile, nc, (uint32_t)c0}, q0, qc, metric,
+                        qnorm ? qnorm + q0 : nullptr, radius, total, st);
+        });
     } else {
-        // the k > 1024 path of dfx_search_impl up to the candidate rows, whatever the radius
         const IvfPlan p = plan_ivf(idx, nq, 1, true);
-        const int nprobe = p.nprobe;
         metric = p.smetric;
-        idx->w_keys.reserve((size_t)nq * nprobe * 4);
-        idx->w_coff.reserve((size_t)p.QC * (nprobe + 1) * 8);
-        idx->r_cnt.reserve((size_t)(p.QC + 1) * 8);
-        idx->r_off.reserve((size_t)(p.QC + 1) * 8);
-        int64_t* coff = idx->w_coff.as<int64_t>();
-        for (int64_t q0 = 0; q0 < nq; q0 += p.QC) {
-            const int64_t qc = std::min(p.QC, nq - q0);
-            const float* xq = d_x + q0 * d;
-            int32_t* keys = idx->w_keys.as<int32_t>() + q0 * nprobe;
-            coarse_probes(idx, p, xq, qc, keys, st);
-            const int G = choose_group(qc, nprobe);
-            const int ngroups = (nprobe + G - 1) / G;
-            idx->w_part.reserve((size_t)qc * p.ld * 8);
-            uint64_t* part = idx->w_part.as<uint64_t>();
-            DFX_LAUNCH(cand_offsets_kernel, (unsigned)dfx_ceil_div(qc, 4), 128, 0, st, keys, qc, nprobe,
-                       idx->list_off.as<int64_t>(), p.ld, coff);
-            if (idx->prof_on) idx->prof_scan.begin(st);
-            launch_list_scan(idx, p, xq, qc, keys, G, ngroups, part, coff, nullptr, nullptr, st);
-            if (idx->prof_on) idx->prof_scan.end(st);
-            range_piece(idx, RangeCandRows{part, coff, nprobe}, q0, qc, metric, nullptr, radius, total, st);
-        }
-        idx->last_nq = nq;
-        idx->last_nprobe = nprobe;
-        idx->last_keys_valid = true;
+        ivf_chunks(idx, p, nq, d_x, nullptr, nullptr, st, [&](const IvfChunk& c) {
+            range_piece(idx, RangeCandRows{c.part, c.coff, p.nprobe}, c.q0, c.qc, metric, nullptr, radius, total, st);
+        });
     }
 
     // lims = the exclusive scan of the per-query totals (tot[nq] = 0); the longest segment picks the sort

@@ -1448,12 +1448,14 @@ void dfx_tc_coarse_search(dfx_index* idx, const float* d_x, int64_t nq, int npro
 // over fp16 planes of the rows (built lazily, rebuilt after an add), the k + 8 groups with the
 // smallest minima, exact canonical values of the columns the screening cannot rule out
 // (rerank_kernel<0>) -- the values gemm_values_kernel would have produced for them, bit for bit.
-// Leaves nq x ncand composites in idx->tc_cand; the caller selects and writes (D, I).
-// Returns ncand, or 0 when this shape is not handled (caller falls back to the FFMA GEMM).
+// Leaves nq x ncand composites in idx->tc_cand and returns ncand; the caller selects and writes (D, I).
+bool dfx_tc_flat_covers(const dfx_index* idx, int k) {
+    return dfx_tc_supported(idx->cfg.d) && idx->n_sorted >= 1024 && k <= 100;
+}
 int dfx_tc_flat_candidates(dfx_index* idx, const float* d_x, int64_t nq, int k, cudaStream_t st) {
+    DFX_REQUIRE(dfx_tc_flat_covers(idx, k), "flat search on tensor cores: the shape is not covered");
     const int d = idx->cfg.d;
     const int64_t N = idx->n_sorted;
-    if (!dfx_tc_supported(d) || N < 1024 || k > 100) return 0;
     const int metric = idx->cfg.metric;
     const int64_t nl_pad = dfx_ceil_div(N, tc::TILE) * tc::TILE;
     const int ng = (int)(nl_pad / 32);
