@@ -90,7 +90,7 @@ int dfx_debug_tc_screen(dfx_index* idx, int64_t nq, const float* d_x, int npl, f
     DFX_REQUIRE(idx && d_x && d_gmin && d_gmin2 && d_gargc, "null argument");
     DFX_REQUIRE(nq >= 1, "nq must be >= 1");
     DFX_REQUIRE(npl == 1 || npl == 2, "npl must be 1 (FAST) or 2 (PRECISE)");
-    DFX_REQUIRE(idx->cfg.kind != DFX_FLAT, "the screening table of an IVF index is its centroids");
+    DFX_REQUIRE(idx->is_ivf(), "the screening table of an IVF index is its centroids");
     std::lock_guard<std::mutex> lk(idx->mu);
     DeviceGuard g(idx->cfg.device);
     idx->join_dev();
@@ -102,7 +102,7 @@ int dfx_debug_tc_screen(dfx_index* idx, int64_t nq, const float* d_x, int npl, f
 int dfx_create(const dfx_cfg* cfg, dfx_index** out) {
     DFX_API_BEGIN
     DFX_REQUIRE(cfg && out, "null argument");
-    DFX_REQUIRE(cfg->kind >= DFX_FLAT && cfg->kind <= DFX_IVF_PQR, "unknown index kind");
+    DFX_REQUIRE(cfg->kind >= DFX_FLAT && cfg->kind <= DFX_FLAT_SQ16, "unknown index kind");
     DFX_REQUIRE(cfg->kind == DFX_IVF_PQR || cfg->refine_m == 0, "refine_m must be 0 for every kind but IVF_PQR");
     DFX_REQUIRE(cfg->metric == DFX_METRIC_IP || cfg->metric == DFX_METRIC_L2,
                 "Only dot and l2 metrics are supported.");
@@ -110,7 +110,16 @@ int dfx_create(const dfx_cfg* cfg, dfx_index** out) {
     require_device(cfg->device);
     std::unique_ptr<dfx_index> idx(new dfx_index());
     idx->cfg = *cfg;
-    if (cfg->kind != DFX_FLAT) {
+    if (cfg->kind == DFX_FLAT_SQ16) {
+        // faiss's IndexScalarQuantizer(QT_fp16): no lists, no codebooks, no refinement
+        DFX_REQUIRE(cfg->nlist == 0 && cfg->pq_m == 0 && cfg->pq_nbits == 0 && cfg->refine_m == 0 &&
+                        cfg->refine_flat == 0,
+                    "FLAT_SQ16: nlist, pq_m, pq_nbits, refine_m and refine_flat must be 0 (an fp16 scalar quantizer "
+                    "without inverted lists), got nlist=" + std::to_string(cfg->nlist) + ", pq_m=" +
+                        std::to_string(cfg->pq_m) + ", pq_nbits=" + std::to_string(cfg->pq_nbits) + ", refine_m=" +
+                        std::to_string(cfg->refine_m) + ", refine_flat=" + std::to_string(cfg->refine_flat));
+    }
+    if (cfg->kind != DFX_FLAT && cfg->kind != DFX_FLAT_SQ16) {
         DFX_REQUIRE(cfg->nlist >= 1 && cfg->nlist < (1ll << 24), "nlist must be in [1, 2^24)");
         DFX_REQUIRE(cfg->d % 4 == 0, "IVF indexes need a dimension that is a multiple of 4");
     }
@@ -251,6 +260,19 @@ int dfx_set_param(dfx_index* idx, const char* name, double value) {
     DFX_API_END
 }
 
+// the device memory of an index's persistent arrays (dfx_get_param "index_bytes"): everything but the
+// search and range-search workspace and the scratch of the screening
+static size_t index_bytes(const dfx_index* idx) {
+    const DevBuf* held[] = {&idx->centroids, &idx->cnorm, &idx->codebooks, &idx->sq_trained, &idx->list_off,
+                            &idx->ids, &idx->payload, &idx->tvals, &idx->xnorm, &idx->p_list, &idx->p_payload,
+                            &idx->p_tvals, &idx->inv, &idx->il_codes, &idx->il_tvals, &idx->il_ids, &idx->blk_off,
+                            &idx->codebooksT, &idx->tc_tab.planes, &idx->tc_tab.cterm, &idx->tc_tab.mean,
+                            &idx->refine_cb, &idx->refine_codes, &idx->refine_vecs};
+    size_t b = 0;
+    for (const DevBuf* h : held) b += h->cap;
+    return b;
+}
+
 int dfx_get_param(dfx_index* idx, const char* name, double* value) {
     DFX_API_BEGIN
     DFX_REQUIRE(idx && name && value, "null argument");
@@ -277,6 +299,7 @@ int dfx_get_param(dfx_index* idx, const char* name, double* value) {
     else if (n == "il2_prefetch") *value = idx->il2_prefetch;
     else if (n == "rows_inflight") *value = idx->rows_inflight;
     else if (n == "workspace_bytes") *value = (double)idx->w_part.cap;  // read-only
+    else if (n == "index_bytes") *value = (double)index_bytes(idx);     // read-only
     else if (n == "k_factor" && (idx->cfg.kind == DFX_IVF_PQR || idx->rflat())) *value = idx->k_factor;
     else if (n == "refine_ms" || n == "refine_launches") {  // read-only
         std::lock_guard<std::mutex> lk(idx->mu);
@@ -479,8 +502,8 @@ int dfx_set_nprobe(dfx_index* idx, int64_t nprobe) {
 int64_t dfx_get_nprobe(const dfx_index* idx) { return idx->nprobe; }
 int64_t dfx_generation(const dfx_index* idx) { return (int64_t)idx->generation.load(); }
 int64_t dfx_ntotal(const dfx_index* idx) { return idx->ntotal(); }
-int64_t dfx_nlist(const dfx_index* idx) { return idx->cfg.kind == DFX_FLAT ? 0 : idx->cfg.nlist; }
-int dfx_is_trained(const dfx_index* idx) { return (idx->trained || idx->cfg.kind == DFX_FLAT) ? 1 : 0; }
+int64_t dfx_nlist(const dfx_index* idx) { return idx->is_flat() ? 0 : idx->cfg.nlist; }
+int dfx_is_trained(const dfx_index* idx) { return (idx->trained || idx->is_flat()) ? 1 : 0; }
 
 int dfx_get_centroids(dfx_index* idx, float* out) {
     DFX_API_BEGIN
@@ -600,6 +623,8 @@ static std::vector<ExchangeArray> exchange_arrays(dfx_index* idx) {
     const int kind = idx->cfg.kind;
     const int64_t n = idx->n_sorted, nlist = idx->cfg.nlist, d = idx->cfg.d, M = idx->M, M2 = idx->M2;
     if (kind == DFX_FLAT) return {{"xb", &idx->payload, C::none, n * d * 4, false, true, "xb: wrong size"}};
+    if (kind == DFX_FLAT_SQ16)
+        return {{"codes16", &idx->payload, C::none, n * d * 2, false, true, "codes16: wrong size (u16[ntotal, d])"}};
     std::vector<ExchangeArray> a{{"centroids", &idx->centroids, C::none, nlist * d * 4, true, true, "centroids: wrong size"}};
     if (idx->has_pq())
         a.push_back({"codebooks", &idx->codebooks, C::none, M * idx->ksub * idx->dsub * 4, true, true, "codebooks: wrong size"});
@@ -695,10 +720,11 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
     const std::vector<ExchangeArray> arrays = exchange_arrays(idx);
     const ExchangeArray* a = find_exchange_array(arrays, n);
     if (!a || !a->importable) throw DfxError{"cannot import array '" + n + "'"};
-    if (idx->cfg.kind == DFX_FLAT) {  // the import sets the number of rows
-        DFX_REQUIRE(nbytes % (d * 4) == 0, a->size_error);
-        idx->n_sorted = nbytes / (d * 4);
-        idx->tc_flat_rows = -1;  // imported rows: any fp16 planes are stale
+    if (idx->is_flat()) {  // the import sets the number of rows
+        const int64_t rb = (int64_t)idx->row_bytes();
+        DFX_REQUIRE(nbytes % rb == 0, a->size_error);
+        idx->n_sorted = nbytes / rb;
+        idx->tc_flat_rows = -1;  // imported rows: any screening table is stale
     } else {
         DFX_REQUIRE(nbytes == a->bytes, a->size_error);
     }
@@ -751,9 +777,11 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
         idx->update_list_lengths();
         idx->n_sorted = idx->h_list_off[(size_t)nlist];
         idx->n_pending = 0;
-    } else if (n == "xb" && idx->cfg.metric == DFX_METRIC_L2) {
+    } else if (idx->is_flat() && idx->cfg.metric == DFX_METRIC_L2) {  // "xb" / "codes16": the rows' norms
         idx->xnorm.reserve((size_t)std::max<int64_t>(idx->n_sorted, 1) * 4);
-        dfx_launch_row_norms(idx->payload.as<float>(), idx->n_sorted, (int)d, idx->xnorm.as<float>(), idx->stream);
+        dfx_with_flat_rows(idx, [&](auto rows) {
+            dfx_launch_row_norms(rows, idx->n_sorted, (int)d, idx->xnorm.as<float>(), idx->stream);
+        });
         DFX_CUDA(cudaStreamSynchronize(idx->stream));
     } else if (n == "refine_codes" || n == "refine_vecs") {
         idx->refine_cap = idx->refine_rows = idx->n_sorted;

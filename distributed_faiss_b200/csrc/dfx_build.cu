@@ -502,7 +502,7 @@ static void start_empty_lists(dfx_index* idx, cudaStream_t st) {
 }
 
 void dfx_train_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) {
-    if (idx->cfg.kind == DFX_FLAT) {
+    if (idx->is_flat()) {  // trained at creation, as faiss's IndexFlat and IndexScalarQuantizer(QT_fp16)
         idx->trained = true;
         return;
     }
@@ -540,19 +540,31 @@ static void ensure_pending(dfx_index* idx, int64_t need, cudaStream_t st) {
     idx->p_cap = cap;
 }
 
-// FLAT: the rows in arrival order, and their norms under L2
+// FLAT_SQ16 encode (faiss QT_fp16 without a residual): code = fp16(x), round to nearest even,
+// overflow to +-inf
+__global__ void f16_encode_kernel(const float* __restrict__ x, int64_t n, __half* __restrict__ codes) {
+    const int64_t t = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (t < n) codes[t] = __float2half_rn(x[t]);
+}
+
+// FLAT / FLAT_SQ16: the rows (fp32, or their fp16 codes) in arrival order, and under L2 the norms of
+// the stored rows
 static void add_flat(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) {
     const int d = idx->cfg.d;
     const int64_t N = idx->n_sorted;
-    if ((size_t)(N + n) * d * 4 > idx->payload.cap) {
+    const size_t rb = idx->row_bytes();
+    if ((size_t)(N + n) * rb > idx->payload.cap) {
         int64_t cap = std::max<int64_t>({N + n, 2 * N, idx->reserve_hint});
-        idx->payload.reserve((size_t)cap * d * 4, (size_t)N * d * 4, st);
+        idx->payload.reserve((size_t)cap * rb, (size_t)N * rb, st);
         if (idx->cfg.metric == DFX_METRIC_L2) idx->xnorm.reserve((size_t)cap * 4, (size_t)N * 4, st);
     }
-    DFX_CUDA(cudaMemcpyAsync(idx->payload.as<float>() + N * d, d_x, (size_t)n * d * 4,
-                             cudaMemcpyDeviceToDevice, st));
+    if (idx->cfg.kind == DFX_FLAT_SQ16)
+        DFX_LAUNCH(f16_encode_kernel, blocks_for(n * d, 256), 256, 0, st, d_x, n * d, idx->payload.as<__half>() + N * d);
+    else
+        DFX_CUDA(cudaMemcpyAsync(idx->payload.as<float>() + N * d, d_x, (size_t)n * d * 4,
+                                 cudaMemcpyDeviceToDevice, st));
     if (idx->cfg.metric == DFX_METRIC_L2)
-        dfx_launch_row_norms(d_x, n, d, idx->xnorm.as<float>() + N, st);
+        dfx_with_flat_rows(idx, [&](auto rows) { dfx_launch_row_norms(rows + N * d, n, d, idx->xnorm.as<float>() + N, st); });
     idx->n_sorted += n;
 }
 
@@ -631,7 +643,7 @@ static void add_by_id(dfx_index* idx, int64_t n, const float* d_x, const int32_t
 void dfx_add_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) {
     if (n <= 0) return;
     DFX_REQUIRE(idx->ntotal() + n < (1ll << 31), "a shard holds at most 2^31-1 vectors");
-    if (idx->cfg.kind == DFX_FLAT) {
+    if (idx->is_flat()) {
         add_flat(idx, n, d_x, st);
         return;
     }
@@ -727,12 +739,12 @@ __global__ void invert_ids_kernel(const int32_t* __restrict__ ids, int64_t n, in
 // holds it (the decoders that add the list's centroid).
 enum class RowFrom { Id, Pos, List };
 
-template <RowFrom FROM>
-struct RowsDec {  // FLAT and the flat refinement (by id), IVF_FLAT (by position): the stored row
-    static constexpr RowFrom kFrom = FROM;
-    const float* rows;
+template <RowFrom FROM, class T = float>
+struct RowsDec {  // FLAT and the flat refinement (by id), IVF_FLAT (by position): the stored row;
+    static constexpr RowFrom kFrom = FROM;  // FLAT_SQ16 (T = __half, by id): the decoded fp16 row
+    const T* rows;
     int d;
-    __device__ float operator()(int k, int64_t, int64_t pos, int64_t) const { return rows[pos * d + k]; }
+    __device__ float operator()(int k, int64_t, int64_t pos, int64_t) const { return dfx_elem_f32(rows[pos * d + k]); }
 };
 
 struct Sq16Dec {  // IVF_SQ16: c + r in fp16
@@ -858,6 +870,7 @@ void dfx_reconstruct_impl(dfx_index* idx, int64_t n, const int64_t* d_ids, float
     dfx_refresh_inv(idx, st);
     switch (idx->cfg.kind) {
         case DFX_FLAT: return run(RowsDec<RowFrom::Id>{idx->payload.as<float>(), d});
+        case DFX_FLAT_SQ16: return run(RowsDec<RowFrom::Id, __half>{idx->payload.as<__half>(), d});
         case DFX_IVF_FLAT: return run(RowsDec<RowFrom::Pos>{idx->payload.as<float>(), d});
         case DFX_IVF_SQ16: return run(Sq16Dec{idx->payload.as<__half>(), cent, d});
         case DFX_IVF_SQ8: return run(Sq8Dec{idx->payload.as<uint8_t>(), cent, idx->sq_trained.as<float>(), d});

@@ -171,6 +171,24 @@ __device__ __forceinline__ float dfx_dot_seqk(const float* q, const float* x, in
     }
     return acc;
 }
+// the same over fp16 rows (FLAT_SQ16): each element widened exactly, the same chain of fmas, so the
+// value equals the one over the fp32 rows they decode to.  d % 4 == 0, x 8-byte aligned.
+__device__ __forceinline__ float dfx_dot_seqk(const float* q, const __half* x, int d) {
+    float acc = 0.f;
+#pragma unroll 8
+    for (int k = 0; k < d; k += 4) {
+        const __half2* xh = reinterpret_cast<const __half2*>(x + k);
+        const float2 a = __half22float2(xh[0]), b = __half22float2(xh[1]);
+        acc = __fmaf_rn(q[k + 0], a.x, acc);
+        acc = __fmaf_rn(q[k + 1], a.y, acc);
+        acc = __fmaf_rn(q[k + 2], b.x, acc);
+        acc = __fmaf_rn(q[k + 3], b.y, acc);
+    }
+    return acc;
+}
+// one stored element as fp32 (exact for both row types)
+__device__ __forceinline__ float dfx_elem_f32(float v) { return v; }
+__device__ __forceinline__ float dfx_elem_f32(__half v) { return __half2float(v); }
 // ranking value of column col from its inner product with the query: -ip (IP), or |x|^2 - 2 ip
 // (L2, |q|^2 left out); xnorm is only read for L2
 __device__ __forceinline__ float dfx_rank_value(float ip, int metric, const float* xnorm, int64_t col) {

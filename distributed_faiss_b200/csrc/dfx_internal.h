@@ -17,6 +17,9 @@ int dfx_smem_optin();
 // A screening table of the tensor-core coarse quantizer (dfx_tc.cu): an index's centroids, the
 // rows of a FLAT index, or the centroids of one k-means step.  Rows are screened centred on
 // their mean m, which leaves the ranking unchanged and shrinks the screening error.
+// The rows of a FLAT_SQ16 index are screened as they are stored: one exact fp16 plane (`rows`, the
+// index's codes), no mean (m = 0, a zero vector in `mean`), scale 1, and the column term read
+// from `rows_cterm` (L2: the stored |x|^2, IP: none) -- nothing per row is copied.
 struct dfx_tc_table {
     DevBuf planes;        // fp16 [2][n_pad][d]: hi and lo planes of (c - m) * scale
     DevBuf cterm;         // f32 [n_pad]: column term, L2 |c - m|^2, IP -m.c; 3e38 for padded rows
@@ -24,6 +27,9 @@ struct dfx_tc_table {
     float scale = 1.f;    // power of two of the planes
     float cmax2 = 0.f;    // max |c|^2
     float cmax2c = 0.f;   // max |c - m|^2
+    const __half* rows = nullptr;        // one exact plane [n][d] (FLAT_SQ16), else nullptr
+    const float* rows_cterm = nullptr;   // its column terms [n] (nullptr: 0), columns >= n never selected
+    bool one_plane() const { return rows != nullptr; }
 };
 
 // Device time of one search stage (dfx_profile_enable): begin / end bracket its launches on a stream,
@@ -83,9 +89,9 @@ struct dfx_index {
     // h_len_top[p]: vectors in the p longest lists together (bounds one query's candidates at k > 1024)
     std::vector<int64_t> h_len_top;
     DevBuf ids;                         // int32[n_sorted] shard-local ids, list-sorted
-    DevBuf payload;                     // kind-specific rows, list-sorted (FLAT: arrival order)
+    DevBuf payload;                     // kind-specific rows, list-sorted (FLAT, FLAT_SQ16: arrival order)
     DevBuf tvals;                       // IVF_PQ: f32[n_sorted] (IVF_PQ_FS has none)
-    DevBuf xnorm;                       // FLAT + L2: f32[n]
+    DevBuf xnorm;                       // FLAT / FLAT_SQ16 + L2: f32[n], |x|^2 of the stored rows
     DevBuf p_list, p_payload, p_tvals;  // pending: int32 list per row, payload rows, tvals
     int64_t p_cap = 0;
     int64_t reserve_hint = 0;
@@ -130,8 +136,9 @@ struct dfx_index {
     int rows_inflight = 0;      // vectors in flight per warp of scan_rows_kernel: 0 = by row size, else 4 / 8
     int il2_threads = 0;        // scan_pq_il2 CTA shape: 0 = default (env DFX_IL2_THREADS or 256), 256, 512
     int il2_prefetch = -1;      // L2 prefetch distance in blocks: -1 = default (env DFX_IL2_PREFETCH or 4)
-    bool flat_tc = true;        // FLAT: search through the tensor-core screening (dfx_tc_flat_candidates)
-    int64_t tc_flat_rows = -1;  // rows covered by the fp16 copy of a FLAT index (-1: none)
+    bool flat_tc = true;        // FLAT / FLAT_SQ16: search through the tensor-core screening (dfx_tc_flat_candidates)
+    int64_t tc_flat_rows = -1;  // rows covered by the screening table of a flat index (-1: none)
+    bool tc_flat_finite = true; // FLAT_SQ16: every code of those rows is finite (else the FFMA GEMM serves)
 
     // IVF_PQR: the refinement PQ (M2 sub-quantizers of 256 centroids, dsub2 = d / M2), its codes by
     // id (u8[ntotal][M2], arrival order; refine_cap rows allocated), k' = k * k_factor, and the
@@ -211,6 +218,7 @@ struct dfx_index {
         switch (cfg.kind) {
             case DFX_FLAT:
             case DFX_IVF_FLAT: return (size_t)cfg.d * 4;
+            case DFX_FLAT_SQ16: return (size_t)cfg.d * 2;
             case DFX_IVF_PQ: return ksub == 16 ? (size_t)M / 2 : (size_t)M;  // 4-bit codes: two per byte
             case DFX_IVF_PQ_FS: return (size_t)M / 2;
             case DFX_IVF_PQR: return (size_t)M;  // the refine codes live outside the lists
@@ -229,7 +237,10 @@ struct dfx_index {
         h_len_top.assign(nl + 1, 0);
         for (size_t l = 0; l < nl; l++) h_len_top[l + 1] = h_len_top[l] + len[l];
     }
-    bool is_ivf() const { return cfg.kind != DFX_FLAT; }
+    // the kinds without lists, training or probes: every stored row is scored by every search, rows are
+    // kept in arrival order, and ids are positions (FLAT: fp32 rows, FLAT_SQ16: fp16 rows)
+    bool is_flat() const { return cfg.kind == DFX_FLAT || cfg.kind == DFX_FLAT_SQ16; }
+    bool is_ivf() const { return !is_flat(); }
     bool rflat() const { return cfg.refine_flat != 0; }
     // the kinds with PQ codebooks (IVF_PQ / IVF_PQR: residual codes, IVF_PQ_FS: codes of the raw vectors)
     bool has_pq() const { return cfg.kind == DFX_IVF_PQ || cfg.kind == DFX_IVF_PQ_FS || cfg.kind == DFX_IVF_PQR; }
@@ -242,7 +253,18 @@ struct dfx_index {
 void dfx_launch_gemm_values(const float* Q, int64_t nq, const float* X, const float* xnorm,
                             int64_t ncols, int d, int metric, float* out, int64_t ld_out,
                             cudaStream_t st);
+void dfx_launch_gemm_values(const float* Q, int64_t nq, const __half* X, const float* xnorm,
+                            int64_t ncols, int d, int metric, float* out, int64_t ld_out,
+                            cudaStream_t st);
 void dfx_launch_row_norms(const float* X, int64_t n, int d, float* out, cudaStream_t st);
+void dfx_launch_row_norms(const __half* X, int64_t n, int d, float* out, cudaStream_t st);
+// the stored rows of a flat index as their element type: f(const float*) for FLAT, f(const __half*)
+// for FLAT_SQ16
+template <class F>
+static auto dfx_with_flat_rows(const dfx_index* idx, F&& f) {
+    if (idx->cfg.kind == DFX_FLAT_SQ16) return f(idx->payload.as<__half>());
+    return f(idx->payload.as<float>());
+}
 // top-k columns per row of a values matrix -> keys int32[nrows,k] (and optional values)
 void dfx_launch_select_cols(const float* vals, int64_t nrows, int n, int64_t ld, int k,
                             uint32_t col_base, int32_t* keys, float* kvals, uint64_t* comp_out,
@@ -306,6 +328,9 @@ void dfx_tc_coarse_search(dfx_index* idx, const float* d_x, int64_t nq, int npro
                           cudaStream_t st);
 // the flat searches dfx_tc_flat_candidates serves (d as dfx_tc_supported, N >= 1024, k <= 100)
 bool dfx_tc_flat_covers(const dfx_index* idx, int k);
+// (re)builds the screening table of a flat index's rows when they changed; false when the rows cannot
+// be screened (a FLAT_SQ16 index holding a non-finite code), which leaves the search to the FFMA GEMM
+bool dfx_tc_flat_table(dfx_index* idx, cudaStream_t st);
 int dfx_tc_flat_candidates(dfx_index* idx, const float* d_x, int64_t nq, int k, cudaStream_t st);
 void dfx_tc_debug_screen(dfx_index* idx, int64_t nq, const float* d_x, int npl, float* gmin, float* gmin2,
                          uint8_t* gargc, cudaStream_t st);

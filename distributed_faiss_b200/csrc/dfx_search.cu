@@ -38,8 +38,9 @@
 // =====================================================================================
 // The FFMA tile shared by K1a and K7a: the CTA computes rows m0 .. m0 + BM of Q against columns
 // n0 .. n0 + BN of X; thread (tx, ty) leaves acc[i][j] = q(m0 + ty TM + i) . x(n0 + tx TN + j).
-template <int BM, int BN, int BK, int TM, int TN>
-__device__ __forceinline__ void gemm_tile_ffma(const float* __restrict__ Q, int64_t nq, const float* __restrict__ X,
+// X holds fp32 rows, or the fp16 rows of FLAT_SQ16, widened exactly as they are staged.
+template <int BM, int BN, int BK, int TM, int TN, class TX>
+__device__ __forceinline__ void gemm_tile_ffma(const float* __restrict__ Q, int64_t nq, const TX* __restrict__ X,
                                                int64_t ncols, int d, int64_t m0, int64_t n0, int tx, int ty,
                                                float (&acc)[TM][TN]) {
     constexpr int THREADS = (BM / TM) * (BN / TN);
@@ -62,7 +63,7 @@ __device__ __forceinline__ void gemm_tile_ffma(const float* __restrict__ Q, int6
             int n = e / BK, kk = e % BK;
             int64_t gn = n0 + n;
             int gk = k0 + kk;
-            sX[kk][n] = (gn < ncols && gk < d) ? X[gn * d + gk] : 0.f;
+            sX[kk][n] = (gn < ncols && gk < d) ? dfx_elem_f32(X[gn * d + gk]) : 0.f;
         }
         __syncthreads();
 #pragma unroll
@@ -83,9 +84,9 @@ __device__ __forceinline__ void gemm_tile_ffma(const float* __restrict__ Q, int6
     // in a way that matters: acc + (+0) keeps acc), so the canonical order is preserved.
 }
 
-template <int BM, int BN, int BK, int TM, int TN>
+template <int BM, int BN, int BK, int TM, int TN, class TX>
 __global__ void __launch_bounds__((BM / TM) * (BN / TN))
-gemm_values_kernel(const float* __restrict__ Q, int64_t nq, const float* __restrict__ X,
+gemm_values_kernel(const float* __restrict__ Q, int64_t nq, const TX* __restrict__ X,
                    const float* __restrict__ xnorm, int64_t ncols, int d, int metric,
                    float* __restrict__ out, int64_t ld_out) {
     const int tid = threadIdx.x;
@@ -107,38 +108,56 @@ gemm_values_kernel(const float* __restrict__ Q, int64_t nq, const float* __restr
     }
 }
 
-void dfx_launch_gemm_values(const float* Q, int64_t nq, const float* X, const float* xnorm,
-                            int64_t ncols, int d, int metric, float* out, int64_t ld_out,
-                            cudaStream_t st) {
+template <class TX>
+static void launch_gemm_values(const float* Q, int64_t nq, const TX* X, const float* xnorm, int64_t ncols, int d,
+                               int metric, float* out, int64_t ld_out, cudaStream_t st) {
     if (nq <= 0 || ncols <= 0) return;
     if (nq <= 16) {
         constexpr int BM = 16, BN = 128, BK = 16, TM = 2, TN = 4;
         dim3 grid((unsigned)dfx_ceil_div(ncols, BN), (unsigned)dfx_ceil_div(nq, BM));
-        auto kern = gemm_values_kernel<BM, BN, BK, TM, TN>;
+        auto kern = gemm_values_kernel<BM, BN, BK, TM, TN, TX>;
         DFX_LAUNCH(kern, grid, (BM / TM) * (BN / TN), 0, st, Q, nq, X, xnorm, ncols, d, metric, out,
                    ld_out);
     } else {
         constexpr int BM = 128, BN = 128, BK = 8, TM = 8, TN = 8;
         dim3 grid((unsigned)dfx_ceil_div(ncols, BN), (unsigned)dfx_ceil_div(nq, BM));
-        auto kern = gemm_values_kernel<BM, BN, BK, TM, TN>;
+        auto kern = gemm_values_kernel<BM, BN, BK, TM, TN, TX>;
         DFX_LAUNCH(kern, grid, (BM / TM) * (BN / TN), 0, st, Q, nq, X, xnorm, ncols, d, metric, out,
                    ld_out);
     }
 }
+void dfx_launch_gemm_values(const float* Q, int64_t nq, const float* X, const float* xnorm,
+                            int64_t ncols, int d, int metric, float* out, int64_t ld_out,
+                            cudaStream_t st) {
+    launch_gemm_values(Q, nq, X, xnorm, ncols, d, metric, out, ld_out, st);
+}
+void dfx_launch_gemm_values(const float* Q, int64_t nq, const __half* X, const float* xnorm,
+                            int64_t ncols, int d, int metric, float* out, int64_t ld_out,
+                            cudaStream_t st) {
+    launch_gemm_values(Q, nq, X, xnorm, ncols, d, metric, out, ld_out, st);
+}
 
-// |x|^2 in seq-k order
-__global__ void row_norms_kernel(const float* __restrict__ X, int64_t n, int d,
+// |x|^2 in seq-k order (fp16 rows: of the rows they decode to)
+template <class TX>
+__global__ void row_norms_kernel(const TX* __restrict__ X, int64_t n, int d,
                                  float* __restrict__ out) {
     int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
-    const float* x = X + i * d;
+    const TX* x = X + i * d;
     float acc = 0.f;
-    for (int k = 0; k < d; k++) acc = __fmaf_rn(x[k], x[k], acc);
+    for (int k = 0; k < d; k++) {
+        const float v = dfx_elem_f32(x[k]);
+        acc = __fmaf_rn(v, v, acc);
+    }
     out[i] = acc;
 }
 void dfx_launch_row_norms(const float* X, int64_t n, int d, float* out, cudaStream_t st) {
     if (n <= 0) return;
-    DFX_LAUNCH(row_norms_kernel, (unsigned)dfx_ceil_div(n, 128), 128, 0, st, X, n, d, out);
+    DFX_LAUNCH(row_norms_kernel<float>, (unsigned)dfx_ceil_div(n, 128), 128, 0, st, X, n, d, out);
+}
+void dfx_launch_row_norms(const __half* X, int64_t n, int d, float* out, cudaStream_t st) {
+    if (n <= 0) return;
+    DFX_LAUNCH(row_norms_kernel<__half>, (unsigned)dfx_ceil_div(n, 128), 128, 0, st, X, n, d, out);
 }
 
 // =====================================================================================
@@ -750,7 +769,7 @@ static const float* query_norms(dfx_index* idx, int64_t nq, const float* d_x, De
     return buf.as<float>();
 }
 
-// The FFMA values of a flat shard (K1a), shared by search and range search: per chunk of up to 1024
+// The FFMA values of a flat shard (K1a, over its fp32 or fp16 rows), shared by search and range search: per chunk of up to 1024
 // queries, each tile of up to kFlatTile columns goes to w_vals (ld kFlatTile, 128 MB at most), and
 // tile(q0, qc, c0, nc) reads it before the next tile overwrites it.
 static constexpr int64_t kFlatTile = 32768;
@@ -765,8 +784,10 @@ static void flat_tiles(dfx_index* idx, int64_t nq, const float* d_x, cudaStream_
         const int64_t qc = std::min(QC, nq - q0);
         for (int64_t c0 = 0; c0 < N; c0 += kFlatTile) {
             const int64_t nc = std::min(kFlatTile, N - c0);
-            dfx_launch_gemm_values(d_x + q0 * d, qc, idx->payload.as<float>() + c0 * d, xnorm ? xnorm + c0 : nullptr,
-                                   nc, d, idx->cfg.metric, idx->w_vals.as<float>(), kFlatTile, st);
+            dfx_with_flat_rows(idx, [&](auto rows) {
+                dfx_launch_gemm_values(d_x + q0 * d, qc, rows + c0 * d, xnorm ? xnorm + c0 : nullptr, nc, d,
+                                       idx->cfg.metric, idx->w_vals.as<float>(), kFlatTile, st);
+            });
             tile(q0, qc, c0, nc);
         }
     }
@@ -786,7 +807,8 @@ static void search_flat(dfx_index* idx, int64_t nq, const float* d_x, int64_t k6
         return;
     }
     const float* qnorm = query_norms(idx, nq, d_x, idx->w_dis0, st);
-    if (idx->flat_tc && idx->tc_enabled && dfx_tc_flat_covers(idx, k)) {  // screening on tensor cores + exact re-rank
+    if (idx->flat_tc && idx->tc_enabled && dfx_tc_flat_covers(idx, k) &&
+        dfx_tc_flat_table(idx, st)) {  // screening on tensor cores + exact re-rank
         const int64_t ng = dfx_ceil_div(N, 128) * 4;
         const int64_t QT = std::max<int64_t>(128, ((64ll << 20) / (ng * 4)) / 128 * 128);
         for (int64_t q0 = 0; q0 < nq; q0 += QT) {
@@ -1123,11 +1145,11 @@ static void begin_query(dfx_index* idx, cudaStream_t st) {
 
 void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, float* d_D,
                      int64_t* d_I, cudaStream_t st) {
-    DFX_REQUIRE(idx->trained || idx->cfg.kind == DFX_FLAT, "index is not trained");
+    DFX_REQUIRE(idx->trained || idx->is_flat(), "index is not trained");
     DFX_REQUIRE(k64 >= 1, "k must be >= 1");
     if (nq <= 0) return;
     begin_query(idx, st);
-    if (idx->cfg.kind == DFX_FLAT) return search_flat(idx, nq, d_x, k64, d_D, d_I, st);
+    if (idx->is_flat()) return search_flat(idx, nq, d_x, k64, d_D, d_I, st);
 
     const IvfPlan p = plan_ivf(idx, nq, k64);
     const int k = p.k, kout = p.kout;
@@ -1318,7 +1340,7 @@ void dfx_range_impl(dfx_index* idx, int64_t nq, const float* d_x, float radius, 
                     cudaStream_t st) {
     // every refusal before anything is launched
     const int kind = idx->cfg.kind;
-    DFX_REQUIRE(idx->trained || kind == DFX_FLAT, "index is not trained");
+    DFX_REQUIRE(idx->trained || idx->is_flat(), "index is not trained");
     DFX_REQUIRE(!std::isnan(radius), "range search: the radius is NaN");
     DFX_REQUIRE(kind != DFX_IVF_PQ_FS,
                 "range search is not supported for IVF_PQ_FS (IVF-PQ FastScan) shards: their distances are "
@@ -1343,7 +1365,7 @@ void dfx_range_impl(dfx_index* idx, int64_t nq, const float* d_x, float radius, 
     int metric = idx->cfg.metric;
     const float* qnorm = nullptr;
     bool grouped = true;  // the pieces left each query's results contiguous
-    if (kind == DFX_FLAT) {
+    if (idx->is_flat()) {
         qnorm = query_norms(idx, nq, d_x, idx->r_qn, st);  // dfx_range_fetch_impl reads r_qn
         grouped = idx->n_sorted <= kFlatTile;
         flat_tiles(idx, nq, d_x, st, [&](int64_t q0, int64_t qc, int64_t c0, int64_t nc) {

@@ -29,6 +29,7 @@
 // resident in shared memory and B (centroids) streams through a ring of 16 KB stages; larger d
 // (config C4, d = 768): A and B k-atoms stream through the ring together.
 #include "dfx_internal.h"
+#include <cmath>
 #include <utility>
 #include "dfx_select.cuh"
 #include "dfx_topk.cuh"
@@ -300,10 +301,11 @@ f16_rows_kernel(const float* __restrict__ x, int64_t n, int64_t n_pad, int d, co
 // epilogue's centred ranking value fma(acc, mult[row], cterm[col]), its packed (min, runner-up,
 // arg-min) per 32 centroids, and the row term added to the minimum and runner-up with their
 // column bits kept.  Everything downstream (group selection, exact canonical re-evaluation, the
-// overflow fallback, the drivers) is the product code.
+// overflow fallback, the drivers) is the product code.  one: the table is one exact plane of ncols rows
+// (the kernel's ONE: PRECISE accumulates qh.c + ql.c); the column term as the kernel reads it.
 static void emu_tc_screen(const __half* qh, const float* qmult, const float* qterm, int64_t nq, int64_t nq_pad,
-                          const __half* ch, int64_t nl_pad, int d, int npl, const float* cterm, float* gmin,
-                          float* gmin2, uint8_t* gargc, float* tmin, int ng) {
+                          const __half* ch, int64_t nl_pad, int64_t ncols, bool one, int d, int npl,
+                          const float* cterm, float* gmin, float* gmin2, uint8_t* gargc, float* tmin, int ng) {
     const float big = 3.0e38f;
     auto repack = [](float v, float col_of) {  // v with the 5 low bits of col_of
         uint32_t u, c;
@@ -313,8 +315,9 @@ static void emu_tc_screen(const __half* qh, const float* qmult, const float* qte
         memcpy(&v, &u, 4);
         return v;
     };
-    std::vector<float> cf((size_t)npl * nl_pad * d), qf((size_t)npl * d);
-    for (size_t i = 0; i < cf.size(); i++) cf[i] = __half2float(ch[i]);
+    std::vector<float> cf((size_t)npl * nl_pad * d, 0.f), qf((size_t)npl * d);
+    const size_t present = one ? (size_t)ncols * d : cf.size();  // one plane: rows >= ncols read as zeros
+    for (size_t i = 0; i < present; i++) cf[i] = __half2float(ch[i]);
     for (int64_t row = 0; row < nq; row++) {
         for (int pl = 0; pl < npl; pl++)
             for (int k = 0; k < d; k++) qf[(size_t)pl * d + k] = __half2float(qh[(size_t)pl * nq_pad * d + row * d + k]);
@@ -327,9 +330,10 @@ static void emu_tc_screen(const __half* qh, const float* qmult, const float* qte
                 for (int k = 0; k < d; k++) acc += qf[k] * h[k];
                 if (npl == 2) {
                     const float* l = &cf[(size_t)nl_pad * d + (size_t)col * d];
-                    for (int k = 0; k < d; k++) acc += qf[d + k] * h[k] + qf[k] * l[k];
+                    for (int k = 0; k < d; k++) acc += qf[d + k] * h[k] + (one ? 0.f : qf[k] * l[k]);
                 }
-                const float v = fmaf(acc, qmult[row], cterm[col]);
+                const float ct = col < ncols ? (cterm ? cterm[col] : 0.f) : big;
+                const float v = fmaf(acc, qmult[row], ct);
                 uint32_t u;
                 memcpy(&u, &v, 4);
                 u = (u & ~31u) | (uint32_t)j;
@@ -359,10 +363,13 @@ static void emu_tc_screen(const __half* qh, const float* qmult, const float* qte
 // (f16_rows_kernel); cterm: float [nl_pad], the column term (padded with 3e38)
 // gmin / gmin2: float [nq][ng], gargc: u8 [nq][ng], ng = nl_pad/32
 // KT: d / 64 at compile time for the resident shapes (1, 2, 4); 0 = streamed, k-atoms at run time
-template <int KT, int NPL>
+// ONE: the table is one exact fp16 plane (FLAT_SQ16 rows, tmC [ncols, d]) -- PRECISE is then (qh, c) and
+// (ql, c), two MMAs per k-step; FAST (NPL 1) is the same kernel for either table
+// cterm: column c < ncols reads cterm[c] (0 when cterm is null), columns >= ncols are never selected
+template <int KT, int NPL, bool ONE = false>
 __global__ void __launch_bounds__(tc::THREADS, KT != 0 ? tc::Smem::ctas_per_sm(true, KT, NPL) : 1)
 tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant__ CUtensorMap tmC, int nq,
-                 int nq_pad, int nl_pad, int katoms_rt, const float* __restrict__ cterm,
+                 int nq_pad, int nl_pad, int ncols, int katoms_rt, const float* __restrict__ cterm,
                  const float* __restrict__ qmult, const float* __restrict__ qterm, int ctiles_per_cta,
                  float* __restrict__ gmin, float* __restrict__ gmin2, uint8_t* __restrict__ gargc,
                  float* __restrict__ tmin, int ng) {
@@ -372,8 +379,10 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
     constexpr int NSTAGE = Smem::nstage(RES, KT, NPL);
     constexpr int STAGE_BYTES = Smem::stage_bytes(RES);
     constexpr int TN = TILE;  // centroids per tile
-    // operand pairs accumulated per k-atom: FAST (qh, ch); PRECISE (qh, ch), (ql, ch), (qh, cl)
-    constexpr int NCOMBO = NPL == 1 ? 1 : 3;
+    // operand pairs accumulated per k-atom: FAST (qh, ch); PRECISE (qh, ch), (ql, ch), (qh, cl) -- or,
+    // with an exact table plane, (qh, c), (ql, c)
+    constexpr int NCOMBO = NPL == 1 ? 1 : ONE ? 2 : 3;
+    constexpr int NBPL = ONE ? 1 : NPL;  // table planes
     extern __shared__ unsigned char smem_raw_tc[];
     unsigned char* smem = reinterpret_cast<unsigned char*>(
         (reinterpret_cast<uintptr_t>(smem_raw_tc) + 1023) & ~(uintptr_t)1023);  // SWIZZLE_128B atoms
@@ -407,7 +416,7 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 
     if (warp == CONSUMERS / 32) {
         // ===================== TMA producer =====================
-        // RES: per tile, the B atoms of the hi plane then (PRECISE) of the lo plane.
+        // RES: per tile, the B atoms of the hi plane then (PRECISE, two table planes) of the lo plane.
         // streamed: per tile and k-atom, the (A atom, B atom) pair of every combo.
         if (lane == 0) {
             if (RES) {
@@ -421,7 +430,7 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
             for (int t = 0; t < ntiles; t++) {
                 const int crow = (ct0 + t) * TN;
                 // RES: c = B plane; streamed: c = combo
-                for (int c = 0; c < (RES ? NPL : NCOMBO); c++)
+                for (int c = 0; c < (RES ? NBPL : NCOMBO); c++)
                 for (int ka = 0; ka < KATOMS; ka++) {
                     mbar_wait(&empty[stage], phase ^ 1);
                     mbar_expect_tx(&full[stage], STAGE_BYTES);
@@ -485,10 +494,11 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
         const int col0 = (ct0 + t) * TN;
         // the column term of column threadIdx.x % 128 of the tile (`big` past nlist); loaded now,
         // shared through this warpgroup's copy once the MMAs are issued
-        const float cn_own = cterm[col0 + (threadIdx.x & (TN - 1))];
+        const int own_col = col0 + (threadIdx.x & (TN - 1));
+        const float cn_own = own_col < ncols ? (cterm ? cterm[own_col] : 0.f) : big;
         if (RES && (wg == 1 || t > 0)) asm volatile("bar.sync %0, %1;" ::"r"(2 + wg), "n"(CONSUMERS) : "memory");
         int prev = -1;  // stage of the group still in flight
-        for (int c = 0; c < (RES ? NPL : NCOMBO); c++)
+        for (int c = 0; c < (RES ? NBPL : NCOMBO); c++)
         for (int ka = 0; ka < KATOMS; ka++) {
             mbar_wait(&full[stage], phase);
             const uint32_t st_addr = r_base + stage * STAGE_BYTES;
@@ -615,7 +625,19 @@ tc_coarse_kernel(const __grid_constant__ CUtensorMap tmQ, const __grid_constant_
 //     and for q.c, 2^-24 for their difference), no longer shared with the screening value; for
 //     inner product, where a centred value is bounded by V + Vc, the centred-frame terms on V.
 // tol = 2 e, +5 % slack.  The row term itself (fp64, rounded once) is a constant per row.
-static float screen_tol_rel(int d, bool fast) {
+//
+// An exact table plane (FLAT_SQ16: the stored fp16 rows, m = 0, scale 1) drops the table's rounding
+// and the subtractions: only the query is rounded, and q.c is accumulated from exact products:
+//     FAST (qh . c, one MMA): err = 2^-11 + d 2^-24
+//     PRECISE (qh . c + ql . c, two MMAs): qh + ql represents q to 2^-22, 2d products accumulated:
+//         err = 2^-22 + 2 d 2^-24
+// With m = 0 the centred and the original frame coincide (sc = s, Vc = V, the row term is 0), so the
+// other two terms of screen_tol stand as they are; they still cover the epilogue's fma, the column
+// term (for L2 the stored |x|^2, the very value the canonical one adds), the packed column index and
+// the canonical value's own rounding.
+static float screen_tol_rel(int d, bool fast, bool exact_table = false) {
+    if (exact_table)
+        return (float)(4.2 * (fast ? 1.0 / 2048 + d / 16777216.0 : 1.0 / 4194304 + 2.0 * d / 16777216.0));
     const double err = fast ? (1.0 / 1024 + 1.0 / 4194304 + d / 16777216.0) : (3.0 / 4194304 + 3.0 * d / 16777216.0);
     return (float)(4.2 * (err + 1.0 / 8388608));
 }
@@ -799,9 +821,10 @@ topg_collect_kernel(const float* __restrict__ coarse, int64_t nq, int n, int G, 
 //   MODE 1: write the arg-min centroid to assign[row]
 //   MODE 2: select the nprobe smallest in shared memory and write keys[row][0..nprobe) (sorted)
 // rows: optional indirection (the CTA for list entry b handles row rows[b]); nrows_dev: its length.
-template <int MODE>
+// T: the table's row type, float, or __half for the stored rows of FLAT_SQ16 (MODE 0)
+template <int MODE, class T = float>
 __global__ void __launch_bounds__(128)
-rerank_kernel(const float* __restrict__ Q, int d, const float* __restrict__ cent, const float* __restrict__ cnorm,
+rerank_kernel(const float* __restrict__ Q, int d, const T* __restrict__ cent, const float* __restrict__ cnorm,
               int64_t nlist, int metric, const int32_t* __restrict__ groups, int G, int nprobe,
               const float* __restrict__ gmin, const float* __restrict__ gmin2, const uint8_t* __restrict__ gargc,
               int ng, ScreenTol tol, uint64_t* __restrict__ out, int32_t* __restrict__ assign,
@@ -1024,9 +1047,10 @@ __global__ void assign_resolve_kernel(const int32_t* __restrict__ groups, const 
 // composites over ALL columns, canonical values computed on the fly (seq-k FMA, the same chain as
 // rerank_kernel), selected by the radix select of dfx_select.cuh.  Rare by construction (more than
 // `margin` group minima within the tolerance: duplicate centroids / duplicate rows); slow but exact.
+template <class T>  // the table's row type (rerank_kernel)
 struct ExactLoader {
     const float* q;  // the row's query, staged in shared memory by the kernel
-    const float* X;
+    const T* X;
     const float* xnorm;
     int d, metric;   // d % 4 == 0 (the tensor-core path requires d % 64 == 0)
     __device__ __forceinline__ uint64_t operator()(int64_t /*row*/, int e) const {
@@ -1046,8 +1070,9 @@ struct ExactWriter {  // mode 2: keys[row][K]; mode 1: assign[row]; mode 0: out[
     }
 };
 // dynamic smem: P composites, then the row's query (d floats)
+template <class T>
 __global__ void __launch_bounds__(256)
-tc_exact_rows_kernel(const float* __restrict__ Q, ExactLoader ld, ExactWriter wr, const int32_t* __restrict__ ovf,
+tc_exact_rows_kernel(const float* __restrict__ Q, ExactLoader<T> ld, ExactWriter wr, const int32_t* __restrict__ ovf,
                      int n, int k, int P, int sort_cap) {
     DFX_DYN_SMEM(unsigned char, ex_smem, 16);
     uint64_t* s_out = reinterpret_cast<uint64_t*>(ex_smem);
@@ -1063,19 +1088,21 @@ tc_exact_rows_kernel(const float* __restrict__ Q, ExactLoader ld, ExactWriter wr
     }
 }
 // mode / K as in ExactWriter; Q rows are indexed by the values in ovf (chunk-relative)
-static void launch_exact_rows(const float* Q, const float* X, const float* xnorm, int64_t ncols, int d, int metric,
+template <class T>
+static void launch_exact_rows(const float* Q, const T* X, const float* xnorm, int64_t ncols, int d, int metric,
                               const int32_t* ovf, int64_t nrows, int mode, int K, int32_t* keys, int32_t* assign,
                               uint64_t* out, cudaStream_t st) {
     DFX_REQUIRE(K >= 1 && K <= 4096 && ncols < (1ll << 31), "exact fallback: bad K / column count");
     const int sort_cap = 2048, n = (int)ncols;
     const int base = (n <= sort_cap) ? (n > K ? n : K) : K;
     const int P = dfx_next_pow2(base < 2 ? 2 : base);
-    ExactLoader ld{nullptr, X, xnorm, d, metric};
+    ExactLoader<T> ld{nullptr, X, xnorm, d, metric};
     ExactWriter wr{mode, K, keys, assign, out};
     const unsigned grid = (unsigned)std::min<int64_t>(nrows, 2 * dfx_num_sms());
     const size_t smem = (size_t)P * 8 + (size_t)d * 4;
-    DFX_CUDA(cudaFuncSetAttribute(tc_exact_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    DFX_LAUNCH(tc_exact_rows_kernel, grid, 256, smem, st, Q, ld, wr, ovf, n, K, P, sort_cap);
+    auto kern = tc_exact_rows_kernel<T>;
+    DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    DFX_LAUNCH(kern, grid, 256, smem, st, Q, ld, wr, ovf, n, K, P, sort_cap);
 }
 
 // ------------------------------------------------------------------ host side
@@ -1229,8 +1256,8 @@ static void tc_stats_post(dfx_index* idx, const int32_t* ovf, int64_t rows, bool
 // the tolerance of a launch against table `tab`, for the rows tc_screen last prepared
 static ScreenTol tc_tol(const dfx_index* idx, const dfx_tc_table& tab, int d, bool fast) {
     ScreenTol t;
-    t.rel = screen_tol_rel(d, fast);
-    t.rel_fast = (!fast && idx->tc_mode == 0) ? screen_tol_rel(d, true) : 0.f;
+    t.rel = screen_tol_rel(d, fast, tab.one_plane());
+    t.rel_fast = (!fast && idx->tc_mode == 0) ? screen_tol_rel(d, true, tab.one_plane()) : 0.f;
     t.raw = screen_tol_raw(d);
     t.cmax2 = tab.cmax2;
     t.cmax2c = tab.cmax2c;
@@ -1254,11 +1281,14 @@ static void tc_screen(dfx_index* idx, int d, const float* d_x, int64_t nq, const
     DFX_LAUNCH(f16_rows_kernel, (unsigned)dfx_ceil_div(nq_pad, 8), 256, 0, st, d_x, nq, nq_pad, d,
                (const float*)tab.mean.as<float>(), 1, tab.scale, metric == DFX_METRIC_IP ? -1.f : -2.f, npl,
                idx->tc_q.as<__half>(), idx->tc_qmult.as<float>(), idx->tc_qn.as<float2>(), idx->tc_qterm.as<float>());
-    const void* table_h = tab.planes.p;
-    const float* cterm = tab.cterm.as<float>();
+    // one exact plane: the stored rows themselves, nlist of them (TMA zero-fills the last tile's tail)
+    const bool one = tab.one_plane();
+    const void* table_h = one ? static_cast<const void*>(tab.rows) : tab.planes.p;
+    const float* cterm = one ? tab.rows_cterm : tab.cterm.as<float>();
 #ifdef DFX_EMU
     emu_tc_screen(idx->tc_q.as<__half>(), idx->tc_qmult.as<float>(), idx->tc_qterm.as<float>(), nq, nq_pad,
-                  static_cast<const __half*>(table_h), nl_pad, d, npl, cterm, gmin, gmin2, gargc, tmin, ng);
+                  static_cast<const __half*>(table_h), nl_pad, nlist, one, d, npl, cterm, gmin, gmin2, gargc, tmin,
+                  ng);
     return;
 #else
     const int katoms = d / KATOM;
@@ -1266,7 +1296,7 @@ static void tc_screen(dfx_index* idx, int d, const float* d_x, int64_t nq, const
     const bool res = Smem::resident(katoms, npl) && (katoms == 1 || katoms == 2 || katoms == 4);
     CUtensorMap tmQ, tmC;
     make_tmap(&tmQ, idx->tc_q.p, npl * nq_pad, d);
-    make_tmap(&tmC, table_h, npl * nl_pad, d);
+    make_tmap(&tmC, table_h, one ? nlist : npl * nl_pad, d);
     const int qtiles = (int)(nq_pad / TILE), ctiles = (int)(nl_pad / TILE);
     const size_t smem = (size_t)Smem::total(res, katoms, npl) + 1024;
     const int slots = dfx_num_sms() * Smem::ctas_per_sm(res, katoms, npl);  // CTAs resident at once
@@ -1292,23 +1322,27 @@ static void tc_screen(dfx_index* idx, int d, const float* d_x, int64_t nq, const
     }
     dim3 grid((unsigned)csplit, (unsigned)qtiles);
     DFX_REQUIRE(qtiles <= 65535, "too many query tiles in one screening launch");
-#define DFX_TC_LAUNCH(KT_, NP)                                                                           \
+#define DFX_TC_LAUNCH(KT_, NP, ONE_)                                                                     \
     do {                                                                                                 \
-        auto kern = tc_coarse_kernel<KT_, NP>;                                                           \
+        auto kern = tc_coarse_kernel<KT_, NP, ONE_>;                                                     \
         DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));    \
-        DFX_LAUNCH(kern, grid, THREADS, smem, st, tmQ, tmC, (int)nq, (int)nq_pad, (int)nl_pad, katoms, cterm, \
-                   idx->tc_qmult.as<float>(), idx->tc_qterm.as<float>(), per, gmin, gmin2, gargc, tmin, ng); \
+        DFX_LAUNCH(kern, grid, THREADS, smem, st, tmQ, tmC, (int)nq, (int)nq_pad, (int)nl_pad, (int)nlist, katoms, \
+                   cterm, idx->tc_qmult.as<float>(), idx->tc_qterm.as<float>(), per, gmin, gmin2, gargc, tmin, ng); \
     } while (0)
-    // resident shapes get their k-atom count at compile time (npl * katoms <= 4)
+    // resident shapes get their k-atom count at compile time (npl * katoms <= 4); FAST takes either table
     if (npl == 1) {
-        if (res && katoms == 1) DFX_TC_LAUNCH(1, 1);
-        else if (res && katoms == 2) DFX_TC_LAUNCH(2, 1);
-        else if (res && katoms == 4) DFX_TC_LAUNCH(4, 1);
-        else DFX_TC_LAUNCH(0, 1);
+        if (res && katoms == 1) DFX_TC_LAUNCH(1, 1, false);
+        else if (res && katoms == 2) DFX_TC_LAUNCH(2, 1, false);
+        else if (res && katoms == 4) DFX_TC_LAUNCH(4, 1, false);
+        else DFX_TC_LAUNCH(0, 1, false);
+    } else if (one) {
+        if (res && katoms == 1) DFX_TC_LAUNCH(1, 2, true);
+        else if (res && katoms == 2) DFX_TC_LAUNCH(2, 2, true);
+        else DFX_TC_LAUNCH(0, 2, true);
     } else {
-        if (res && katoms == 1) DFX_TC_LAUNCH(1, 2);
-        else if (res && katoms == 2) DFX_TC_LAUNCH(2, 2);
-        else DFX_TC_LAUNCH(0, 2);
+        if (res && katoms == 1) DFX_TC_LAUNCH(1, 2, false);
+        else if (res && katoms == 2) DFX_TC_LAUNCH(2, 2, false);
+        else DFX_TC_LAUNCH(0, 2, false);
     }
 #undef DFX_TC_LAUNCH
 #endif  // DFX_EMU
@@ -1441,28 +1475,81 @@ void dfx_tc_coarse_search(dfx_index* idx, const float* d_x, int64_t nq, int npro
     }
 }
 
-// Flat search on tensor cores (default for d in {64, 128}, N >= 1024, k <= 100; dfx_set_param
+// Flat search on tensor cores (default for d a multiple of 64 up to 2048, N >= 1024, k <= 100; dfx_set_param
 // "flat_tensor_cores" = 0 selects the FFMA GEMM; the results are bit-identical): flat search (reference
 // index.py:94 IndexFlatIP, and IndexFlatL2 of the C-ABI) through the same machinery, with the
 // database rows in place of the centroids and k in place of nprobe.  Screening on tensor cores
 // over fp16 planes of the rows (built lazily, rebuilt after an add), the k + 8 groups with the
 // smallest minima, exact canonical values of the columns the screening cannot rule out
 // (rerank_kernel<0>) -- the values gemm_values_kernel would have produced for them, bit for bit.
+// FLAT_SQ16 screens its stored fp16 rows as one exact plane (tc_install_rows) and re-ranks them in place.
 // Leaves nq x ncand composites in idx->tc_cand and returns ncand; the caller selects and writes (D, I).
 bool dfx_tc_flat_covers(const dfx_index* idx, int k) {
     return dfx_tc_supported(idx->cfg.d) && idx->n_sorted >= 1024 && k <= 100;
 }
-int dfx_tc_flat_candidates(dfx_index* idx, const float* d_x, int64_t nq, int k, cudaStream_t st) {
-    DFX_REQUIRE(dfx_tc_flat_covers(idx, k), "flat search on tensor cores: the shape is not covered");
+
+// max over fp16 rows of |x|^2 (one warp per row, fp64 sums rounded once; atomicMax on the bits of
+// non-negative floats).  A non-finite code makes it +inf or NaN.
+__global__ void __launch_bounds__(256)
+rows_max2_kernel(const __half* __restrict__ x, int64_t n, int d, float* __restrict__ max2) {
+    const int lane = threadIdx.x & 31;
+    const int64_t row = (int64_t)blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+    if (row >= n) return;
+    double n2 = 0.0;
+    for (int k = lane; k < d; k += 32) {
+        const double v = __half2float(x[row * d + k]);
+        n2 += v * v;
+    }
+    n2 = tc_warp_sum(n2);
+    const float r = (float)n2;
+    if (lane == 0) atomicMax(reinterpret_cast<int*>(max2), __float_as_int(r <= FLT_MAX ? r : INFINITY));  // NaN too
+}
+
+// The screening table of a FLAT_SQ16 index: its stored rows as one exact fp16 plane, no mean, scale 1,
+// the column term |x|^2 (L2) or 0 (IP); synchronises.  Only max |x|^2 is computed, for the tolerance.
+static void tc_install_rows(dfx_index* idx, cudaStream_t st) {
     const int d = idx->cfg.d;
     const int64_t N = idx->n_sorted;
+    dfx_tc_table& tab = idx->tc_tab;
+    tab.mean.reserve((size_t)d * 4 + 8);  // m = 0, then the maximum
+    float* max2 = tab.mean.as<float>() + d;
+    DFX_CUDA(cudaMemsetAsync(tab.mean.p, 0, (size_t)d * 4 + 8, st));
+    DFX_LAUNCH(rows_max2_kernel, (unsigned)dfx_ceil_div(N, 8), 256, 0, st, idx->payload.as<__half>(), N, d, max2);
+    float h = 0.f;
+    DFX_CUDA(cudaMemcpyAsync(&h, max2, 4, cudaMemcpyDeviceToHost, st));
+    DFX_CUDA(cudaStreamSynchronize(st));
+    tab.cmax2 = tab.cmax2c = h;
+    tab.scale = 1.f;
+    idx->tc_flat_finite = std::isfinite(h);
+    if (idx->tc_mode == 0) idx->tc_fast = false;
+    idx->tc_stat_pending = false;
+    idx->tc_acc_rows = idx->tc_acc_bad = 0;
+}
+
+bool dfx_tc_flat_table(dfx_index* idx, cudaStream_t st) {
+    const int64_t N = idx->n_sorted;
+    const bool sq16 = idx->cfg.kind == DFX_FLAT_SQ16;
+    if (idx->tc_flat_rows != N) {  // (re)build the screening table of the rows
+        if (sq16) tc_install_rows(idx, st);
+        else tc_install_table(idx, idx->payload.as<float>(), N, st);
+        idx->tc_flat_rows = N;
+    }
+    if (sq16) {  // the rows may have moved (an add grows the store)
+        idx->tc_tab.rows = idx->payload.as<__half>();
+        idx->tc_tab.rows_cterm = idx->cfg.metric == DFX_METRIC_L2 ? idx->xnorm.as<float>() : nullptr;
+    }
+    return idx->tc_flat_finite;
+}
+
+int dfx_tc_flat_candidates(dfx_index* idx, const float* d_x, int64_t nq, int k, cudaStream_t st) {
+    DFX_REQUIRE(dfx_tc_flat_covers(idx, k), "flat search on tensor cores: the shape is not covered");
+    const int64_t N = idx->n_sorted;
+    DFX_REQUIRE(idx->tc_flat_rows == N && idx->tc_flat_finite,
+                "flat search on tensor cores: no usable screening table (dfx_tc_flat_table)");
+    const int d = idx->cfg.d;
     const int metric = idx->cfg.metric;
     const int64_t nl_pad = dfx_ceil_div(N, tc::TILE) * tc::TILE;
     const int ng = (int)(nl_pad / 32);
-    if (idx->tc_flat_rows != N) {  // (re)build the screening table of the rows
-        tc_install_table(idx, idx->payload.as<float>(), N, st);
-        idx->tc_flat_rows = N;
-    }
     tc_stats_poll(idx, st);
     const bool fast = idx->tc_fast;
     int G = k + 8;
@@ -1471,13 +1558,16 @@ int dfx_tc_flat_candidates(dfx_index* idx, const float* d_x, int64_t nq, int k, 
     idx->tc_cand.reserve((size_t)nq * ncand * 8);
     const Screened s = tc_screen_chunk(idx, d, d_x, nq, nq, ng, G, idx->tc_tab, fast ? 1 : 2, N, metric, st);
     const ScreenTol tol = tc_tol(idx, idx->tc_tab, d, fast);
-    auto kern = rerank_kernel<0>;
-    DFX_LAUNCH(kern, (unsigned)nq, 128, (size_t)d * 4, st, d_x, d, idx->payload.as<float>(), idx->xnorm.as<float>(), N,
-               metric, s.groups, G, k, s.gmin, s.gmin2, s.gargc, ng, tol, idx->tc_cand.as<uint64_t>(),
-               (int32_t*)nullptr, (const int32_t*)nullptr, (const int32_t*)nullptr, nq, (int32_t*)nullptr, s.ovf);
-    // rows with more near-ties than selected groups: their ncand slots become the exact top-ncand
-    launch_exact_rows(d_x, idx->payload.as<float>(), idx->xnorm.as<float>(), N, d, metric, s.ovf, nq, 0, ncand,
-                      nullptr, nullptr, idx->tc_cand.as<uint64_t>(), st);
+    dfx_with_flat_rows(idx, [&](auto rows) {
+        using T = std::remove_cv_t<std::remove_pointer_t<decltype(rows)>>;
+        auto kern = rerank_kernel<0, T>;
+        DFX_LAUNCH(kern, (unsigned)nq, 128, (size_t)d * 4, st, d_x, d, rows, idx->xnorm.as<float>(), N, metric,
+                   s.groups, G, k, s.gmin, s.gmin2, s.gargc, ng, tol, idx->tc_cand.as<uint64_t>(), (int32_t*)nullptr,
+                   (const int32_t*)nullptr, (const int32_t*)nullptr, nq, (int32_t*)nullptr, s.ovf);
+        // rows with more near-ties than selected groups: their ncand slots become the exact top-ncand
+        launch_exact_rows(d_x, rows, idx->xnorm.as<float>(), N, d, metric, s.ovf, nq, 0, ncand, nullptr, nullptr,
+                          idx->tc_cand.as<uint64_t>(), st);
+    });
     tc_stats_post(idx, s.ovf, nq, fast, st);
     return ncand;
 }

@@ -25,9 +25,13 @@ LIB_PATH = os.path.join(_HERE, "libdfx.so")
 
 KIND_FLAT, KIND_IVF_FLAT, KIND_IVF_PQ, KIND_IVF_SQ16, KIND_IVF_SQ8, KIND_IVF_PQ_FS = 0, 1, 2, 3, 4, 5
 KIND_IVF_PQR = 6
+KIND_FLAT_SQ16 = 7  # faiss IndexScalarQuantizer(QT_fp16), the factory string "SQfp16"
 METRIC_INNER_PRODUCT, METRIC_L2 = 0, 1  # faiss enum values (reference index_cfg.py:44-52)
 KIND_NAMES = {KIND_FLAT: "flat", KIND_IVF_FLAT: "ivf_flat", KIND_IVF_PQ: "ivf_pq", KIND_IVF_SQ16: "ivf_sq",
-              KIND_IVF_SQ8: "ivf_sq8", KIND_IVF_PQ_FS: "ivf_pq_fs", KIND_IVF_PQR: "ivf_pqr"}
+              KIND_IVF_SQ8: "ivf_sq8", KIND_IVF_PQ_FS: "ivf_pq_fs", KIND_IVF_PQR: "ivf_pqr",
+              KIND_FLAT_SQ16: "flat_sq16"}
+# the kinds without lists: every row is scored, ids are positions, `metric` is the search metric
+FLAT_KINDS = (KIND_FLAT, KIND_FLAT_SQ16)
 
 # every symbol include/dfx.h declares (tests check that the library exports each one)
 EXPORTED_SYMBOLS = [
@@ -65,6 +69,7 @@ STATE_ARRAYS = {
 # a flat refinement (",RFlat") adds STATE_RFLAT's
 STATE_KINDS = {
     "flat": (("metric",), ("xb",)),
+    "flat_sq16": (("metric",), ("codes16",)),  # the fp16 rows in id order
     "ivf_flat": (("nlist", "metric"), ("centroids", "list_off", "ids", "vecs")),
     "ivf_pq": (("nlist", "coarse_metric", "M", "ksub"), ("centroids", "codebooks", "list_off", "ids", "codes", "tvals")),
     "ivf_sq": (("nlist", "coarse_metric"), ("centroids", "list_off", "ids", "codes16")),
@@ -169,10 +174,12 @@ class _Quantizer:
 class GpuIndex:
     """One shard resident in the HBM of one H100, behind the faiss-object surface."""
 
-    def __init__(self, kind, d, metric=METRIC_INNER_PRODUCT, nlist=0, pq_m=0, pq_nbits=8, device=None, refine_m=0,
+    def __init__(self, kind, d, metric=METRIC_INNER_PRODUCT, nlist=0, pq_m=0, pq_nbits=None, device=None, refine_m=0,
                  refine_flat=False):
         import torch  # device bookkeeping only
 
+        if pq_nbits is None:  # 8 (faiss's default) wherever it means something; FLAT_SQ16 takes none
+            pq_nbits = 0 if int(kind) == KIND_FLAT_SQ16 else 8
         if device is None:
             device = torch.cuda.current_device() if torch.cuda.is_available() else 0
         self.kind, self.d, self.metric = int(kind), int(d), int(metric)
@@ -181,7 +188,7 @@ class GpuIndex:
                            int(refine_m), 1 if refine_flat else 0)
         self._h = C.c_void_p()
         _check(lib().dfx_create(C.byref(self._cfg), C.byref(self._h)))
-        if self.kind != KIND_FLAT:
+        if self.kind not in FLAT_KINDS:
             self.quantizer = _Quantizer(self)
         self.pq_m = int(pq_m)
         self.pq_nbits = int(pq_nbits)
@@ -215,9 +222,10 @@ class GpuIndex:
 
     @property
     def search_metric(self):
-        """The metric of the distances search and range_search report: `metric` for FLAT and IVF_FLAT;
-        L2 for the codecs, whose `metric` is the coarse quantizer's (the reference never forwards it)."""
-        return self.metric if self.kind in (KIND_FLAT, KIND_IVF_FLAT) else METRIC_L2
+        """The metric of the distances search and range_search report: `metric` for FLAT, FLAT_SQ16 and
+        IVF_FLAT; L2 for the IVF codecs, whose `metric` is the coarse quantizer's (the reference never
+        forwards it)."""
+        return self.metric if self.kind in (KIND_FLAT, KIND_FLAT_SQ16, KIND_IVF_FLAT) else METRIC_L2
 
     @property
     def generation(self):

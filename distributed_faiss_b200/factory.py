@@ -9,6 +9,9 @@ an oracle-backed engine.
 
 Tokens are case-sensitive, as in faiss:
   "Flat"                          -> flat      (IndexFlat, the given metric)
+  "SQfp16"                        -> flat_sq16 (IndexScalarQuantizer QT_fp16, the given metric: every row
+                                              stored as its fp16 rounding, 2 d bytes per vector, no
+                                              training; searched exactly over the decoded rows)
   "IVF{n},Flat"                   -> ivf_flat  (IndexIVFFlat, the given metric)
   "IVF{n},PQ{M}" / "IVF{n},PQ{M}x8" -> ivf_pq  (IndexIVFPQ, 8-bit codes, L2 only; M a multiple of 4,
                                               at most 128, that divides d)
@@ -31,14 +34,15 @@ Tokens are case-sensitive, as in faiss:
                                               L2 only
 Everything else (OPQ / PCA prefixes, HNSW, IVF{n}_HNSW quantizers, RFlat after Flat, IVF{n},Flat or
 PQ{M}+{M2}, every Refine(...) spelling, IDMap, PQ{M}x4, PQ{M}x4fsr, a FastScan block size suffix "_{bbs}",
-SQ4 / SQ6, malformed n or M) raises RuntimeError.
+SQ4 / SQ6, SQ8 or any other scalar quantizer without IVF (they need trained ranges), SQfp16 with a suffix,
+malformed n or M) raises RuntimeError.
 """
 import re
 from typing import NamedTuple
 
 METRIC_INNER_PRODUCT, METRIC_L2 = 0, 1  # faiss enum values
 
-ACCEPTED_FORMS = ("Flat", "IVF{n},Flat", "IVF{n},PQ{M}", "IVF{n},PQ{M}x8", "IVF{n},PQ{M}x4fs", "IVF{n},PQ{M}+{M2}",
+ACCEPTED_FORMS = ("Flat", "SQfp16", "IVF{n},Flat", "IVF{n},PQ{M}", "IVF{n},PQ{M}x8", "IVF{n},PQ{M}x4fs", "IVF{n},PQ{M}+{M2}",
                   "IVF{n},SQfp16", "IVF{n},SQ8", "IVF{n},PQ{M},RFlat", "IVF{n},PQ{M}x8,RFlat", "IVF{n},PQ{M}x4fs,RFlat",
                   "IVF{n},SQfp16,RFlat", "IVF{n},SQ8,RFlat")
 
@@ -49,8 +53,8 @@ _PQ_M_MAX = 128
 
 
 class FactorySpec(NamedTuple):
-    """kind: a name of engine.KIND_NAMES ("flat", "ivf_flat", "ivf_pq", "ivf_sq", "ivf_sq8", "ivf_pq_fs",
-    "ivf_pqr").  metric: flat / ivf_flat: the search metric; the codecs: the coarse quantizer's metric
+    """kind: a name of engine.KIND_NAMES ("flat", "flat_sq16", "ivf_flat", "ivf_pq", "ivf_sq", "ivf_sq8",
+    "ivf_pq_fs", "ivf_pqr").  metric: flat / flat_sq16 / ivf_flat: the search metric; the codecs: the coarse quantizer's metric
     (their search is L2).  refine_m: ivf_pqr's M2 (bytes of the refinement code), else 0.
     refine_flat: the string ends in ",RFlat" (exact re-ranking on stored fp32 vectors)."""
     kind: str
@@ -75,6 +79,8 @@ def parse_factory(dim: int, factory_string: str, metric: int) -> FactorySpec:
     s = factory_string if isinstance(factory_string, str) else ""
     if s == "Flat":
         return FactorySpec("flat", int(metric))
+    if s == "SQfp16":
+        return FactorySpec("flat_sq16", int(metric))
     m = _IVF.fullmatch(s)
     # re-ranking an exact index is a no-op, and IVF-PQR has its own refinement: RFlat follows a codec only
     rflat = m is not None and m.group(6) is not None

@@ -1,7 +1,8 @@
 """Reader / writer for the faiss on-disk index format, for the four index types the reference's
 builders create (reference index.py:94 IndexFlatIP, :36-40 IndexIVFFlat, :43-48 IndexIVFPQ,
-:63-68 IndexIVFScalarQuantizer(QT_fp16)) and the 8-bit scalar quantizer of the factory string
-"IVF{n},SQ8" (IndexIVFScalarQuantizer(QT_8bit)); the reference saves shards with
+:63-68 IndexIVFScalarQuantizer(QT_fp16)), the 8-bit scalar quantizer of the factory string
+"IVF{n},SQ8" (IndexIVFScalarQuantizer(QT_8bit)) and the fp16 scalar quantizer without lists of the
+factory string "SQfp16" (IndexScalarQuantizer(QT_fp16)); the reference saves shards with
 `faiss.write_index(self.faiss_index, index_file)` (index.py:459) and loads them with
 `faiss.read_index` (index.py:303).  SURVEY.md section 8(f) next-3.
 
@@ -21,6 +22,10 @@ with or without a flat refinement.
 Layout (little endian, no padding; `vec<T>` = u64 count + raw elements):
   header   : i32 d, i64 ntotal, i64 1<<20, i64 1<<20, u8 is_trained, i32 metric (0 IP, 1 L2)
   flat     : fourcc "IxFI" | "IxF2", header, vec<f32> xb
+  SQ       : fourcc "IxSQ", header (with the search metric), SQ (i32 qtype = 4 (fp16), i32 rangestat = 0,
+             f32 rangestat_arg = 0, u64 d, u64 code_size = 2 d, vec<f32> trained (empty)), vec<u8> codes
+             [ntotal][2 d] (little-endian fp16 of the raw rows, in id order); other qtypes are refused
+             [faiss-upstream: IndexScalarQuantizer, index_write.cpp]
   ivf hdr  : header, u64 nlist, u64 nprobe, <quantizer: flat index of the centroids>,
              u8 direct-map type (0), vec<i64> direct map (empty)
   invlists : fourcc "ilar", u64 nlist, u64 code_size, fourcc "full" + vec<u64> sizes  (or "sprs" +
@@ -244,6 +249,15 @@ def write_index(state: Dict, path: str, nprobe: int = 1) -> None:
                 _wheader(f, state["d"], len(state["ids"]), METRIC_L2)
         if kind == "flat":
             _write_flat(f, state["xb"], int(state["metric"]))
+        elif kind == "flat_sq16":
+            d = int(state["d"])
+            c16 = np.ascontiguousarray(state["codes16"], dtype="<u2").reshape(-1, d)
+            f.write(b"IxSQ")
+            _wheader(f, d, c16.shape[0], int(state["metric"]))
+            _w(f, "iif", QT_FP16, 0, 0.0)
+            _w(f, "QQ", d, 2 * d)
+            _w(f, "Q", 0)  # trained: empty for fp16
+            _wvec(f, c16.view(np.uint8), np.uint8)
         elif kind == "ivf_flat":
             f.write(b"IwFl")
             _write_ivf_header(f, state, int(state["metric"]), int(state["metric"]), nprobe)
@@ -331,10 +345,25 @@ def _read_one(f: BinaryIO, cc: str) -> Tuple[Dict, int]:
     if cc in ("IxFI", "IxF2", "IxFl"):
         st = _read_flat_body(f, cc)
         return st, 1
+    if cc == "IxSQ":
+        d, ntotal, _, metric = _rheader(f)
+        qtype, _, _ = _r(f, "iif")
+        sd, scs = _r(f, "QQ")
+        trained = _rvec(f, np.float32)
+        codes = _rvec(f, np.uint8)
+        if qtype != QT_FP16 or sd != d or scs != 2 * d or trained.size != 0:
+            raise FaissFormatError(f"IndexScalarQuantizer: only QT_fp16 (qtype {QT_FP16}) with 2 * d bytes per "
+                                   f"vector is supported (qtype={qtype}, d={sd}, code_size={scs})")
+        if metric not in (METRIC_IP, METRIC_L2):
+            raise FaissFormatError(f"IndexScalarQuantizer: metric {metric} is not supported")
+        if codes.size != ntotal * 2 * d:
+            raise FaissFormatError("IndexScalarQuantizer: the codes do not hold ntotal vectors")
+        return {"kind": "flat_sq16", "d": d, "metric": metric, "codes16": codes.view("<u2").reshape(ntotal, d)}, 1
     if cc not in ("IwFl", "IwPQ", "IwQR", "IwSq"):
         raise FaissFormatError(
             f"faiss index type {cc!r} is not one of the types the GPU search path serves "
-            "(IndexFlat, IndexIVFFlat, IndexIVFPQ, IndexIVFPQR, IndexIVFScalarQuantizer fp16 / 8bit)")
+            "(IndexFlat, IndexScalarQuantizer fp16, IndexIVFFlat, IndexIVFPQ, IndexIVFPQR, "
+            "IndexIVFScalarQuantizer fp16 / 8bit)")
     d, ntotal, metric, nlist, nprobe, cent, cmetric = _read_ivf_header(f)
     st = {"d": d, "nlist": nlist, "centroids": cent}
     if cc == "IwFl":

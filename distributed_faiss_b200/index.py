@@ -20,7 +20,8 @@ Builders (reference index.py:93-100):
                   says, nprobe = cfg.nprobe (index.py:71-86)
   no builder, `faiss_factory` set -> the factory string with {centroids} substituted, the cfg metric
                   for the index and its quantizer, nprobe = the faiss default 1 (index.py:385-396)
-Factory strings are parsed by factory.parse_factory ("Flat", "IVF{n},Flat", "IVF{n},PQ{M}[x8]",
+Factory strings are parsed by factory.parse_factory ("Flat", "SQfp16" (IndexScalarQuantizer QT_fp16: the
+rows stored as fp16, searched exactly over the decoded rows), "IVF{n},Flat", "IVF{n},PQ{M}[x8]",
 "IVF{n},PQ{M}x4fs" (FastScan: 4-bit codes of the raw vectors, 8-bit quantized distance tables),
 "IVF{n},PQ{M}+{M2}" (IndexIVFPQR: IVF-PQ candidates re-ranked on a second, M2-byte residual code),
 "IVF{n},SQfp16", "IVF{n},SQ8", and each codec form but PQ{M}+{M2} followed by ",RFlat" (IndexRefineFlat:
@@ -63,7 +64,7 @@ def factory_spec(cfg: IndexCfg):
         # and faiss's default metric, L2, for the index and its quantizer (cfg.metric only picks the
         # k-means clustering index)
         spec = parse_factory(cfg.dim, cfg.faiss_factory, METRIC_L2)
-        if spec.kind == "flat":
+        if spec.kind in ("flat", "flat_sq16"):
             raise RuntimeError(f"ivf_gpu needs an IVF factory string, got {cfg.faiss_factory!r} "
                                "(faiss.extract_index_ivf fails on it in the reference)")
         return spec
@@ -83,7 +84,7 @@ def default_engine_factory(cfg: IndexCfg, device: Optional[int] = None):
     spec = factory_spec(cfg)
     if spec is not None:
         kind = {name: k for k, name in engine.KIND_NAMES.items()}[spec.kind]
-        nbits = 4 if spec.kind == "ivf_pq_fs" else 8  # FastScan: 4-bit codes
+        nbits = {"ivf_pq_fs": 4, "flat_sq16": 0}.get(spec.kind, 8)  # FastScan: 4-bit codes; SQfp16: none
         idx = engine.GpuIndex(kind, cfg.dim, spec.metric, nlist=spec.nlist, pq_m=spec.pq_m, pq_nbits=nbits,
                               device=device, refine_m=spec.refine_m, refine_flat=spec.refine_flat)
         if spec.refine_flat and "k_factor" in cfg.extra:

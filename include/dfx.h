@@ -47,11 +47,17 @@ enum {
                          "IVF{n},PQ{M}x4fs" (index.py:380-396).  4-bit codes packed two per byte; the
                          search quantizes each query's distance table to 8 bits and sums it in
                          integers (DESIGN.md section 2).  L2 only, for the index and its quantizer */
-    DFX_IVF_PQR = 6   /* faiss.IndexIVFPQR: the factory string "IVF{n},PQ{M}+{M2}" (index.py:380-396).
+    DFX_IVF_PQR = 6,  /* faiss.IndexIVFPQR: the factory string "IVF{n},PQ{M}+{M2}" (index.py:380-396).
                          An 8-bit IVF-PQ (by_residual) whose residual error is encoded again by a second
                          8-bit PQ of M2 bytes, stored by id outside the lists.  A search runs the IVF-PQ
                          search for k' = k * k_factor candidates and re-ranks them on the reconstruction
                          c + PQ1 + PQ2 (DESIGN.md section 2).  L2 only, for the index and its quantizer */
+    DFX_FLAT_SQ16 = 7 /* faiss.IndexScalarQuantizer(d, QT_fp16, metric): the factory string "SQfp16"
+                         (index.py:385-396).  No training.  Each row is stored as its fp16 rounding
+                         (2 d bytes per vector, plus its fp32 squared norm under L2), ids are positions,
+                         and a search returns bit for bit what a FLAT index of the same metric returns over
+                         the decoded rows (DESIGN.md section 2).  nlist, pq_m, pq_nbits, refine_m and
+                         refine_flat must be 0 */
 };
 
 /* faiss.METRIC_INNER_PRODUCT / faiss.METRIC_L2 (index_cfg.py:44-52) */
@@ -59,7 +65,7 @@ enum { DFX_METRIC_IP = 0, DFX_METRIC_L2 = 1 };
 
 typedef struct dfx_cfg {
     int32_t kind;     /* DFX_FLAT ... */
-    int32_t metric;   /* FLAT / IVF_FLAT: search metric.  IVF_PQ / IVF_SQ16 / IVF_SQ8: metric of
+    int32_t metric;   /* FLAT / IVF_FLAT / FLAT_SQ16: search metric.  IVF_PQ / IVF_SQ16 / IVF_SQ8: metric of
                          the coarse quantizer only -- the reference never forwards it to the
                          index, which is therefore always L2 (index.py:44-46, 64-66).
                          IVF_PQ_FS: must be L2 (an inner-product metric is refused). */
@@ -103,8 +109,9 @@ int dfx_add_dev(dfx_index *idx, int64_t n, const float *d_x, void *stream);
  *   groups, and back as soon as it does),
  *   1 = FAST (fp16 operands, one MMA per k-step), 2 = PRECISE (fp16 hi/lo split, three MMAs);
  *   "tc_auto_window" (16384): rows AUTO observes before PRECISE may become FAST;
- * "flat_tensor_cores" (1): 0 runs FLAT searches through the FFMA GEMM instead of the tensor-core
- *   screening + exact re-rank;
+ * "flat_tensor_cores" (1): 0 runs FLAT and FLAT_SQ16 searches through the FFMA GEMM instead of the
+ *   tensor-core screening + exact re-rank (a FLAT_SQ16 shard holding a non-finite code, an input
+ *   beyond +-65504, always takes the FFMA GEMM);
  * "interleaved" (1): 0 keeps IVF-PQ (M = 32) codes row-major (one vector per lane, table from
  *   pq_prep_kernel) instead of the block-interleaved layout of the fused table-build + scan;
  * "il2_threads" (0 = 256) / "il2_prefetch" (-1 = 4 blocks): CTA shape and L2 prefetch distance of
@@ -125,7 +132,10 @@ int dfx_set_param(dfx_index *idx, const char *name, double value);
  * rows of IVF searches with k > 1024; IVF searches keep it within 128 MiB by their query chunk),
  * "refine_ms" / "refine_launches" (IVF_PQR / refine_flat with profiling on: summed device time and number of
  * the refinement stages -- re-rank kernel and final selection -- since the last reset of
- * dfx_profile_read; synchronises) */
+ * dfx_profile_read; synchronises), "index_bytes" (bytes of device memory the index's persistent
+ * arrays hold: the stored vectors, their codes, norms, ids and lists, the trained arrays and the
+ * tensor-core screening table; not the search workspace; the allocated capacity, so it includes
+ * the headroom of a growing store, which dfx_reserve avoids) */
 int dfx_get_param(dfx_index *idx, const char *name, double *value);
 /* pre-size the shard for n_total vectors (optional; avoids regrowth while bulk loading) */
 int dfx_reserve(dfx_index *idx, int64_t n_total);
@@ -150,11 +160,11 @@ int dfx_search_dev(dfx_index *idx, int64_t nq, const float *d_x, int64_t k, floa
  * vector is returned when its distance D passes the radius strictly, as in faiss: D < radius for
  * L2, D > radius for inner product (a distance equal to the radius is excluded; NaN never
  * passes; +-inf radii are allowed, a NaN radius is refused).  The metric is the shard's SEARCH
- * metric: cfg.metric for FLAT and IVF_FLAT, L2 for IVF_PQ, IVF_SQ16 and IVF_SQ8 (whose cfg.metric
+ * metric: cfg.metric for FLAT, FLAT_SQ16 and IVF_FLAT, L2 for IVF_PQ, IVF_SQ16 and IVF_SQ8 (whose cfg.metric
  * is the coarse quantizer's).  Every returned (D, I) pair is bit for bit the pair dfx_search at a
  * large enough k reports for that id, and each query's results are sorted best first in the total
  * order of the search (ranking value ascending, then id ascending; inner product descending).
- * Served: FLAT, IVF_FLAT, IVF_PQ (8- and 4-bit codes, every layout), IVF_SQ16, IVF_SQ8.  Refused
+ * Served: FLAT, FLAT_SQ16, IVF_FLAT, IVF_PQ (8- and 4-bit codes, every layout), IVF_SQ16, IVF_SQ8.  Refused
  * before anything is launched: IVF_PQ_FS (its distances are dequantized after the selection),
  * IVF_PQR and refine_flat (a radius over two stages of distances is not defined), an untrained IVF
  * index.  Limits: an IVF query chunk's candidates obey the rule of k > 1024 (the nprobe longest
@@ -248,6 +258,7 @@ int dfx_map_ids_dev(int64_t n, const int64_t *d_ids, const int64_t *d_table, int
  *   (IVF_PQ_FS: "centroids", "codebooks" f32[M,16,dsub], "list_off", "ids" and "codes" u8[ntotal,M],
  *   one 4-bit code per byte as for IVF_PQ; no "tvals", since the codes are not residuals)
  *   "vecs" f32[ntotal,d] (IVF_FLAT)   "codes16" u16[ntotal,d]   "xb" f32[ntotal,d] (FLAT)
+ *   (FLAT_SQ16: "codes16" alone, the fp16 rows in id order; like "xb" its import sets ntotal)
  *   "sq_trained" f32[2,d] (IVF_SQ8: vmin, then vdiff -- faiss's ScalarQuantizer::trained)
  *   "codes8" u8[ntotal,d] (IVF_SQ8)
  *   (IVF_PQR: the IVF_PQ arrays with 8-bit codes, plus "refine_codebooks" f32[M2,256,d/M2] and
