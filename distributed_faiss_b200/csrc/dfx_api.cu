@@ -102,7 +102,7 @@ int dfx_debug_tc_screen(dfx_index* idx, int64_t nq, const float* d_x, int npl, f
 int dfx_create(const dfx_cfg* cfg, dfx_index** out) {
     DFX_API_BEGIN
     DFX_REQUIRE(cfg && out, "null argument");
-    DFX_REQUIRE(cfg->kind >= DFX_FLAT && cfg->kind <= DFX_FLAT_SQ16, "unknown index kind");
+    DFX_REQUIRE(cfg->kind >= DFX_FLAT && cfg->kind <= DFX_FLAT_PQ, "unknown index kind");
     DFX_REQUIRE(cfg->kind == DFX_IVF_PQR || cfg->refine_m == 0, "refine_m must be 0 for every kind but IVF_PQR");
     DFX_REQUIRE(cfg->metric == DFX_METRIC_IP || cfg->metric == DFX_METRIC_L2,
                 "Only dot and l2 metrics are supported.");
@@ -119,7 +119,22 @@ int dfx_create(const dfx_cfg* cfg, dfx_index** out) {
                         std::to_string(cfg->pq_m) + ", pq_nbits=" + std::to_string(cfg->pq_nbits) + ", refine_m=" +
                         std::to_string(cfg->refine_m) + ", refine_flat=" + std::to_string(cfg->refine_flat));
     }
-    if (cfg->kind != DFX_FLAT && cfg->kind != DFX_FLAT_SQ16) {
+    if (cfg->kind == DFX_FLAT_PQ) {
+        // faiss's IndexPQ(d, M, 8, metric): no lists, no refinement; the limits of 8-bit IVF-PQ (one query's
+        // fp32 table, M x 256 x 4 B, is staged in one thread block's shared memory)
+        DFX_REQUIRE(cfg->nlist == 0 && cfg->refine_m == 0 && cfg->refine_flat == 0,
+                    "FLAT_PQ: nlist, refine_m and refine_flat must be 0 (a product quantizer without inverted "
+                    "lists), got nlist=" + std::to_string(cfg->nlist) + ", refine_m=" + std::to_string(cfg->refine_m) +
+                        ", refine_flat=" + std::to_string(cfg->refine_flat));
+        DFX_REQUIRE(cfg->pq_nbits == 8, "FLAT_PQ: 8 bits per sub-quantizer, got " + std::to_string(cfg->pq_nbits));
+        DFX_REQUIRE(cfg->pq_m >= 4 && cfg->pq_m <= 128 && cfg->pq_m % 4 == 0 && cfg->d % cfg->pq_m == 0,
+                    "FLAT_PQ: the number of sub-quantizers must be a multiple of 4, at most 128, that divides d, "
+                    "got M=" + std::to_string(cfg->pq_m) + ", d=" + std::to_string(cfg->d));
+        idx->M = cfg->pq_m;
+        idx->ksub = 256;
+        idx->dsub = cfg->d / cfg->pq_m;
+    }
+    if (cfg->kind != DFX_FLAT && cfg->kind != DFX_FLAT_SQ16 && cfg->kind != DFX_FLAT_PQ) {
         DFX_REQUIRE(cfg->nlist >= 1 && cfg->nlist < (1ll << 24), "nlist must be in [1, 2^24)");
         DFX_REQUIRE(cfg->d % 4 == 0, "IVF indexes need a dimension that is a multiple of 4");
     }
@@ -503,7 +518,7 @@ int64_t dfx_get_nprobe(const dfx_index* idx) { return idx->nprobe; }
 int64_t dfx_generation(const dfx_index* idx) { return (int64_t)idx->generation.load(); }
 int64_t dfx_ntotal(const dfx_index* idx) { return idx->ntotal(); }
 int64_t dfx_nlist(const dfx_index* idx) { return idx->is_flat() ? 0 : idx->cfg.nlist; }
-int dfx_is_trained(const dfx_index* idx) { return (idx->trained || idx->is_flat()) ? 1 : 0; }
+int dfx_is_trained(const dfx_index* idx) { return (idx->trained || idx->flat_rows()) ? 1 : 0; }
 
 int dfx_get_centroids(dfx_index* idx, float* out) {
     DFX_API_BEGIN
@@ -625,6 +640,9 @@ static std::vector<ExchangeArray> exchange_arrays(dfx_index* idx) {
     if (kind == DFX_FLAT) return {{"xb", &idx->payload, C::none, n * d * 4, false, true, "xb: wrong size"}};
     if (kind == DFX_FLAT_SQ16)
         return {{"codes16", &idx->payload, C::none, n * d * 2, false, true, "codes16: wrong size (u16[ntotal, d])"}};
+    if (kind == DFX_FLAT_PQ)
+        return {{"codebooks", &idx->codebooks, C::none, M * idx->ksub * idx->dsub * 4, true, true, "codebooks: wrong size"},
+                {"codes", &idx->payload, C::none, n * M, false, true, "codes: wrong size (u8[ntotal, M])"}};
     std::vector<ExchangeArray> a{{"centroids", &idx->centroids, C::none, nlist * d * 4, true, true, "centroids: wrong size"}};
     if (idx->has_pq())
         a.push_back({"codebooks", &idx->codebooks, C::none, M * idx->ksub * idx->dsub * 4, true, true, "codebooks: wrong size"});
@@ -720,7 +738,7 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
     const std::vector<ExchangeArray> arrays = exchange_arrays(idx);
     const ExchangeArray* a = find_exchange_array(arrays, n);
     if (!a || !a->importable) throw DfxError{"cannot import array '" + n + "'"};
-    if (idx->is_flat()) {  // the import sets the number of rows
+    if (idx->is_flat() && a->buf == &idx->payload) {  // the import of the rows sets their number
         const int64_t rb = (int64_t)idx->row_bytes();
         DFX_REQUIRE(nbytes % rb == 0, a->size_error);
         idx->n_sorted = nbytes / rb;
@@ -777,7 +795,7 @@ int dfx_set_array(dfx_index* idx, const char* name, const void* in, int64_t nbyt
         idx->update_list_lengths();
         idx->n_sorted = idx->h_list_off[(size_t)nlist];
         idx->n_pending = 0;
-    } else if (idx->is_flat() && idx->cfg.metric == DFX_METRIC_L2) {  // "xb" / "codes16": the rows' norms
+    } else if (idx->flat_rows() && idx->cfg.metric == DFX_METRIC_L2) {  // "xb" / "codes16": the rows' norms
         idx->xnorm.reserve((size_t)std::max<int64_t>(idx->n_sorted, 1) * 4);
         dfx_with_flat_rows(idx, [&](auto rows) {
             dfx_launch_row_norms(rows, idx->n_sorted, (int)d, idx->xnorm.as<float>(), idx->stream);
@@ -815,6 +833,7 @@ int dfx_import_done(dfx_index* idx) {
         dfx_tc_prepare_centroids(idx, idx->stream);
         DFX_CUDA(cudaStreamSynchronize(idx->stream));
     }
+    if (idx->cfg.kind == DFX_FLAT_PQ) DFX_REQUIRE(idx->codebooks.p, "import: codebooks are required");
     idx->trained = true;
     DFX_API_END
 }

@@ -435,13 +435,14 @@ static void train_subquantizers(dfx_index* idx, const float* rows, int64_t ns, i
     }
 }
 
-// the codec of the kind, trained on the first rows of the k-means sample xt f32[nt][d]
+// the codec of the kind, trained on the first rows of the k-means sample xt f32[nt][d] (FLAT_PQ: of the
+// training rows themselves)
 static void train_codec(dfx_index* idx, int64_t nt, const float* xt, int niter, cudaStream_t st) {
     const int kind = idx->cfg.kind, d = idx->cfg.d;
     const uint64_t seed = idx->train_seed;
     if (idx->has_pq()) {
         // faiss ProductQuantizer on the first min(nt, 256 * ksub) rows: their residuals (IVF_PQ,
-        // IVF_PQR), or the raw sub-vectors (FastScan is not by_residual)
+        // IVF_PQR), or the raw sub-vectors (FastScan is not by_residual; FLAT_PQ has no lists)
         const int M = idx->M, ksub = idx->ksub, dsub = idx->dsub;
         const int64_t ns = std::min<int64_t>(nt, 256ll * ksub);
         DFX_REQUIRE(ns >= ksub, "train: need at least " + std::to_string(ksub) + " vectors for PQ");
@@ -502,15 +503,21 @@ static void start_empty_lists(dfx_index* idx, cudaStream_t st) {
 }
 
 void dfx_train_impl(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) {
-    if (idx->is_flat()) {  // trained at creation, as faiss's IndexFlat and IndexScalarQuantizer(QT_fp16)
+    if (idx->flat_rows()) {  // trained at creation, as faiss's IndexFlat and IndexScalarQuantizer(QT_fp16)
         idx->trained = true;
         return;
     }
     const int d = idx->cfg.d;
     const int64_t nlist = idx->cfg.nlist;
+    const int niter = idx->kmeans_niter > 0 ? idx->kmeans_niter : 25;
+    if (!idx->is_ivf()) {  // FLAT_PQ (faiss IndexPQ::train): the codebooks alone, and an empty index
+        train_codec(idx, n, d_x, niter, st);
+        idx->n_sorted = 0;
+        idx->trained = true;
+        return;
+    }
     DFX_REQUIRE(n >= nlist, "train: need at least nlist=" + std::to_string(nlist) +
                                 " training vectors, got " + std::to_string(n));
-    const int niter = idx->kmeans_niter > 0 ? idx->kmeans_niter : 25;
 
     // faiss Clustering: at most 256 points per centroid (random subset)
     const int64_t nt = std::min<int64_t>(n, (int64_t)idx->max_points_per_centroid * nlist);
@@ -547,23 +554,28 @@ __global__ void f16_encode_kernel(const float* __restrict__ x, int64_t n, __half
     if (t < n) codes[t] = __float2half_rn(x[t]);
 }
 
-// FLAT / FLAT_SQ16: the rows (fp32, or their fp16 codes) in arrival order, and under L2 the norms of
-// the stored rows
+// FLAT / FLAT_SQ16 / FLAT_PQ: the rows (fp32, their fp16 codes, or their PQ codes) in arrival order, and
+// under FLAT / FLAT_SQ16 L2 the norms of the stored rows
 static void add_flat(dfx_index* idx, int64_t n, const float* d_x, cudaStream_t st) {
     const int d = idx->cfg.d;
     const int64_t N = idx->n_sorted;
     const size_t rb = idx->row_bytes();
+    const bool norms = idx->flat_rows() && idx->cfg.metric == DFX_METRIC_L2;
+    DFX_REQUIRE(idx->trained || idx->flat_rows(), "add: index is not trained");
     if ((size_t)(N + n) * rb > idx->payload.cap) {
         int64_t cap = std::max<int64_t>({N + n, 2 * N, idx->reserve_hint});
         idx->payload.reserve((size_t)cap * rb, (size_t)N * rb, st);
-        if (idx->cfg.metric == DFX_METRIC_L2) idx->xnorm.reserve((size_t)cap * 4, (size_t)N * 4, st);
+        if (norms) idx->xnorm.reserve((size_t)cap * 4, (size_t)N * 4, st);
     }
-    if (idx->cfg.kind == DFX_FLAT_SQ16)
+    if (idx->cfg.kind == DFX_FLAT_PQ)
+        launch_pq_encode(false, d_x, nullptr, nullptr, n, d, idx->M, idx->ksub, idx->dsub, idx->codebooks.as<float>(),
+                         idx->payload.as<uint8_t>() + N * idx->M, st);
+    else if (idx->cfg.kind == DFX_FLAT_SQ16)
         DFX_LAUNCH(f16_encode_kernel, blocks_for(n * d, 256), 256, 0, st, d_x, n * d, idx->payload.as<__half>() + N * d);
     else
         DFX_CUDA(cudaMemcpyAsync(idx->payload.as<float>() + N * d, d_x, (size_t)n * d * 4,
                                  cudaMemcpyDeviceToDevice, st));
-    if (idx->cfg.metric == DFX_METRIC_L2)
+    if (norms)
         dfx_with_flat_rows(idx, [&](auto rows) { dfx_launch_row_norms(rows + N * d, n, d, idx->xnorm.as<float>() + N, st); });
     idx->n_sorted += n;
 }
@@ -797,6 +809,17 @@ struct PqFsDec {  // IVF_PQ_FS: P[m][code_m], no centroid (the codes are of the 
     }
 };
 
+struct PqFlatDec {  // FLAT_PQ: P[m][code_m] of the row stored by id (8-bit codes of the raw vector)
+    static constexpr RowFrom kFrom = RowFrom::Id;
+    const uint8_t* codes;
+    const float* codebooks;
+    int M, dsub;
+    __device__ float operator()(int k, int64_t, int64_t pos, int64_t) const {
+        const int m = k / dsub;
+        return codebooks[((size_t)m * 256 + dfx_pq_code<8>(codes, pos, M, m)) * dsub + (k - m * dsub)];
+    }
+};
+
 // IVF_PQR: (c + P1[m][code_m]) + P2[m2][refine_code_m2], the reconstruction of faiss's IndexIVFPQR;
 // the refinement codes are stored by id
 struct PqrDec {
@@ -871,6 +894,7 @@ void dfx_reconstruct_impl(dfx_index* idx, int64_t n, const int64_t* d_ids, float
     switch (idx->cfg.kind) {
         case DFX_FLAT: return run(RowsDec<RowFrom::Id>{idx->payload.as<float>(), d});
         case DFX_FLAT_SQ16: return run(RowsDec<RowFrom::Id, __half>{idx->payload.as<__half>(), d});
+        case DFX_FLAT_PQ: return run(PqFlatDec{idx->payload.as<uint8_t>(), cb, M, dsub});
         case DFX_IVF_FLAT: return run(RowsDec<RowFrom::Pos>{idx->payload.as<float>(), d});
         case DFX_IVF_SQ16: return run(Sq16Dec{idx->payload.as<__half>(), cent, d});
         case DFX_IVF_SQ8: return run(Sq8Dec{idx->payload.as<uint8_t>(), cent, idx->sq_trained.as<float>(), d});

@@ -89,7 +89,7 @@ struct dfx_index {
     // h_len_top[p]: vectors in the p longest lists together (bounds one query's candidates at k > 1024)
     std::vector<int64_t> h_len_top;
     DevBuf ids;                         // int32[n_sorted] shard-local ids, list-sorted
-    DevBuf payload;                     // kind-specific rows, list-sorted (FLAT, FLAT_SQ16: arrival order)
+    DevBuf payload;                     // kind-specific rows, list-sorted (FLAT, FLAT_SQ16, FLAT_PQ: arrival order)
     DevBuf tvals;                       // IVF_PQ: f32[n_sorted] (IVF_PQ_FS has none)
     DevBuf xnorm;                       // FLAT / FLAT_SQ16 + L2: f32[n], |x|^2 of the stored rows
     DevBuf p_list, p_payload, p_tvals;  // pending: int32 list per row, payload rows, tvals
@@ -219,6 +219,7 @@ struct dfx_index {
             case DFX_FLAT:
             case DFX_IVF_FLAT: return (size_t)cfg.d * 4;
             case DFX_FLAT_SQ16: return (size_t)cfg.d * 2;
+            case DFX_FLAT_PQ: return (size_t)M;
             case DFX_IVF_PQ: return ksub == 16 ? (size_t)M / 2 : (size_t)M;  // 4-bit codes: two per byte
             case DFX_IVF_PQ_FS: return (size_t)M / 2;
             case DFX_IVF_PQR: return (size_t)M;  // the refine codes live outside the lists
@@ -237,13 +238,19 @@ struct dfx_index {
         h_len_top.assign(nl + 1, 0);
         for (size_t l = 0; l < nl; l++) h_len_top[l + 1] = h_len_top[l] + len[l];
     }
-    // the kinds without lists, training or probes: every stored row is scored by every search, rows are
-    // kept in arrival order, and ids are positions (FLAT: fp32 rows, FLAT_SQ16: fp16 rows)
-    bool is_flat() const { return cfg.kind == DFX_FLAT || cfg.kind == DFX_FLAT_SQ16; }
+    // the kinds without lists or probes: every stored row is scored by every search, rows are kept in
+    // arrival order, and ids are positions (FLAT: fp32 rows, FLAT_SQ16: fp16 rows, FLAT_PQ: 8-bit PQ codes)
+    bool is_flat() const { return cfg.kind == DFX_FLAT || cfg.kind == DFX_FLAT_SQ16 || cfg.kind == DFX_FLAT_PQ; }
     bool is_ivf() const { return !is_flat(); }
+    // the flat kinds that store the rows themselves (FLAT, FLAT_SQ16): trained at creation, searched by the
+    // GEMM or the tensor-core screening, with |x|^2 kept under L2.  FLAT_PQ is trained and scores codes.
+    bool flat_rows() const { return cfg.kind == DFX_FLAT || cfg.kind == DFX_FLAT_SQ16; }
     bool rflat() const { return cfg.refine_flat != 0; }
-    // the kinds with PQ codebooks (IVF_PQ / IVF_PQR: residual codes, IVF_PQ_FS: codes of the raw vectors)
-    bool has_pq() const { return cfg.kind == DFX_IVF_PQ || cfg.kind == DFX_IVF_PQ_FS || cfg.kind == DFX_IVF_PQR; }
+    // the kinds with PQ codebooks (IVF_PQ / IVF_PQR: residual codes, IVF_PQ_FS and FLAT_PQ: codes of the
+    // raw vectors)
+    bool has_pq() const {
+        return cfg.kind == DFX_IVF_PQ || cfg.kind == DFX_IVF_PQ_FS || cfg.kind == DFX_IVF_PQR || cfg.kind == DFX_FLAT_PQ;
+    }
     // the kinds whose lists hold IVF-PQ residual codes with t-values (IVF_PQR: its first stage)
     bool pq_res() const { return cfg.kind == DFX_IVF_PQ || cfg.kind == DFX_IVF_PQR; }
 };

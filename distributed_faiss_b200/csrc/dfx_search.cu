@@ -18,6 +18,11 @@
 //                         every vector's composite, MAT = true, and select_cand picks the k best)
 //   K_r  pqr_refine       IVF-PQR: re-ranks the k' = k * k_factor candidates of the IVF-PQ stage on
 //                         c + PQ1 + PQ2 (dfx_refine_dev.cuh), then K_sel picks the k best
+//   K3f/K4f/K1f pq_flat_lut / pq_flat_topk / pq_flat_values   FLAT_PQ: per-query table, then every
+//                         stored code scored per row tile with the tile's top-k fused in (pq_flat_fused:
+//                         k <= 100, or nq * k <= 16384), or the values of flat_tiles' column tiles (every
+//                         other search, range search)
+//                         (dfx_pq_flat_dev.cuh)
 //   K_rf rflat_refine     flat refinement (",RFlat"): re-ranks the k' candidates of the base kind's stage
 //                         on the stored fp32 rows (dfx_rflat_dev.cuh), then K_sel picks the k best
 //   K6   merge            cross-shard merge (float_maxheap_array_t semantics)
@@ -243,6 +248,7 @@ void dfx_launch_select_comp(const uint64_t* comp, int64_t nrows, int n, int64_t 
 #include "dfx_scan_pq_fs_dev.cuh"
 #include "dfx_refine_dev.cuh"
 #include "dfx_rflat_dev.cuh"
+#include "dfx_pq_flat_dev.cuh"
 
 // =====================================================================================
 // K4: scan_pq.  one CTA = (query, group of G consecutive probes).  lane-per-vector:
@@ -760,36 +766,123 @@ static int choose_group(int64_t nq, int nprobe) {
     return (int)G;
 }
 
-// FLAT L2: |q|^2 of every query into buf, added back to the distances the search reports; nullptr for
+// FLAT / FLAT_SQ16 L2: |q|^2 of every query into buf, added back to the distances the search reports; nullptr for
 // inner product
 static const float* query_norms(dfx_index* idx, int64_t nq, const float* d_x, DevBuf& buf, cudaStream_t st) {
-    if (idx->cfg.metric != DFX_METRIC_L2) return nullptr;
+    if (idx->cfg.metric != DFX_METRIC_L2 || !idx->flat_rows()) return nullptr;  // FLAT_PQ: the table holds all of it
     buf.reserve((size_t)nq * 4);
     dfx_launch_row_norms(d_x, nq, idx->cfg.d, buf.as<float>(), st);
     return buf.as<float>();
 }
 
-// The FFMA values of a flat shard (K1a, over its fp32 or fp16 rows), shared by search and range search: per chunk of up to 1024
-// queries, each tile of up to kFlatTile columns goes to w_vals (ld kFlatTile, 128 MB at most), and
-// tile(q0, qc, c0, nc) reads it before the next tile overwrites it.
 static constexpr int64_t kFlatTile = 32768;
+
+// ---- FLAT_PQ (dfx_pq_flat_dev.cuh)
+// f(MT, WIDE) for the instantiation that serves M: M = 8, 16, 32, 64, 96, 128 have their own code width,
+// any other M % 4 == 0 takes the generic shape of its half (M <= 64: P = 64; 64 < M <= 128: P = 128)
+template <class F>
+static void pq_flat_dispatch(int M, F&& f) {
+    if (M > 64) {
+        if (!dispatch_int(IntList<128, 96>{}, M, [&](auto MT) { f(MT, std::true_type{}); }))
+            f(std::integral_constant<int, 0>{}, std::true_type{});
+    } else if (!dispatch_int(IntList<8, 16, 32, 64>{}, M, [&](auto MT) { f(MT, std::false_type{}); })) {
+        f(std::integral_constant<int, 0>{}, std::false_type{});
+    }
+}
+
+// rows per CTA of the FLAT_PQ scoring kernels over n rows for qc queries: kFlatTile, halved (down to
+// 2048) while the grid would hold fewer than 4 CTAs per SM, so that small batches still fill the device
+static int64_t pq_flat_span(int64_t qc, int64_t n) {
+    int64_t r = kFlatTile;
+    while (r > 2048 && qc * dfx_ceil_div(n, r) < 4ll * dfx_num_sms()) r >>= 1;
+    return r;
+}
+
+// K3f: the [M][256] table of each of the qc queries xq into w_lut
+static void pq_flat_tables(dfx_index* idx, const float* xq, int64_t qc, cudaStream_t st) {
+    idx->w_lut.reserve((size_t)qc * idx->M * PQF_KSUB * 4);
+    DFX_LAUNCH(pq_flat_lut_kernel, (unsigned)qc, 256, 0, st, xq, idx->cfg.d, idx->M, idx->dsub,
+               idx->codebooks.as<float>(), idx->cfg.metric, idx->w_lut.as<float>());
+}
+
+// K1f: the values of rows c0 .. c0 + nc for the qc queries whose tables are in w_lut -> w_vals (ld kFlatTile)
+static void pq_flat_values(dfx_index* idx, int64_t qc, int64_t c0, int64_t nc, cudaStream_t st) {
+    const int M = idx->M;
+    const int64_t span = pq_flat_span(qc, nc);
+    const unsigned grid = (unsigned)(qc * dfx_ceil_div(nc, span));
+    const size_t smem = (size_t)M * PQF_KSUB * 4;
+    pq_flat_dispatch(M, [&](auto MT, auto W) {
+        auto kern = pq_flat_values_kernel<decltype(MT)::value, decltype(W)::value>;
+        DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        DFX_LAUNCH(kern, grid, PQF_THREADS, smem, st, idx->w_lut.as<float>(), idx->payload.as<uint8_t>(), c0, (int)nc,
+                   (int)span, (int)qc, M, idx->w_vals.as<float>(), kFlatTile);
+    });
+}
+
+// The values of a flat shard, shared by search and range search: per chunk of up to 1024 queries, each
+// tile of up to kFlatTile columns goes to w_vals (ld kFlatTile, 128 MB at most), and tile(q0, qc, c0, nc)
+// reads it before the next tile overwrites it.  FLAT / FLAT_SQ16: the FFMA GEMM (K1a) over the fp32 or
+// fp16 rows; FLAT_PQ: the chunk's tables (K3f), then K1f over the codes.
 template <class Tile>
 static void flat_tiles(dfx_index* idx, int64_t nq, const float* d_x, cudaStream_t st, Tile&& tile) {
     const int d = idx->cfg.d;
     const int64_t N = idx->n_sorted;
+    const bool pq = idx->cfg.kind == DFX_FLAT_PQ;
     const int64_t QC = std::min<int64_t>(nq, (32ll << 20) / kFlatTile);
     const float* xnorm = idx->xnorm.as<float>();
     idx->w_vals.reserve((size_t)QC * kFlatTile * 4);
     for (int64_t q0 = 0; q0 < nq; q0 += QC) {
         const int64_t qc = std::min(QC, nq - q0);
+        if (pq) pq_flat_tables(idx, d_x + q0 * d, qc, st);
         for (int64_t c0 = 0; c0 < N; c0 += kFlatTile) {
             const int64_t nc = std::min(kFlatTile, N - c0);
-            dfx_with_flat_rows(idx, [&](auto rows) {
-                dfx_launch_gemm_values(d_x + q0 * d, qc, rows + c0 * d, xnorm ? xnorm + c0 : nullptr, nc, d,
-                                       idx->cfg.metric, idx->w_vals.as<float>(), kFlatTile, st);
-            });
+            if (pq) {
+                pq_flat_values(idx, qc, c0, nc, st);
+            } else {
+                dfx_with_flat_rows(idx, [&](auto rows) {
+                    dfx_launch_gemm_values(d_x + q0 * d, qc, rows + c0 * d, xnorm ? xnorm + c0 : nullptr, nc, d,
+                                           idx->cfg.metric, idx->w_vals.as<float>(), kFlatTile, st);
+                });
+            }
             tile(q0, qc, c0, nc);
         }
+    }
+}
+
+// FLAT_PQ searches that take the fused per-tile top-k (K4f) instead of the values tiles (K1f).  Measured on an
+// H100 at N = 10 M (DESIGN.md section 4.14): K4f is ahead at every nq for k <= 100, and at larger k while
+// nq * k <= 16384; above that its per-warp queues of 2 next_pow2(k) composites and the chunk cap's re-reads of
+// the codes cost more than writing and re-reading the values.
+static bool pq_flat_fused(int64_t nq, int k) { return k <= 1024 && (k <= 100 || nq * k <= 16384); }
+
+// FLAT_PQ, pq_flat_fused: per query chunk the tables (K3f), K4f over every row tile into the chunk's partial
+// rows (ntiles * k composites per query), then the k best of each row.  The chunk keeps its partial rows
+// within the 128 MiB the IVF path allows its partial results (a tile grows when one query alone would
+// not fit).
+static void search_flat_pq(dfx_index* idx, int64_t nq, const float* d_x, int k, float* d_D, int64_t* d_I,
+                           cudaStream_t st) {
+    const int d = idx->cfg.d, M = idx->M;
+    const int64_t N = idx->n_sorted;
+    const int64_t part_max = (int64_t)1 << 24;
+    int64_t tile = pq_flat_span(std::min<int64_t>(nq, 1024), N);
+    while (dfx_ceil_div(N, tile) * k > part_max) tile <<= 1;
+    const int64_t ntiles = dfx_ceil_div(N, tile), ld = ntiles * k;
+    const int64_t QC = std::max<int64_t>(1, std::min<int64_t>({nq, 1024, part_max / ld}));
+    const int cap = 2 * dfx_next_pow2(k < 32 ? 32 : k);
+    const size_t smem = (size_t)M * PQF_KSUB * 4 + dfx_scan_queue_smem(PQF_THREADS, cap, false);
+    idx->w_part.reserve((size_t)QC * ld * 8);
+    uint64_t* part = idx->w_part.as<uint64_t>();
+    for (int64_t q0 = 0; q0 < nq; q0 += QC) {
+        const int64_t qc = std::min(QC, nq - q0);
+        pq_flat_tables(idx, d_x + q0 * d, qc, st);
+        pq_flat_dispatch(M, [&](auto MT, auto W) {
+            auto kern = pq_flat_topk_kernel<decltype(MT)::value, decltype(W)::value>;
+            DFX_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+            DFX_LAUNCH(kern, (unsigned)(qc * ntiles), PQF_THREADS, smem, st, idx->w_lut.as<float>(),
+                       idx->payload.as<uint8_t>(), N, tile, (int)qc, M, k, cap, part, ld);
+        });
+        ResultWriter wr{d_D + q0 * k, d_I + q0 * k, k, idx->cfg.metric, nullptr};
+        dfx_launch_select<128>(CompLoader{part, ld}, wr, qc, (int)ld, k, st);
     }
 }
 
@@ -806,8 +899,9 @@ static void search_flat(dfx_index* idx, int64_t nq, const float* d_x, int64_t k6
         dfx_launch_select<128>(ldr, wr, nq, 0, k, st);
         return;
     }
+    if (idx->cfg.kind == DFX_FLAT_PQ && pq_flat_fused(nq, k)) return search_flat_pq(idx, nq, d_x, k, d_D, d_I, st);
     const float* qnorm = query_norms(idx, nq, d_x, idx->w_dis0, st);
-    if (idx->flat_tc && idx->tc_enabled && dfx_tc_flat_covers(idx, k) &&
+    if (idx->flat_rows() && idx->flat_tc && idx->tc_enabled && dfx_tc_flat_covers(idx, k) &&
         dfx_tc_flat_table(idx, st)) {  // screening on tensor cores + exact re-rank
         const int64_t ng = dfx_ceil_div(N, 128) * 4;
         const int64_t QT = std::max<int64_t>(128, ((64ll << 20) / (ng * 4)) / 128 * 128);
@@ -1145,7 +1239,7 @@ static void begin_query(dfx_index* idx, cudaStream_t st) {
 
 void dfx_search_impl(dfx_index* idx, int64_t nq, const float* d_x, int64_t k64, float* d_D,
                      int64_t* d_I, cudaStream_t st) {
-    DFX_REQUIRE(idx->trained || idx->is_flat(), "index is not trained");
+    DFX_REQUIRE(idx->trained || idx->flat_rows(), "index is not trained");
     DFX_REQUIRE(k64 >= 1, "k must be >= 1");
     if (nq <= 0) return;
     begin_query(idx, st);
@@ -1340,7 +1434,7 @@ void dfx_range_impl(dfx_index* idx, int64_t nq, const float* d_x, float radius, 
                     cudaStream_t st) {
     // every refusal before anything is launched
     const int kind = idx->cfg.kind;
-    DFX_REQUIRE(idx->trained || idx->is_flat(), "index is not trained");
+    DFX_REQUIRE(idx->trained || idx->flat_rows(), "index is not trained");
     DFX_REQUIRE(!std::isnan(radius), "range search: the radius is NaN");
     DFX_REQUIRE(kind != DFX_IVF_PQ_FS,
                 "range search is not supported for IVF_PQ_FS (IVF-PQ FastScan) shards: their distances are "

@@ -26,12 +26,13 @@ LIB_PATH = os.path.join(_HERE, "libdfx.so")
 KIND_FLAT, KIND_IVF_FLAT, KIND_IVF_PQ, KIND_IVF_SQ16, KIND_IVF_SQ8, KIND_IVF_PQ_FS = 0, 1, 2, 3, 4, 5
 KIND_IVF_PQR = 6
 KIND_FLAT_SQ16 = 7  # faiss IndexScalarQuantizer(QT_fp16), the factory string "SQfp16"
+KIND_FLAT_PQ = 8  # faiss IndexPQ(d, M, 8), the factory strings "PQ{M}" / "PQ{M}x8"
 METRIC_INNER_PRODUCT, METRIC_L2 = 0, 1  # faiss enum values (reference index_cfg.py:44-52)
 KIND_NAMES = {KIND_FLAT: "flat", KIND_IVF_FLAT: "ivf_flat", KIND_IVF_PQ: "ivf_pq", KIND_IVF_SQ16: "ivf_sq",
               KIND_IVF_SQ8: "ivf_sq8", KIND_IVF_PQ_FS: "ivf_pq_fs", KIND_IVF_PQR: "ivf_pqr",
-              KIND_FLAT_SQ16: "flat_sq16"}
+              KIND_FLAT_SQ16: "flat_sq16", KIND_FLAT_PQ: "flat_pq"}
 # the kinds without lists: every row is scored, ids are positions, `metric` is the search metric
-FLAT_KINDS = (KIND_FLAT, KIND_FLAT_SQ16)
+FLAT_KINDS = (KIND_FLAT, KIND_FLAT_SQ16, KIND_FLAT_PQ)
 
 # every symbol include/dfx.h declares (tests check that the library exports each one)
 EXPORTED_SYMBOLS = [
@@ -70,6 +71,7 @@ STATE_ARRAYS = {
 STATE_KINDS = {
     "flat": (("metric",), ("xb",)),
     "flat_sq16": (("metric",), ("codes16",)),  # the fp16 rows in id order
+    "flat_pq": (("metric", "M", "ksub"), ("codebooks", "codes")),  # the codes in id order
     "ivf_flat": (("nlist", "metric"), ("centroids", "list_off", "ids", "vecs")),
     "ivf_pq": (("nlist", "coarse_metric", "M", "ksub"), ("centroids", "codebooks", "list_off", "ids", "codes", "tvals")),
     "ivf_sq": (("nlist", "coarse_metric"), ("centroids", "list_off", "ids", "codes16")),
@@ -192,7 +194,7 @@ class GpuIndex:
             self.quantizer = _Quantizer(self)
         self.pq_m = int(pq_m)
         self.pq_nbits = int(pq_nbits)
-        self.ksub = 1 << self.pq_nbits if self.kind in (KIND_IVF_PQ, KIND_IVF_PQ_FS, KIND_IVF_PQR) else 0
+        self.ksub = 1 << self.pq_nbits if self.kind in (KIND_IVF_PQ, KIND_IVF_PQ_FS, KIND_IVF_PQR, KIND_FLAT_PQ) else 0
         self.refine_m = int(refine_m)  # IVF-PQR: M2, the bytes of the refinement code
         # flat refinement (",RFlat"): the raw fp32 rows kept by id, k * k_factor candidates re-ranked exactly
         self.refine_flat = bool(refine_flat)
@@ -222,10 +224,10 @@ class GpuIndex:
 
     @property
     def search_metric(self):
-        """The metric of the distances search and range_search report: `metric` for FLAT, FLAT_SQ16 and
-        IVF_FLAT; L2 for the IVF codecs, whose `metric` is the coarse quantizer's (the reference never
+        """The metric of the distances search and range_search report: `metric` for FLAT, FLAT_SQ16, FLAT_PQ
+        and IVF_FLAT; L2 for the IVF codecs, whose `metric` is the coarse quantizer's (the reference never
         forwards it)."""
-        return self.metric if self.kind in (KIND_FLAT, KIND_FLAT_SQ16, KIND_IVF_FLAT) else METRIC_L2
+        return self.metric if self.kind in FLAT_KINDS + (KIND_IVF_FLAT,) else METRIC_L2
 
     @property
     def generation(self):

@@ -12,6 +12,9 @@ Tokens are case-sensitive, as in faiss:
   "SQfp16"                        -> flat_sq16 (IndexScalarQuantizer QT_fp16, the given metric: every row
                                               stored as its fp16 rounding, 2 d bytes per vector, no
                                               training; searched exactly over the decoded rows)
+  "PQ{M}" / "PQ{M}x8"             -> flat_pq   (IndexPQ, 8-bit codes of the raw vectors, the given metric:
+                                              M bytes per vector, no lists; M a multiple of 4, at most
+                                              128, that divides d)
   "IVF{n},Flat"                   -> ivf_flat  (IndexIVFFlat, the given metric)
   "IVF{n},PQ{M}" / "IVF{n},PQ{M}x8" -> ivf_pq  (IndexIVFPQ, 8-bit codes, L2 only; M a multiple of 4,
                                               at most 128, that divides d)
@@ -34,18 +37,19 @@ Tokens are case-sensitive, as in faiss:
                                               L2 only
 Everything else (OPQ / PCA prefixes, HNSW, IVF{n}_HNSW quantizers, RFlat after Flat, IVF{n},Flat or
 PQ{M}+{M2}, every Refine(...) spelling, IDMap, PQ{M}x4, PQ{M}x4fsr, a FastScan block size suffix "_{bbs}",
-SQ4 / SQ6, SQ8 or any other scalar quantizer without IVF (they need trained ranges), SQfp16 with a suffix,
-malformed n or M) raises RuntimeError.
+PQ{M}x4 / PQ{M}x4fs / PQ{M}np / PQ{M} with a suffix without IVF, SQ4 / SQ6, SQ8 or any other scalar quantizer
+without IVF (they need trained ranges), SQfp16 with a suffix, malformed n or M) raises RuntimeError.
 """
 import re
 from typing import NamedTuple
 
 METRIC_INNER_PRODUCT, METRIC_L2 = 0, 1  # faiss enum values
 
-ACCEPTED_FORMS = ("Flat", "SQfp16", "IVF{n},Flat", "IVF{n},PQ{M}", "IVF{n},PQ{M}x8", "IVF{n},PQ{M}x4fs", "IVF{n},PQ{M}+{M2}",
+ACCEPTED_FORMS = ("Flat", "SQfp16", "PQ{M}", "PQ{M}x8", "IVF{n},Flat", "IVF{n},PQ{M}", "IVF{n},PQ{M}x8", "IVF{n},PQ{M}x4fs", "IVF{n},PQ{M}+{M2}",
                   "IVF{n},SQfp16", "IVF{n},SQ8", "IVF{n},PQ{M},RFlat", "IVF{n},PQ{M}x8,RFlat", "IVF{n},PQ{M}x4fs,RFlat",
                   "IVF{n},SQfp16,RFlat", "IVF{n},SQ8,RFlat")
 
+_FLAT_PQ = re.compile(r"PQ([1-9][0-9]*)(x8)?")
 _IVF = re.compile(r"IVF([1-9][0-9]*),(Flat|PQ([1-9][0-9]*)(x8|x4fs|\+([1-9][0-9]*))?|SQfp16|SQ8)(,RFlat)?")
 # one query's fp32 PQ distance table (M x 256 x 4 bytes) must fit in one thread block's shared memory
 # (128 KB at M = 128); more would need split or fp16 tables, which are not bit-exact
@@ -53,9 +57,10 @@ _PQ_M_MAX = 128
 
 
 class FactorySpec(NamedTuple):
-    """kind: a name of engine.KIND_NAMES ("flat", "flat_sq16", "ivf_flat", "ivf_pq", "ivf_sq", "ivf_sq8",
-    "ivf_pq_fs", "ivf_pqr").  metric: flat / flat_sq16 / ivf_flat: the search metric; the codecs: the coarse quantizer's metric
-    (their search is L2).  refine_m: ivf_pqr's M2 (bytes of the refinement code), else 0.
+    """kind: a name of engine.KIND_NAMES ("flat", "flat_sq16", "flat_pq", "ivf_flat", "ivf_pq", "ivf_sq",
+    "ivf_sq8", "ivf_pq_fs", "ivf_pqr").  metric: flat / flat_sq16 / flat_pq / ivf_flat: the search metric; the IVF
+    codecs: the coarse quantizer's metric (their search is L2).  pq_m: the PQ sub-quantizers (flat_pq and the
+    IVF PQ kinds).  refine_m: ivf_pqr's M2 (bytes of the refinement code), else 0.
     refine_flat: the string ends in ",RFlat" (exact re-ranking on stored fp32 vectors)."""
     kind: str
     metric: int
@@ -81,6 +86,9 @@ def parse_factory(dim: int, factory_string: str, metric: int) -> FactorySpec:
         return FactorySpec("flat", int(metric))
     if s == "SQfp16":
         return FactorySpec("flat_sq16", int(metric))
+    m = _FLAT_PQ.fullmatch(s)
+    if m is not None:
+        return FactorySpec("flat_pq", int(metric), 0, _pq_m(factory_string, int(m.group(1)), dim))
     m = _IVF.fullmatch(s)
     # re-ranking an exact index is a no-op, and IVF-PQR has its own refinement: RFlat follows a codec only
     rflat = m is not None and m.group(6) is not None
@@ -112,12 +120,16 @@ def parse_factory(dim: int, factory_string: str, metric: int) -> FactorySpec:
                     f"at most {_PQ_M_MAX}, that divides d={dim}, got {v}")
         return FactorySpec("ivf_pqr", int(metric), nlist, M, M2)
     if codec.startswith("PQ"):
-        M = int(m.group(3))
-        if M % 4 != 0 or M > _PQ_M_MAX or dim % M != 0:
-            why = (" (one query's fp32 distance table, M x 256 x 4 bytes, must fit in one thread block's shared "
-                   "memory)") if M > _PQ_M_MAX else ""
-            raise RuntimeError(
-                f"faiss_factory {factory_string!r}: the number of PQ sub-quantizers must be a multiple of 4, "
-                f"at most {_PQ_M_MAX}, that divides d={dim}{why}")
-        return FactorySpec("ivf_pq", int(metric), nlist, M, 0, rflat)
+        return FactorySpec("ivf_pq", int(metric), nlist, _pq_m(factory_string, int(m.group(3)), dim), 0, rflat)
     return FactorySpec("ivf_sq" if codec == "SQfp16" else "ivf_sq8", int(metric), nlist, 0, 0, rflat)
+
+
+def _pq_m(factory_string: str, M: int, dim: int) -> int:
+    """M of an 8-bit PQ (IVF{n},PQ{M}[x8] and PQ{M}[x8]), or RuntimeError outside the limits"""
+    if M % 4 != 0 or M > _PQ_M_MAX or dim % M != 0:
+        why = (" (one query's fp32 distance table, M x 256 x 4 bytes, must fit in one thread block's shared "
+               "memory)") if M > _PQ_M_MAX else ""
+        raise RuntimeError(
+            f"faiss_factory {factory_string!r}: the number of PQ sub-quantizers must be a multiple of 4, "
+            f"at most {_PQ_M_MAX}, that divides d={dim}{why}")
+    return M

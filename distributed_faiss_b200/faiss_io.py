@@ -1,8 +1,9 @@
 """Reader / writer for the faiss on-disk index format, for the four index types the reference's
 builders create (reference index.py:94 IndexFlatIP, :36-40 IndexIVFFlat, :43-48 IndexIVFPQ,
 :63-68 IndexIVFScalarQuantizer(QT_fp16)), the 8-bit scalar quantizer of the factory string
-"IVF{n},SQ8" (IndexIVFScalarQuantizer(QT_8bit)) and the fp16 scalar quantizer without lists of the
-factory string "SQfp16" (IndexScalarQuantizer(QT_fp16)); the reference saves shards with
+"IVF{n},SQ8" (IndexIVFScalarQuantizer(QT_8bit)), the fp16 scalar quantizer without lists of the
+factory string "SQfp16" (IndexScalarQuantizer(QT_fp16)) and the product quantizer without lists of the
+factory string "PQ{M}" (IndexPQ, 8-bit codes); the reference saves shards with
 `faiss.write_index(self.faiss_index, index_file)` (index.py:459) and loads them with
 `faiss.read_index` (index.py:303).  SURVEY.md section 8(f) next-3.
 
@@ -14,7 +15,8 @@ term `tvals` is not part of the faiss format; the engine recomputes it on import
 STATUS: written from the layout of faiss 1.7.x `impl/index_write.cpp` / `index_read.cpp`; faiss
 itself is not available in this environment (SURVEY.md section 8c), so the format is checked for
 self-consistency only (tests/test_faiss_io.py), never against a file written by faiss.  The same
-holds for the 4-bit IndexIVFPQ codes [faiss-upstream], restated from faiss's PQEncoderGeneric.
+holds for the 4-bit IndexIVFPQ codes [faiss-upstream], restated from faiss's PQEncoderGeneric, and for
+IndexPQ ("IxPq") [faiss-upstream: index_write.cpp], never compared with a file faiss wrote.
 IndexIVFPQFastScan ("IwPf", the factory string "IVF{n},PQ{M}x4fs") is neither read nor written: its
 block-interleaved code layout could not be checked without faiss; such shards use the npz format,
 with or without a flat refinement.
@@ -26,6 +28,10 @@ Layout (little endian, no padding; `vec<T>` = u64 count + raw elements):
              f32 rangestat_arg = 0, u64 d, u64 code_size = 2 d, vec<f32> trained (empty)), vec<u8> codes
              [ntotal][2 d] (little-endian fp16 of the raw rows, in id order); other qtypes are refused
              [faiss-upstream: IndexScalarQuantizer, index_write.cpp]
+  PQ       : fourcc "IxPq", header (with the search metric), PQ (u64 d, u64 M, u64 nbits = 8, vec<f32>
+             centroids [M][256][d / M]), vec<u8> codes [ntotal][M] (in id order), i32 search_type = 0
+             (ST_PQ: exhaustive ADC), u8 encode_signs = 0, i32 polysemous_ht = 0; other nbits and search
+             types are refused [faiss-upstream: IndexPQ, index_write.cpp]
   ivf hdr  : header, u64 nlist, u64 nprobe, <quantizer: flat index of the centroids>,
              u8 direct-map type (0), vec<i64> direct map (empty)
   invlists : fourcc "ilar", u64 nlist, u64 code_size, fourcc "full" + vec<u64> sizes  (or "sprs" +
@@ -258,6 +264,17 @@ def write_index(state: Dict, path: str, nprobe: int = 1) -> None:
             _w(f, "QQ", d, 2 * d)
             _w(f, "Q", 0)  # trained: empty for fp16
             _wvec(f, c16.view(np.uint8), np.uint8)
+        elif kind == "flat_pq":
+            d, M = int(state["d"]), int(state["M"])
+            if int(state["ksub"]) != 256:
+                raise FaissFormatError(f"IndexPQ: 8-bit codes only, got ksub={int(state['ksub'])}")
+            codes = np.ascontiguousarray(state["codes"], dtype=np.uint8).reshape(-1, M)
+            f.write(b"IxPq")
+            _wheader(f, d, codes.shape[0], int(state["metric"]))
+            _w(f, "QQQ", d, M, 8)
+            _wvec(f, state["codebooks"], np.float32)
+            _wvec(f, codes, np.uint8)
+            _w(f, "iBi", 0, 0, 0)  # search_type ST_PQ, encode_signs, polysemous_ht
         elif kind == "ivf_flat":
             f.write(b"IwFl")
             _write_ivf_header(f, state, int(state["metric"]), int(state["metric"]), nprobe)
@@ -359,10 +376,27 @@ def _read_one(f: BinaryIO, cc: str) -> Tuple[Dict, int]:
         if codes.size != ntotal * 2 * d:
             raise FaissFormatError("IndexScalarQuantizer: the codes do not hold ntotal vectors")
         return {"kind": "flat_sq16", "d": d, "metric": metric, "codes16": codes.view("<u2").reshape(ntotal, d)}, 1
+    if cc == "IxPq":
+        d, ntotal, _, metric = _rheader(f)
+        pd, M, nbits = _r(f, "QQQ")
+        cb = _rvec(f, np.float32)
+        codes = _rvec(f, np.uint8)
+        search_type, _, _ = _r(f, "iBi")
+        if nbits != 8 or pd != d or M == 0 or d % M != 0 or cb.size != M * 256 * (d // M):
+            raise FaissFormatError(f"IndexPQ: only 8 bits per sub-quantizer with M dividing d is supported "
+                                   f"(nbits={nbits}, M={M}, d={pd})")
+        if search_type != 0:
+            raise FaissFormatError(f"IndexPQ: only search_type 0 (ST_PQ, exhaustive ADC) is supported, got {search_type}")
+        if metric not in (METRIC_IP, METRIC_L2):
+            raise FaissFormatError(f"IndexPQ: metric {metric} is not supported")
+        if codes.size != ntotal * M:
+            raise FaissFormatError("IndexPQ: the codes do not hold ntotal vectors")
+        return {"kind": "flat_pq", "d": d, "metric": metric, "M": int(M), "ksub": 256,
+                "codebooks": cb.reshape(M, 256, d // M), "codes": codes.reshape(ntotal, M)}, 1
     if cc not in ("IwFl", "IwPQ", "IwQR", "IwSq"):
         raise FaissFormatError(
             f"faiss index type {cc!r} is not one of the types the GPU search path serves "
-            "(IndexFlat, IndexScalarQuantizer fp16, IndexIVFFlat, IndexIVFPQ, IndexIVFPQR, "
+            "(IndexFlat, IndexScalarQuantizer fp16, IndexPQ, IndexIVFFlat, IndexIVFPQ, IndexIVFPQR, "
             "IndexIVFScalarQuantizer fp16 / 8bit)")
     d, ntotal, metric, nlist, nprobe, cent, cmetric = _read_ivf_header(f)
     st = {"d": d, "nlist": nlist, "centroids": cent}

@@ -21,7 +21,8 @@ Builders (reference index.py:93-100):
   no builder, `faiss_factory` set -> the factory string with {centroids} substituted, the cfg metric
                   for the index and its quantizer, nprobe = the faiss default 1 (index.py:385-396)
 Factory strings are parsed by factory.parse_factory ("Flat", "SQfp16" (IndexScalarQuantizer QT_fp16: the
-rows stored as fp16, searched exactly over the decoded rows), "IVF{n},Flat", "IVF{n},PQ{M}[x8]",
+rows stored as fp16, searched exactly over the decoded rows), "PQ{M}[x8]" (IndexPQ: 8-bit codes of the raw
+vectors without lists, M bytes per vector, under either metric), "IVF{n},Flat", "IVF{n},PQ{M}[x8]",
 "IVF{n},PQ{M}x4fs" (FastScan: 4-bit codes of the raw vectors, 8-bit quantized distance tables),
 "IVF{n},PQ{M}+{M2}" (IndexIVFPQR: IVF-PQ candidates re-ranked on a second, M2-byte residual code),
 "IVF{n},SQfp16", "IVF{n},SQ8", and each codec form but PQ{M}+{M2} followed by ",RFlat" (IndexRefineFlat:
@@ -64,7 +65,7 @@ def factory_spec(cfg: IndexCfg):
         # and faiss's default metric, L2, for the index and its quantizer (cfg.metric only picks the
         # k-means clustering index)
         spec = parse_factory(cfg.dim, cfg.faiss_factory, METRIC_L2)
-        if spec.kind in ("flat", "flat_sq16"):
+        if spec.kind in ("flat", "flat_sq16", "flat_pq"):
             raise RuntimeError(f"ivf_gpu needs an IVF factory string, got {cfg.faiss_factory!r} "
                                "(faiss.extract_index_ivf fails on it in the reference)")
         return spec
@@ -590,7 +591,8 @@ class Index:
         keys = [key for key in built.dims if key in built.scalars]
         stored, want = tuple(int(state[key]) for key in keys), tuple(built.dims[key] for key in keys)
         if stored != want:
-            raise RuntimeError(f"the stored {'IVF-PQR' if 'M2' in keys else 'IVF-PQ'} index has ({', '.join(keys)}) = "
+            name = "IVF-PQR" if "M2" in keys else "PQ" if built.kind == "flat_pq" else "IVF-PQ"
+            raise RuntimeError(f"the stored {name} index has ({', '.join(keys)}) = "
                                f"{stored} but the cfg builds {want}; refusing to load it")
         engine.set_state(state)
         if built.refine_flat and "k_factor" in cfg.extra:  # the caller's cfg wins over the stored value

@@ -52,12 +52,18 @@ enum {
                          8-bit PQ of M2 bytes, stored by id outside the lists.  A search runs the IVF-PQ
                          search for k' = k * k_factor candidates and re-ranks them on the reconstruction
                          c + PQ1 + PQ2 (DESIGN.md section 2).  L2 only, for the index and its quantizer */
-    DFX_FLAT_SQ16 = 7 /* faiss.IndexScalarQuantizer(d, QT_fp16, metric): the factory string "SQfp16"
+    DFX_FLAT_SQ16 = 7, /* faiss.IndexScalarQuantizer(d, QT_fp16, metric): the factory string "SQfp16"
                          (index.py:385-396).  No training.  Each row is stored as its fp16 rounding
                          (2 d bytes per vector, plus its fp32 squared norm under L2), ids are positions,
                          and a search returns bit for bit what a FLAT index of the same metric returns over
                          the decoded rows (DESIGN.md section 2).  nlist, pq_m, pq_nbits, refine_m and
                          refine_flat must be 0 */
+    DFX_FLAT_PQ = 8   /* faiss.IndexPQ(d, M, 8, metric): the factory string "PQ{M}" / "PQ{M}x8"
+                         (index.py:385-396).  Trained (one 256-centroid k-means per sub-quantizer on the
+                         raw sub-vectors), no lists: each row is stored as its M one-byte codes in arrival
+                         order, ids are positions, and a search sums each query's [M][256] distance table
+                         (L2, or the negated inner product) over the codes of every row (DESIGN.md
+                         section 2).  nlist, refine_m and refine_flat must be 0 */
 };
 
 /* faiss.METRIC_INNER_PRODUCT / faiss.METRIC_L2 (index_cfg.py:44-52) */
@@ -65,7 +71,7 @@ enum { DFX_METRIC_IP = 0, DFX_METRIC_L2 = 1 };
 
 typedef struct dfx_cfg {
     int32_t kind;     /* DFX_FLAT ... */
-    int32_t metric;   /* FLAT / IVF_FLAT / FLAT_SQ16: search metric.  IVF_PQ / IVF_SQ16 / IVF_SQ8: metric of
+    int32_t metric;   /* FLAT / IVF_FLAT / FLAT_SQ16 / FLAT_PQ: search metric.  IVF_PQ / IVF_SQ16 / IVF_SQ8: metric of
                          the coarse quantizer only -- the reference never forwards it to the
                          index, which is therefore always L2 (index.py:44-46, 64-66).
                          IVF_PQ_FS: must be L2 (an inner-product metric is refused). */
@@ -73,12 +79,14 @@ typedef struct dfx_cfg {
     int32_t pq_m;     /* IVF_PQ: sub-quantizers  (cfg.extra["code_size"], index.py:44).  8-bit codes
                          (and IVF_PQR): 4 <= M <= 128, M % 4 == 0, d % M == 0 (128: one query's fp32
                          table, M x 256 x 4 B, must fit in one thread block's shared memory).  4-bit
-                         codes and IVF_PQ_FS: 8 <= M <= 128, M % 8 == 0, d % M == 0 */
+                         codes and IVF_PQ_FS: 8 <= M <= 128, M % 8 == 0, d % M == 0.  FLAT_PQ:
+                         sub-quantizers, as for 8-bit IVF_PQ */
     int32_t pq_nbits; /* IVF_PQ: bits per code   (cfg.extra["bits_per_vector"], index.py:45): 8, or 4
                          (ksub = 16; codes stored two per byte, low nibble first, as faiss packs
-                         them).  IVF_PQ_FS: must be 4.  IVF_PQR: must be 8 */
+                         them).  IVF_PQ_FS: must be 4.  IVF_PQR and FLAT_PQ: must be 8 */
     int32_t device;   /* CUDA device ordinal this shard lives on */
-    int64_t nlist;    /* IVF_*: number of inverted lists (cfg.centroids); IVF kinds need d % 4 == 0 */
+    int64_t nlist;    /* IVF_*: number of inverted lists (cfg.centroids); IVF kinds need d % 4 == 0.
+                         Must be 0 for FLAT_SQ16 and FLAT_PQ */
     int32_t refine_m; /* IVF_PQR: sub-quantizers of the refinement PQ (M2; 8 bits each): 4 <= M2 <= 128,
                          M2 % 4 == 0, d % M2 == 0.  Must be 0 for every other kind */
     int32_t refine_flat; /* non-zero: flat refinement (faiss IndexRefineFlat, the ",RFlat" suffix of a
@@ -160,14 +168,14 @@ int dfx_search_dev(dfx_index *idx, int64_t nq, const float *d_x, int64_t k, floa
  * vector is returned when its distance D passes the radius strictly, as in faiss: D < radius for
  * L2, D > radius for inner product (a distance equal to the radius is excluded; NaN never
  * passes; +-inf radii are allowed, a NaN radius is refused).  The metric is the shard's SEARCH
- * metric: cfg.metric for FLAT, FLAT_SQ16 and IVF_FLAT, L2 for IVF_PQ, IVF_SQ16 and IVF_SQ8 (whose cfg.metric
+ * metric: cfg.metric for FLAT, FLAT_SQ16, FLAT_PQ and IVF_FLAT, L2 for IVF_PQ, IVF_SQ16 and IVF_SQ8 (whose cfg.metric
  * is the coarse quantizer's).  Every returned (D, I) pair is bit for bit the pair dfx_search at a
  * large enough k reports for that id, and each query's results are sorted best first in the total
  * order of the search (ranking value ascending, then id ascending; inner product descending).
- * Served: FLAT, FLAT_SQ16, IVF_FLAT, IVF_PQ (8- and 4-bit codes, every layout), IVF_SQ16, IVF_SQ8.  Refused
+ * Served: FLAT, FLAT_SQ16, FLAT_PQ, IVF_FLAT, IVF_PQ (8- and 4-bit codes, every layout), IVF_SQ16, IVF_SQ8.  Refused
  * before anything is launched: IVF_PQ_FS (its distances are dequantized after the selection),
  * IVF_PQR and refine_flat (a radius over two stages of distances is not defined), an untrained IVF
- * index.  Limits: an IVF query chunk's candidates obey the rule of k > 1024 (the nprobe longest
+ * or FLAT_PQ index.  Limits: an IVF query chunk's candidates obey the rule of k > 1024 (the nprobe longest
  * lists together at most 2^24 vectors), and one call returns at most 2^27 results; a call that
  * would return more raises once its counts are known, returns nothing, and leaves the shard
  * searchable (split the batch).
@@ -176,9 +184,9 @@ int dfx_search_dev(dfx_index *idx, int64_t nq, const float *d_x, int64_t k, floa
  * float32 and I int64.  The results stay in index-owned workspace until the next search or range
  * search of the index, and can be fetched any number of times until then.
  * dfx_range_search_dev: device queries and device d_lims, *total = lims[nq] on the host; it reads
- * counts back, synchronising once per query chunk (FLAT: per chunk and 32768-row tile) and once at
- * the end, so it cannot be captured in a CUDA graph.  dfx_range_fetch_dev maps the results into
- * device d_D / d_I on the stream. */
+ * counts back, synchronising once per query chunk (FLAT, FLAT_SQ16, FLAT_PQ: per chunk and 32768-row
+ * tile) and once at the end, so it cannot be captured in a CUDA graph.  dfx_range_fetch_dev maps the
+ * results into device d_D / d_I on the stream. */
 int dfx_range_search(dfx_index *idx, int64_t nq, const float *x, float radius, int64_t *lims);
 int dfx_range_fetch(dfx_index *idx, float *D, int64_t *I);
 int dfx_range_search_dev(dfx_index *idx, int64_t nq, const float *d_x, float radius, int64_t *d_lims,
@@ -259,6 +267,8 @@ int dfx_map_ids_dev(int64_t n, const int64_t *d_ids, const int64_t *d_table, int
  *   one 4-bit code per byte as for IVF_PQ; no "tvals", since the codes are not residuals)
  *   "vecs" f32[ntotal,d] (IVF_FLAT)   "codes16" u16[ntotal,d]   "xb" f32[ntotal,d] (FLAT)
  *   (FLAT_SQ16: "codes16" alone, the fp16 rows in id order; like "xb" its import sets ntotal)
+ *   (FLAT_PQ: "codebooks" f32[M,256,dsub], then "codes" u8[ntotal,M] in id order, whose import sets
+ *   ntotal)
  *   "sq_trained" f32[2,d] (IVF_SQ8: vmin, then vdiff -- faiss's ScalarQuantizer::trained)
  *   "codes8" u8[ntotal,d] (IVF_SQ8)
  *   (IVF_PQR: the IVF_PQ arrays with 8-bit codes, plus "refine_codebooks" f32[M2,256,d/M2] and
