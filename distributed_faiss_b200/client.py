@@ -286,7 +286,8 @@ class IndexClient:
             out_scores.append(np.array([s for s, _ in kept], dtype=np.float32).reshape(-1, 1))
         return out_scores, out_meta
 
-    def range_search(self, query: np.ndarray, radius: float, index_id: str) -> Tuple[np.ndarray, np.ndarray, List]:
+    def range_search(self, query: np.ndarray, radius: float, index_id: str, return_embeddings: bool = False
+                     ) -> Tuple:
         """Every indexed vector within `radius` of each query, faiss's `range_search` over all shards:
         `(lims int64[nq + 1], scores float32[lims[-1]], meta)`, query i's results at lims[i]:lims[i + 1]
         and `meta` a flat list of their metadata.  A shard keeps what its `search` would score with a
@@ -295,16 +296,20 @@ class IndexClient:
         `metric` says).  Each query's results are merged best first; among equal scores the earlier
         shard, then the shard's own order, comes first.  The scores are faiss's values: unlike
         `search`, which negates them for metric "dot" as the reference does, they are never negated.
-        Always over the sockets, also when a search plane is attached."""
-        results = self._all(lambda s: s.range_search(index_id, query, radius))
+        With `return_embeddings` a fourth item `embs` float32[lims[-1], d] holds the hits' vectors in
+        result order, decoded by their shards (the stored fp32 row of a `,RFlat` shard).
+        Over the search plane when one is attached (one collective; the merge runs on the GPU and a
+        call returns at most 2^27 hits over all shards), else over the sockets; both return the same."""
+        if self.plane is not None:
+            return self._range_search_plane(query, radius, index_id, return_embeddings)
+        results = self._all(lambda s: s.range_search(index_id, query, radius, return_embeddings))
         metrics = {int(r[3]) for r in results}
         if len(metrics) > 1:
-            raise RuntimeError(f"range_search: the shards of index {index_id!r} report different search metrics "
-                               f"{sorted(metrics)}; their distances cannot be merged")
+            raise RuntimeError(self._range_metrics_differ(index_id, metrics))
         maximize = metrics == {0}  # faiss METRIC_INNER_PRODUCT
         nq = int(np.asarray(query).shape[0])
         qs, scores, meta = [], [], []
-        for lims, D, m, _ in results:
+        for lims, D, m, *_ in results:
             qs.append(np.repeat(np.arange(nq, dtype=np.int64), np.diff(lims)))
             scores.append(np.asarray(D, dtype=np.float32))
             meta.extend(m)
@@ -315,7 +320,17 @@ class IndexClient:
         order = np.lexsort((-D if maximize else D, q))
         lims = np.zeros(nq + 1, dtype=np.int64)
         np.cumsum(np.bincount(q, minlength=nq), out=lims[1:])
-        return lims, D[order], [meta[i] for i in order.tolist()]
+        out = (lims, D[order], [meta[i] for i in order.tolist()])
+        if not return_embeddings:
+            return out
+        d = int(np.asarray(query).shape[1])
+        embs = np.concatenate([np.asarray(r[4], dtype=np.float32).reshape(-1, d) for r in results])
+        return out + (embs[order],)
+
+    @staticmethod
+    def _range_metrics_differ(index_id, metrics):
+        return (f"range_search: the shards of index {index_id!r} report different search metrics "
+                f"{sorted(metrics)}; their distances cannot be merged")
 
     # ---- NCCL data plane (spmd.SearchPlane): same contracts, one collective instead of S RPCs
     def _get_meta_kind(self, index_id: str) -> str:
@@ -376,6 +391,26 @@ class IndexClient:
         # the reference returns list[nq][k] of per-winner vectors (client.py:299-307)
         picked = [[embs[q, j] if I[q, j] >= 0 else None for j in range(I.shape[1])] for q in range(I.shape[0])]
         return D, meta, picked
+
+    def _range_search_plane(self, query, radius, index_id, return_embeddings):
+        from . import spmd
+
+        for attempt in (0, 1):
+            int_meta = self._get_meta_kind(index_id) == "int"
+            try:
+                lims, D, P, embs = self.plane.range_search(index_id, query, radius, int_meta=int_meta,
+                                                           return_embeddings=return_embeddings)
+                break
+            except spmd.MetaKindChanged:
+                self._meta_kind.pop(index_id, None)
+                if attempt:
+                    raise
+            except spmd.RangeMetricsDiffer as e:
+                raise RuntimeError(self._range_metrics_differ(index_id, e.metrics))
+            except spmd.PlaneError as e:
+                raise rpc.ServerException(str(e))
+        meta = P.tolist() if int_meta else self._exchange_ids_to_meta(index_id, P)
+        return (lims, D, meta, embs) if return_embeddings else (lims, D, meta)
 
     def _search_with_filter_plane(self, query, top_k, index_id, filter_pos, filter_value):
         from . import spmd

@@ -564,6 +564,14 @@ int dfx_merge_packed_dev(int64_t R, int64_t S_loc, int64_t nq, int64_t k, const 
                           (cudaStream_t)stream);
     DFX_API_END
 }
+int dfx_range_merge_dev(int64_t S, int64_t nq, const int64_t* d_lims, const float* d_D, const int64_t* d_P,
+                        int64_t total, int maximize, int64_t* d_out_lims, float* d_outD, int64_t* d_outP,
+                        int64_t* d_order, void* stream) {
+    DFX_API_BEGIN
+    dfx_range_merge_impl(S, nq, d_lims, d_D, d_P, total, maximize, d_out_lims, d_outD, d_outP, d_order,
+                         (cudaStream_t)stream);
+    DFX_API_END
+}
 int dfx_encode_ids_dev(int64_t n, const int64_t* d_ids, int64_t shard_tag, const int32_t* d_col,
                        int32_t drop_code, int64_t* d_out, void* stream) {
     DFX_API_BEGIN

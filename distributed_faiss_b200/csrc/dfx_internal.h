@@ -283,6 +283,9 @@ void dfx_merge_impl(int64_t S, int64_t nq, int64_t k, const float* d_D, const in
 void dfx_merge_packed_impl(int64_t R, int64_t S_loc, int64_t nq, int64_t k, const void* d_packed,
                            int64_t rank_stride, int64_t off_I, int negate, float* d_outD,
                            int64_t* d_outI, cudaStream_t st);
+void dfx_range_merge_impl(int64_t S, int64_t nq, const int64_t* d_lims, const float* d_D, const int64_t* d_P,
+                          int64_t total, int maximize, int64_t* d_out_lims, float* d_outD, int64_t* d_outP,
+                          int64_t* d_order, cudaStream_t st);
 void dfx_encode_ids_impl(int64_t n, const int64_t* d_ids, int64_t tag, const int32_t* d_col,
                          int32_t drop_code, int64_t* d_out, cudaStream_t st);
 void dfx_filter_compact_impl(int64_t nq, int64_t kin, int64_t kout, const float* d_D, const int64_t* d_I,

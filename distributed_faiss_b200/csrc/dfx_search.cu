@@ -1514,6 +1514,103 @@ void dfx_range_fetch_impl(dfx_index* idx, float* d_D, int64_t* d_I, cudaStream_t
                idx->r_qnorm ? idx->r_qn.as<float>() : nullptr, d_D, d_I);
 }
 
+// ---- the cross-shard range merge (dfx_range_merge_dev).  S shards' range results, concatenated
+// shard-major: shard s's query q holds entries base[s] + lims[s][q] .. base[s] + lims[s][q + 1] - 1,
+// with base[s] = the totals lims[s'][nq] of the shards s' < s.  The merged order is the one of a stable
+// sort by (query, score) over that concatenation, scores compared as floats (L2 ascending, IP
+// descending): per query best first, equal scores by shard, then by the shard's own order.  Each run
+// (one shard, one query) is already sorted that way, so every entry's output slot follows from ranks
+// alone (co-ranking): the query's merged offset, the entry's rank r in its own run, and per other shard
+// s' the entries of run (s', q) that precede it -- not worse than it when s' < s, strictly better when
+// s' > s -- found by a binary search.  No atomics, no sort, deterministic.
+// K_rml: one CTA; out_lims = exclusive scan over the queries of the summed run lengths
+__global__ void __launch_bounds__(256)
+range_merge_lims_kernel(int64_t S, int64_t nq, const int64_t* __restrict__ lims, int64_t* __restrict__ out_lims) {
+    __shared__ long long s[256];
+    long long carry = 0;
+    for (int64_t q0 = 0; q0 < nq; q0 += 256) {
+        const int64_t q = q0 + threadIdx.x;
+        long long c = 0;
+        if (q < nq)
+            for (int64_t sh = 0; sh < S; sh++) c += lims[sh * (nq + 1) + q + 1] - lims[sh * (nq + 1) + q];
+        s[threadIdx.x] = c;
+        __syncthreads();
+        for (int off = 1; off < 256; off <<= 1) {  // inclusive scan, Hillis-Steele
+            const long long o = threadIdx.x >= off ? s[threadIdx.x - off] : 0;
+            __syncthreads();
+            s[threadIdx.x] += o;
+            __syncthreads();
+        }
+        if (q < nq) out_lims[q] = carry + s[threadIdx.x] - c;
+        carry += s[255];
+        __syncthreads();
+    }
+    if (threadIdx.x == 0) out_lims[nq] = carry;
+}
+
+// entries of the sorted run x[0, n) that precede a value v: not worse (ties included) or strictly better
+__device__ __forceinline__ int64_t range_merge_rank(const float* __restrict__ x, int64_t n, float v, bool maximize,
+                                                    bool ties) {
+    int64_t lo = 0, hi = n;
+    while (lo < hi) {
+        const int64_t mid = lo + ((hi - lo) >> 1);
+        const float e = x[mid];
+        const bool before = maximize ? (ties ? e >= v : e > v) : (ties ? e <= v : e < v);
+        if (before) lo = mid + 1;
+        else hi = mid;
+    }
+    return lo;
+}
+
+// K_rmm: one thread per entry i of the concatenation: its slot, then D, the payload and order[slot] = i
+__global__ void __launch_bounds__(256)
+range_merge_kernel(int64_t S, int64_t nq, int64_t T, const int64_t* __restrict__ lims, const float* __restrict__ D,
+                   const int64_t* __restrict__ P, int maximize, const int64_t* __restrict__ out_lims,
+                   float* __restrict__ outD, int64_t* __restrict__ outP, int64_t* __restrict__ order) {
+    const int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= T) return;
+    // the shard: the last s whose base is <= i
+    int64_t s = 0, base = 0;
+    for (;;) {
+        const int64_t tot = lims[s * (nq + 1) + nq];
+        if (i < base + tot || s == S - 1) break;
+        base += tot;
+        s++;
+    }
+    // the query: the last q with lims[s][q] <= i - base
+    const int64_t* L = lims + s * (nq + 1);
+    const int64_t loc = i - base;
+    int64_t lo = 0, hi = nq;  // lims[s][lo] <= loc < lims[s][hi]
+    while (hi - lo > 1) {
+        const int64_t mid = (lo + hi) >> 1;
+        if (L[mid] <= loc) lo = mid;
+        else hi = mid;
+    }
+    const int64_t q = lo;
+    const float v = D[i];
+    int64_t slot = out_lims[q] + (loc - L[q]);
+    int64_t b2 = 0;
+    for (int64_t s2 = 0; s2 < S; s2++) {
+        const int64_t* L2 = lims + s2 * (nq + 1);
+        if (s2 != s) slot += range_merge_rank(D + b2 + L2[q], L2[q + 1] - L2[q], v, maximize != 0, s2 < s);
+        b2 += L2[nq];
+    }
+    outD[slot] = v;
+    outP[slot] = P[i];
+    order[slot] = i;
+}
+
+void dfx_range_merge_impl(int64_t S, int64_t nq, const int64_t* d_lims, const float* d_D, const int64_t* d_P,
+                          int64_t total, int maximize, int64_t* d_out_lims, float* d_outD, int64_t* d_outP,
+                          int64_t* d_order, cudaStream_t st) {
+    DFX_REQUIRE(S >= 1 && nq >= 0 && total >= 0, "range merge: bad S / nq / total");
+    DFX_REQUIRE(total <= (((int64_t)1 << 31) - 1) * 256, "range merge: too many entries");  // gridDim.x <= 2^31 - 1
+    DFX_LAUNCH(range_merge_lims_kernel, 1, 256, 0, st, S, nq, d_lims, d_out_lims);
+    if (total == 0 || nq == 0) return;
+    DFX_LAUNCH(range_merge_kernel, (unsigned)dfx_ceil_div(total, 256), 256, 0, st, S, nq, total, d_lims, d_D, d_P,
+               maximize, d_out_lims, d_outD, d_outP, d_order);
+}
+
 // =====================================================================================
 // K7a: fused nearest-centroid assignment (build path).  Same FFMA tile as K1a, but the
 // epilogue reduces each row's tile to one composite (value, column) and folds it into

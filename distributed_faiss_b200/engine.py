@@ -43,7 +43,7 @@ EXPORTED_SYMBOLS = [
     "dfx_reconstruct_dev", "dfx_map_ids_dev", "dfx_get_array", "dfx_set_array", "dfx_import_done",
     "dfx_last_stats", "dfx_profile_enable", "dfx_profile_read", "dfx_launch_count", "dfx_synth_init", "dfx_synth_rows_dev", "dfx_free",
     "dfx_last_error", "dfx_version", "dfx_debug_il_byte", "dfx_debug_tc_screen",
-    "dfx_range_search", "dfx_range_fetch", "dfx_range_search_dev", "dfx_range_fetch_dev",
+    "dfx_range_search", "dfx_range_fetch", "dfx_range_search_dev", "dfx_range_fetch_dev", "dfx_range_merge_dev",
 ]
 
 
@@ -318,6 +318,26 @@ class GpuIndex:
         _check(lib().dfx_range_fetch(self._h, _np_ptr(D), _np_ptr(I)))
         return lims, D, I
 
+    def range_search_dev(self, x_t, radius):
+        """`range_search` on device: x_t a torch float32 CUDA tensor [nq, d]; returns torch CUDA tensors
+        (lims int64[nq + 1], D float32[T], I int64[T]), exactly what `range_search` returns.  Runs on
+        torch's current stream, but synchronises with it once per query chunk (FLAT kinds: per chunk and
+        column tile) to read counts back, so it cannot be captured in a CUDA graph."""
+        import torch
+
+        assert x_t.is_cuda and x_t.dtype == torch.float32 and x_t.is_contiguous()
+        assert x_t.ndim == 2 and x_t.shape[1] == self.d, f"query must be [nq, {self.d}] float32"
+        nq = x_t.shape[0]
+        st = C.c_void_p(torch.cuda.current_stream(x_t.device).cuda_stream)
+        lims_t = torch.empty((nq + 1,), dtype=torch.int64, device=x_t.device)
+        total = C.c_int64(0)
+        _check(lib().dfx_range_search_dev(self._h, C.c_int64(nq), C.c_void_p(x_t.data_ptr()), C.c_float(float(radius)),
+                                          C.c_void_p(lims_t.data_ptr()), C.byref(total), st))
+        D_t = torch.empty((total.value,), dtype=torch.float32, device=x_t.device)
+        I_t = torch.empty((total.value,), dtype=torch.int64, device=x_t.device)
+        _check(lib().dfx_range_fetch_dev(self._h, C.c_void_p(D_t.data_ptr()), C.c_void_p(I_t.data_ptr()), st))
+        return lims_t, D_t, I_t
+
     def reconstruct_rows(self, ids):
         ids = np.ascontiguousarray(ids, dtype=np.int64).reshape(-1)
         out = np.empty((ids.shape[0], self.d), dtype=np.float32)
@@ -441,6 +461,31 @@ def merge_packed_dev(packed_t, R, S_loc, nq, k, rank_stride, off_I, negate=False
                                       C.c_int(1 if negate else 0), C.c_void_p(outD.data_ptr()),
                                       C.c_void_p(outI.data_ptr()), C.c_void_p(st)))
     return outD, outI
+
+
+def range_merge_dev(lims_t, D_t, P_t, maximize):
+    """The cross-shard range merge (include/dfx.h dfx_range_merge_dev) on torch CUDA tensors: lims_t
+    int64[S, nq + 1] (each shard's own offsets), D_t float32[T] and P_t int64[T] concatenated shard-major.
+    Returns (lims int64[nq + 1], D float32[T], P int64[T], order int64[T]); order[j] is the input entry of
+    output slot j.  `maximize`: inner-product scores (best = largest)."""
+    import torch
+
+    S, nq1 = lims_t.shape
+    T = D_t.numel()
+    assert lims_t.dtype == torch.int64 and D_t.dtype == torch.float32 and P_t.dtype == torch.int64
+    assert lims_t.is_contiguous() and D_t.is_contiguous() and P_t.is_contiguous() and P_t.numel() == T
+    dev = D_t.device
+    out_lims = torch.empty((nq1,), dtype=torch.int64, device=dev)
+    outD = torch.empty((T,), dtype=torch.float32, device=dev)
+    outP = torch.empty((T,), dtype=torch.int64, device=dev)
+    order = torch.empty((T,), dtype=torch.int64, device=dev)
+    st = torch.cuda.current_stream(dev).cuda_stream
+    _check(lib().dfx_range_merge_dev(C.c_int64(S), C.c_int64(nq1 - 1), C.c_void_p(lims_t.data_ptr()),
+                                     C.c_void_p(D_t.data_ptr()), C.c_void_p(P_t.data_ptr()), C.c_int64(T),
+                                     C.c_int(1 if maximize else 0), C.c_void_p(out_lims.data_ptr()),
+                                     C.c_void_p(outD.data_ptr()), C.c_void_p(outP.data_ptr()),
+                                     C.c_void_p(order.data_ptr()), C.c_void_p(st)))
+    return out_lims, outD, outP, order
 
 
 EXCHANGE_LOCAL_BITS = 40            # exchange id = (shard tag << 40) | shard-local id

@@ -312,14 +312,20 @@ class Index:
                 embs = None
         return scores, self._ids_to_meta(ids), embs
 
-    def range_search(self, query_batch: np.ndarray, radius: float) -> Tuple[np.ndarray, np.ndarray, List[object]]:
+    def range_search(self, query_batch: np.ndarray, radius: float, return_embeddings: bool = False) -> Tuple:
         """faiss's range search on this shard: `(lims int64[nq + 1], scores float32[lims[-1]], meta)`,
         query i's results at lims[i]:lims[i + 1], best first; `meta` is a flat list of lims[-1]
-        metadata entries.  L2 keeps scores < radius, inner product scores > radius (search_metric())."""
+        metadata entries.  L2 keeps scores < radius, inner product scores > radius (search_metric()).
+        With `return_embeddings` a fourth item holds the hits' decoded vectors, float32[lims[-1], d]
+        (`reconstruct_rows`, as search_and_reconstruct decodes)."""
         with self.index_lock:
             if self.state != IndexState.TRAINED:
                 raise RuntimeError(f"Server index is not trained. state: {self.state}")
             lims, scores, ids = self.faiss_index.range_search(query_batch, radius)
+            if return_embeddings:
+                embs = np.asarray(self.faiss_index.reconstruct_rows(ids)).reshape(len(ids), self.faiss_index.d)
+        if return_embeddings:
+            return lims, scores, self._ids_to_meta(ids), embs
         return lims, scores, self._ids_to_meta(ids)
 
     def search_metric(self) -> int:

@@ -158,11 +158,13 @@ class IndexServer:
     def search(self, index_id: str, query_batch: np.ndarray, top_k: int, return_embeddings: bool) -> Tuple:
         return self._get_index(index_id).search(query_batch, top_k=top_k, return_embeddings=return_embeddings)
 
-    def range_search(self, index_id: str, query_batch: np.ndarray, radius: float) -> Tuple:
-        """(lims, scores, meta, search metric) of this shard; IndexClient.range_search merges them"""
+    def range_search(self, index_id: str, query_batch: np.ndarray, radius: float,
+                     return_embeddings: bool = False) -> Tuple:
+        """(lims, scores, meta, search metric) of this shard, and with `return_embeddings` the hits'
+        vectors float32[lims[-1], d] as a fifth item; IndexClient.range_search merges them"""
         index = self._get_index(index_id)
-        lims, scores, meta = index.range_search(query_batch, radius)
-        return lims, scores, meta, index.search_metric()
+        lims, scores, meta, *embs = index.range_search(query_batch, radius, return_embeddings)
+        return (lims, scores, meta, index.search_metric(), *embs)
 
     def search_ids(self, index_id: str, query_batch: np.ndarray, top_k: int):
         return self._get_index(index_id).search_ids(query_batch, top_k)

@@ -89,6 +89,20 @@ class CudaBackend:
     def reconstruct_owned(self, shard, I_t, R_t, tag):
         shard.reconstruct_dev(I_t, R_t, tag)
 
+    def range_local(self, shard, x_t, radius, embs):
+        """(lims [nq + 1], D [T], shard-local ids [T], their decoded rows [T, d] or None)"""
+        lims, D, I = shard.range_search_dev(x_t, radius)
+        R = None
+        if embs:
+            R = torch.empty((I.numel(), x_t.shape[1]), dtype=torch.float32, device=x_t.device)
+            shard.reconstruct_dev(I, R)
+        return lims, D, I, R
+
+    def range_merge(self, lims_t, D_t, P_t, maximize):
+        from . import engine
+
+        return engine.range_merge_dev(lims_t, D_t, P_t, maximize)
+
     # kept for callers of the round-1 interface
     def merge(self, D_t, I_t, negate):
         from . import engine
@@ -373,11 +387,40 @@ class ShardGroup:
 # =================================================================================================
 # IndexClient.search over the collective
 # =================================================================================================
-OP_STOP, OP_SEARCH, OP_TIMER_START, OP_TIMER_STOP = 0, 1, 2, 3
+OP_STOP, OP_SEARCH, OP_TIMER_START, OP_TIMER_STOP, OP_RANGE = 0, 1, 2, 3, 4
 F_MAXIMIZE, F_EMBS, F_INT_META, F_FILTER, F_HAVE_QUERY = 1, 2, 4, 8, 16
 HDR_WORDS = 32                      # int64 words: 8 scalars + 128 bytes of index id + spare
 HDR_RING = 64                       # pinned header buffers in flight (see SearchPlane.__init__)
 ST_OK, ST_NOT_TRAINED, ST_META_KIND, ST_NO_INDEX, ST_ERROR = 0, 1, 2, 3, 4
+# range search only, decided by every rank alike from the gathered per-shard totals and metrics
+ST_RANGE_METRICS, ST_RANGE_LIMIT = 5, 6
+# hits one range_search call may return over ALL shards: the engine's per-shard limit (dfx_range_search).
+# Every rank also needs device memory for the exchange and the merge (range_need_bytes); a call whose need
+# exceeds what some rank has free is refused before anything is allocated, like one beyond this bound.
+RANGE_MAX_HITS = 1 << 27
+RANGE_MSG_BYTES = 256               # the first error of a rank travels in the small all-gather
+RANGE_MEM_SLACK = 256 << 20         # allocator rounding and the merge's small buffers
+
+
+def range_layout(S_loc, nq, d, embs, T_max):
+    """Byte offsets of one rank's packed block of the range exchange: per-shard lims i64[S_loc][nq + 1] at
+    0, D f32[T_max] at off_D, payloads i64[T_max] at off_P, rows f32[T_max][d] at off_E; every part and the
+    block itself (stride) 8-byte aligned, so each rank's block can be viewed as int64 wherever it starts."""
+    off_D = 8 * S_loc * (nq + 1)
+    off_P = off_D + _align8(4 * T_max)
+    off_E = off_P + 8 * T_max
+    stride = _align8(off_E + (4 * T_max * d if embs else 0))
+    return off_D, off_P, off_E, stride
+
+
+def range_need_bytes(world, S_loc, nq, d, embs, totals):
+    """Device memory one rank may need after the small all-gather: the gathered blocks (world > 1), and on
+    rank 0 the concatenated inputs, the merge's outputs and the reordered rows.  totals: hits per rank and
+    local shard.  The same for every rank, so every rank reaches the same decision."""
+    T = int(totals.sum())
+    exchange = world * range_layout(S_loc, nq, d, embs, int(totals.sum(axis=1).max()))[3] if world > 1 else 0
+    rows = 4 * d if embs else 0
+    return exchange + 8 * world * S_loc * (nq + 1) + T * (12 + rows) + T * 20 + T * rows + 8 * (nq + 1)
 
 _plane_lock = threading.Lock()
 _current_plane = None
@@ -390,6 +433,37 @@ def current_plane():
 
 class PlaneError(RuntimeError):
     pass
+
+
+def range_decide(ai, S_loc, nq, d, embs):
+    """Whether a range search goes on after its small all-gather, and if not the status and message.
+    ai: the gathered info, one row per rank: status, message length, usable device bytes, hits per local
+    shard, search metric per local shard, message bytes.  Every rank decides alike from the same rows."""
+    world = ai.shape[0]
+    st = int(ai[:, 0].max())
+    message = ""
+    for r in range(world):
+        if ai[r, 1] > 0:
+            message = ai[r, 3 + 2 * S_loc:].view(np.uint8)[:ai[r, 1]].tobytes().decode("utf-8", "replace")
+            break
+    if st != ST_OK:
+        return st, message
+    totals = ai[:, 3:3 + S_loc]
+    smetrics = sorted(set(ai[:, 3 + S_loc:3 + 2 * S_loc].reshape(-1).tolist()))
+    if len(smetrics) > 1:
+        return ST_RANGE_METRICS, smetrics
+    T = int(totals.sum())
+    if T > RANGE_MAX_HITS:
+        return ST_RANGE_LIMIT, (f"range_search: this call's results ({T} over all shards) exceed "
+                                f"{RANGE_MAX_HITS} (2^27); split the query batch")
+    need = range_need_bytes(world, S_loc, nq, d, embs, totals) + RANGE_MEM_SLACK
+    r = int(np.argmin(ai[:, 2]))
+    if need > int(ai[r, 2]):
+        return ST_RANGE_LIMIT, (f"range_search: this call's {T} results need {need / 2**30:.2f} GiB of device "
+                                f"memory per rank for the exchange and the merge, more than the "
+                                f"{int(ai[r, 2]) / 2**30:.2f} GiB free on plane rank {r}; split the query batch"
+                                + (" or leave out the embeddings" if embs else ""))
+    return ST_OK, ""
 
 
 class SearchPlane:
@@ -507,6 +581,8 @@ class SearchPlane:
                     self._timer_stop()
                 elif op == OP_SEARCH:
                     self._run_search(h, index_id, blob, None)
+                elif op == OP_RANGE:
+                    self._run_range(h, index_id, None)
 
     def stop(self):
         """End the plane: ranks != 0 leave `serve_forever`, and the plane stops being this process's
@@ -611,7 +687,172 @@ class SearchPlane:
             for ix in locked:
                 ix.index_lock.release()
 
+    def _run_range(self, h, index_id, x_t):
+        """One range search, every rank: each local shard under its index_lock answers (range_local),
+        its ids become integer metadata (map_ids) or exchange ids (encode_ids), and with embeddings its
+        hits are decoded right away.  One small all-gather carries each rank's status, per-shard totals and
+        search metrics; every rank then decides alike whether the call goes on.  If it does, one all-gather
+        of the packed blocks (per-shard lims | D | payload | rows, padded to the largest rank's) brings
+        every shard's results to rank 0, which merges them (range_merge).  Failures become status words,
+        never an exception on one rank.  The small all-gather also carries each rank's usable device memory,
+        so a call whose exchange and merge would not fit is refused alike by every rank (range_decide)
+        before anything is allocated.  Returns (status, message, lims, D, P, embs) on rank 0."""
+        import logging
+
+        log = logging.getLogger("distributed_faiss_b200")
+        be = self.backend
+        nq, flags, d = int(h[1]), int(h[3]), int(h[4])
+        radius = float(np.int64(h[5]).view(np.float64))
+        dev = self.device
+        if x_t is None:
+            x_t = torch.empty((nq, d), dtype=torch.float32, device=dev)
+        if self.world > 1:
+            dist.broadcast(x_t, src=0, group=self.group)
+        embs = bool(flags & F_EMBS)
+        int_meta = bool(flags & F_INT_META)
+        indexes = [s.indexes.get(index_id) for s in self.servers]
+        status = ST_OK if all(ix is not None for ix in indexes) else ST_NO_INDEX
+        errors = []
+        tables = None
+        if int_meta:  # before any index_lock (they take buffer_lock)
+            try:
+                tables = [ix.meta_int_table(dev) if ix is not None else None for ix in indexes]
+                if any(t is None and ix is not None for t, ix in zip(tables, indexes)):
+                    status = max(status, ST_META_KIND)
+            except Exception as e:
+                log.exception("plane rank %d: metadata tables failed", self.rank)
+                errors.append(str(e))
+                status = ST_ERROR
+        S_loc = self.S_loc
+        parts, metrics = [], []
+        locked = []
+        try:
+            for j, ix in enumerate(indexes):
+                part, metric = None, -1
+                if ix is not None:
+                    ix.index_lock.acquire()   # one search at a time per shard (reference index.py:246-252)
+                    locked.append(ix)
+                    if not ix.is_searchable():
+                        status = max(status, ST_NOT_TRAINED)
+                    elif status == ST_OK:
+                        try:
+                            lims, D, I, R = be.range_local(ix.faiss_index, x_t, radius, embs)
+                            P = torch.empty_like(I)
+                            if int_meta:
+                                be.map_ids(I, tables[j], P)
+                            else:
+                                be.encode_ids(I, self.rank * S_loc + j, P)
+                            part, metric = (lims, D, P, R), int(ix.faiss_index.search_metric)
+                        except Exception as e:   # the engine's refusals and limits, never on one rank only
+                            log.error("range search failed: %s", e)
+                            errors.append(str(e))
+                            status = ST_ERROR
+                if part is None:
+                    part = (torch.zeros((nq + 1,), dtype=torch.int64, device=dev),
+                            torch.empty((0,), dtype=torch.float32, device=dev),
+                            torch.empty((0,), dtype=torch.int64, device=dev),
+                            torch.empty((0, d), dtype=torch.float32, device=dev) if embs else None)
+                parts.append(part)
+                metrics.append(metric)
+            msg = errors[0].encode("utf-8", "replace")[:RANGE_MSG_BYTES] if errors else b""
+            info = np.zeros(3 + 2 * S_loc + RANGE_MSG_BYTES // 8, dtype=np.int64)
+            info[0], info[1], info[2] = status, len(msg), self._usable_bytes()
+            info[3:3 + S_loc] = [p[1].numel() for p in parts]
+            info[3 + S_loc:3 + 2 * S_loc] = metrics
+            info[3 + 2 * S_loc:].view(np.uint8)[:len(msg)] = np.frombuffer(msg, dtype=np.uint8)
+            info_t = torch.from_numpy(info).to(dev)
+            if self.world > 1:
+                all_info = torch.empty((self.world * info.size,), dtype=torch.int64, device=dev)
+                dist.all_gather_into_tensor(all_info, info_t, group=self.group)
+                ai = all_info.cpu().numpy().reshape(self.world, info.size)
+            else:
+                ai = info[None]
+            st, message = range_decide(ai, S_loc, nq, d, embs)
+            if st != ST_OK:
+                return st, message, None, None, None, None
+            totals = ai[:, 3:3 + S_loc]
+            maximize = int(ai[0, 3 + S_loc]) == 0   # faiss METRIC_INNER_PRODUCT
+            if self.world == 1:
+                L = torch.stack([p[0] for p in parts])
+                D = torch.cat([p[1] for p in parts])
+                P = torch.cat([p[2] for p in parts])
+                E = torch.cat([p[3] for p in parts]) if embs else None
+            else:
+                L, D, P, E = self._range_exchange(parts, totals, nq, d, embs)
+                if self.rank != 0:
+                    return st, "", None, None, None, None
+            lims, D, P, order = be.range_merge(L, D, P, maximize)
+            return st, "", lims, D, P, (E[order] if embs else None)
+        finally:
+            for ix in locked:
+                ix.index_lock.release()
+
+    def _usable_bytes(self):
+        """device memory this rank can still allocate: the driver's free memory and torch's cached blocks"""
+        if self.device.type != "cuda":
+            return 1 << 62
+        free, _ = torch.cuda.mem_get_info(self.device)
+        return free + torch.cuda.memory_reserved(self.device) - torch.cuda.memory_allocated(self.device)
+
+    def _range_exchange(self, parts, totals, nq, d, embs):
+        """The all-gather of every rank's block; on rank 0 the shard-major concatenation of all shards'
+        (lims [S, nq + 1], D, payload, rows)"""
+        dev = self.device
+        S_loc = self.S_loc
+        off_D, off_P, off_E, stride = range_layout(S_loc, nq, d, embs, int(totals.sum(axis=1).max()))
+        all_packed = torch.empty((self.world * stride,), dtype=torch.uint8, device=dev)
+        blk = all_packed[self.rank * stride:(self.rank + 1) * stride]
+        T_r = int(totals[self.rank].sum())
+        blk[:off_D].view(torch.int64).view(S_loc, nq + 1).copy_(torch.stack([p[0] for p in parts]))
+        blk[off_D:off_D + 4 * T_r].view(torch.float32).copy_(torch.cat([p[1] for p in parts]))
+        blk[off_P:off_P + 8 * T_r].view(torch.int64).copy_(torch.cat([p[2] for p in parts]))
+        if embs:
+            blk[off_E:off_E + 4 * T_r * d].view(torch.float32).view(T_r, d).copy_(torch.cat([p[3] for p in parts]))
+        dist.all_gather_into_tensor(all_packed, blk, group=self.group)
+        if self.rank != 0:
+            return None, None, None, None
+        Ls, Ds, Ps, Es = [], [], [], []
+        for r in range(self.world):
+            b = all_packed[r * stride:(r + 1) * stride]
+            n = int(totals[r].sum())
+            Ls.append(b[:off_D].view(torch.int64).view(S_loc, nq + 1))
+            Ds.append(b[off_D:off_D + 4 * n].view(torch.float32))
+            Ps.append(b[off_P:off_P + 8 * n].view(torch.int64))
+            if embs:
+                Es.append(b[off_E:off_E + 4 * n * d].view(torch.float32).view(n, d))
+        return torch.cat(Ls), torch.cat(Ds), torch.cat(Ps), (torch.cat(Es) if embs else None)
+
     # ------------------------------------------------------------ client side (plane rank 0)
+    def range_search(self, index_id: str, query, radius: float, *, int_meta: bool, return_embeddings: bool = False):
+        """`IndexClient.range_search` as one collective.  Returns host arrays (lims int64[nq + 1],
+        D float32[T], P int64[T], embs float32[T, d] | None) in merged order; P holds caller integers in
+        int_meta mode and exchange ids otherwise.  Raises RangeMetricsDiffer, MetaKindChanged or
+        PlaneError; the plane stays usable."""
+        assert self.rank == 0, "the client lives in the process of plane rank 0"
+        query = np.ascontiguousarray(query, dtype=np.float32)
+        nq, d = query.shape
+        flags = (F_EMBS if return_embeddings else 0) | (F_INT_META if int_meta else 0) | F_HAVE_QUERY
+        rbits = int(np.float64(radius).view(np.int64))
+        with self._lock, self._stream_ctx():
+            h = self._send_header([OP_RANGE, nq, 0, flags, d, rbits], index_id)
+            x_t = torch.from_numpy(query).to(self.device)
+            st, message, lims, D, P, E = self._run_range(h, index_id, x_t)
+            if st == ST_OK:
+                out = (lims.cpu().numpy(), D.cpu().numpy(), P.cpu().numpy(), E.cpu().numpy() if E is not None else None)
+        if st == ST_OK:
+            return out
+        if st == ST_RANGE_METRICS:
+            raise RangeMetricsDiffer(message)
+        if st == ST_META_KIND:
+            raise MetaKindChanged()
+        if st == ST_NOT_TRAINED:
+            raise PlaneError("Server index is not trained. (reported by the plane)")
+        if st == ST_NO_INDEX:
+            raise PlaneError("Server has no index with this id (reported by the plane)")
+        if st == ST_RANGE_LIMIT:
+            raise PlaneError(message)
+        raise PlaneError("range search failed on the plane" + (f": {message}" if message else " (see the ranks' logs)"))
+
     def search(self, index_id: str, query, k: int, *, maximize: bool, return_embeddings: bool = False,
                int_meta: bool = False, filter_pos: int = -1, filter_value=None, k_out: Optional[int] = None):
         """Returns host arrays (D [nq,kk] f32, I [nq,kk] i64, count [nq] i32 | None,
@@ -704,6 +945,14 @@ class SearchPlane:
 
 class MetaKindChanged(PlaneError):
     """a shard's metadata stopped being all-integer since the client last asked"""
+
+
+class RangeMetricsDiffer(PlaneError):
+    """the shards of a range search report different search metrics (`metrics`, sorted)"""
+
+    def __init__(self, metrics):
+        super().__init__(f"search metrics {metrics}")
+        self.metrics = metrics
 
 
 def init_process_group_from_env(backend: Optional[str] = None):

@@ -236,6 +236,22 @@ int dfx_merge_packed_dev(int64_t R, int64_t S_loc, int64_t nq, int64_t k, const 
                          int64_t rank_stride_bytes, int64_t off_I_bytes, int negate,
                          float *d_outD, int64_t *d_outI, void *stream);
 
+/* the cross-shard merge of range search results (IndexClient.range_search over the search plane).
+ * Input: S shards' results of the same nq queries, concatenated shard-major: d_lims int64[S][nq + 1]
+ * (each shard's own offsets, lims[s][0] = 0), d_D float32[total] and one int64 payload per entry d_P
+ * [total] (ids or metadata codes; carried, never read), total = the sum of lims[s][nq].  Shard s's query q
+ * holds entries base_s + lims[s][q] .. base_s + lims[s][q + 1] - 1, base_s = the totals of the shards
+ * before s, and each such run must be sorted best first, as dfx_range_fetch returns it.
+ * Output: d_out_lims int64[nq + 1], d_outD / d_outP [total] and d_order int64[total] (the input entry of
+ * each output slot, to move embeddings or metadata the same way).  The order is that of a stable sort of
+ * the concatenation by (query, score): per query best first -- maximize == 0: ascending (L2), != 0:
+ * descending (inner product) --, equal scores by shard, then by the shard's own order.  Scores compare as
+ * floats (-0 == +0) and are never negated; NaN must not occur (no NaN passes a radius).  Deterministic, no
+ * atomics, graph-capturable (no read-back). */
+int dfx_range_merge_dev(int64_t S, int64_t nq, const int64_t *d_lims, const float *d_D, const int64_t *d_P,
+                        int64_t total, int maximize, int64_t *d_out_lims, float *d_outD, int64_t *d_outP,
+                        int64_t *d_order, void *stream);
+
 /* shard-local ids -> exchange ids: out = ids < 0 ? -1 : (shard_tag << 40) | ids, so that the
  * client can tell which (shard, local id) won after the merge (the reference's synthetic
  * positions, client.py:288).  d_col (optional): one int32 code per local id for ONE metadata
